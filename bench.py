@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py - frames/sec of RefVSR 4x SR (LR 270x480 -> 1080x1920) through refvsr_b200 on N B200s.
+"""bench.py - frames/sec of RefVSR 4x SR (LR 270x480 -> 1080x1920) through refvsr_b200 on N H100s.
 
     python bench.py --gpus 1 --steps 20 --warmup 3                # our arm (CUDA path)
+    python bench.py --gpus 1 --steps 20 --dump-outputs DIR         # + what the last timed step returned, as DIR/<name>.npy
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
     python bench.py --impl reference --steps K --warmup W          # reference algorithm on host cores
 
@@ -41,7 +42,8 @@ def measured_peaks():
         d = json.load(open(p))
         return dict(hbm=d['hbm_gbs'], tensor_burst=d['bf16_tflops'], tensor_sustained=d['bf16_tflops_sustained'],
                     source='measured (MEASURED_PEAKS.json)')
-    return dict(hbm=6650.0, tensor_burst=1590.0, tensor_sustained=1400.0, source='fallback (B200_PROFILING.md)')
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s - a bound, not a measured rate
+    return dict(hbm=3350.0, tensor_burst=989.0, tensor_sustained=989.0, source='H100 SXM data sheet (not measured)')
 
 
 class ClockSampler(threading.Thread):
@@ -111,34 +113,6 @@ def make_model(workload, precision, device, graphs=True, fuse=False):
     return cfg, net.to(device)
 
 
-def ncu_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the roofline kernel, from the committed
-    newest committed `ncu --set full` capture (profiles/r02_ncu_conv_lr.json, else round 1's); None when absent."""
-    for name in ('r02_ncu_conv_lr.json', 'r01_ncu_conv_lr.json'):
-        try:
-            with open(os.path.join(ROOT, 'profiles', name)) as f:
-                return float(json.load(f)['traffic'])
-        except Exception:
-            continue
-    return None
-
-
-def attach_ncu_traffic(entries):
-    """per-launch DRAM traffic (dram__bytes_read + write) of the same kernels from the committed `ncu --set full` captures
-    (profiles/r02_ncu_kernels.json, written by tools/summarize_r02.py); None where no capture exists"""
-    try:
-        with open(os.path.join(ROOT, 'profiles', 'r02_ncu_kernels.json')) as f:
-            ncu = json.load(f)
-    except Exception:
-        ncu = {}
-    key = {'warp_up': 'warp_vec', 'warp3': 'warp3', 'gather_aa1': 'gather_cells', 'aligned_sample': 'aligned_sample2',
-           'reconstruct': 'reconstruct4', 'match_argmax': 'match_tc', 'conv3x3_lr_chain': 'conv_chain', 'conv3x3_lr_trunk': 'conv_tc'}
-    for k, v in entries.items():
-        cap = ncu.get(key.get(k, ''), None)
-        v['traffic'] = (cap['traffic'] / (60.0 if k == 'conv3x3_lr_chain' else 1.0)) if cap else None
-    return entries
-
-
 def host_threads():
     """threads for the CPU legs: all cores up to 16 - beyond that the oracle's many small ATen ops lose to
     oversubscription (measured on the 128-core GPU host: 128 threads were >10x slower than 8)."""
@@ -164,7 +138,7 @@ def kernel_rooflines(net, peaks):
     dev = 'cuda'
     out = {}
     e = 2 if dt != torch.float32 else 4
-    nrot = max(2, int(160e6 // (H * W * C * e)) + 1)          # rotate through ~160 MB > 126 MB L2
+    nrot = max(2, int(160e6 // (H * W * C * e)) + 1)          # rotate through ~160 MB > 50 MB L2
 
     def timeit(fn, iters=30, warm=5):
         # the `iters` launches are captured into one CUDA graph so the number is device time per launch, not the
@@ -209,7 +183,7 @@ def kernel_rooflines(net, peaks):
     out['conv3x3_lr_trunk'] = dict(bound='tensor', achieved=flops / ttr / 1e12, peak=peaks['tensor_burst'], unit='TFLOP/s',
                                    frac=flops / ttr / 1e12 / peaks['tensor_burst'], seconds=ttr, algorithmic_flops=flops,
                                    note='per conv of a 60-launch dependent chain on L2-resident maps (the propagation trunk); '
-                                        '~6.0 us of it is launch / prologue / hand-off skeleton, profiles/r02_trunk_knockout.md')
+                                        'includes each launch\'s prologue and hand-off')
     del pa, pt, pb
     # fused residual block (rv_resblock): conv3x3 -> ReLU -> conv3x3 -> + x in one launch
     if net.Network.fuse_resblocks and dt != torch.float32:
@@ -253,7 +227,7 @@ def kernel_rooflines(net, peaks):
         tch = timeit(lambda i: ops.conv_chain(cb, layers, flags), iters=10, warm=2) / (2 * nblk)
         out['conv3x3_lr_chain'] = dict(bound='tensor', achieved=flops / tch / 1e12, peak=peaks['tensor_burst'], unit='TFLOP/s',
                                        frac=flops / tch / 1e12 / peaks['tensor_burst'], seconds=tch, algorithmic_flops=flops,
-                                       note='per layer of a 60-layer rv_conv_chain launch (opt-in: slower than per-layer launches, profiles/r02_conv_chain.md)')
+                                       note='per layer of a 60-layer rv_conv_chain call (opt-in)')
     # K3 / K4 / K7: the remaining HBM kernels of the north_star's >= 60 % list
     idx = torch.randint(0, (H // 2) * (W // 2), (H * W,), device=dev, dtype=torch.int32)
     vd = [torch.randn((H // 2, W // 2, C), device=dev).to(dt) for _ in range(nrot)]
@@ -376,7 +350,7 @@ def cpu_baseline_sample(workload, threads=None):
 
 
 def eager_b200(workload, dev, windows=3):
-    """SURVEY 8(d) last bullet / VERDICT r1 item 6b: the reference's own modules in eager PyTorch on THIS B200 - the practical
+    """SURVEY 8(d) last bullet / VERDICT r1 item 6b: the reference's own modules in eager PyTorch on THIS GPU - the practical
     number to beat (the reference has no Blackwell kernels of its own; this is cuDNN / cuBLAS through ATen).  One first
     window (untimed: cuDNN heuristics, allocator growth), then `windows` steady windows timed with CUDA events, for fp32
     (TF32 off: the reference's default numerics) and for autocast in this workload's 16-bit type."""
@@ -486,6 +460,32 @@ def clip_leg(args, net, dev, world, rank, wl):
             'note': 'time to the last frame of ONE clip incl. the T//2-frame input-halo exchange and the forward-state hand-offs '
                     '(62 MB per rank boundary inside a reset segment); the forward chain is serial inside each 9-frame segment '
                     '(1 of 5 propagation steps per frame), backward branches / per-frame products / upsampling tails are local'}
+
+
+DUMP_LIMIT = 64 << 20        # bytes of .npy payload per --dump-outputs directory
+
+
+def dump_outputs(d, out):
+    """The tensors of SRNet.forward's result dict (the timed path's last step) as float32 DIR/<key>.npy.  Inputs and weights are
+    seeded, so two builds run with the same arguments can be compared output for output.  An array that would push the total
+    past DUMP_LIMIT is replaced by a fixed, seeded sample of its elements (DIR/<key>.sample_idx.npy holds the flat indices)."""
+    import numpy as np
+    import torch
+    os.makedirs(d, exist_ok=True)
+    used = 0
+    for k in sorted(out):
+        v = out[k]
+        if not torch.is_tensor(v):
+            continue
+        a = v.detach().float().cpu().numpy()
+        if used + a.nbytes > DUMP_LIMIT:
+            n = max(1, min(a.size, (DUMP_LIMIT - used) // 12))      # 4 bytes of value + 8 of index per sampled element
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=n, replace=False))
+            np.save(os.path.join(d, f'{k}.sample_idx.npy'), idx)
+            a = a.reshape(-1)[idx]
+            used += idx.nbytes
+        np.save(os.path.join(d, f'{k}.npy'), a)
+        used += a.nbytes
 
 
 def run_ours(args):
@@ -630,10 +630,11 @@ def run_ours(args):
         n0 = net.Network.executed_kernels
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-        fn(Wm, Wm + K)
+        ret = fn(Wm, Wm + K)
         e1.record()
         barrier()
         clocks = sampler.stop()
+        timed.last = ret
         ms = torch.tensor([e0.elapsed_time(e1)], device=dev)
         if world > 1:
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
@@ -644,13 +645,15 @@ def run_ours(args):
     net.Network.reset_state()
     run_resident(0, Wm + K)
     ms_res, launches, clocks = timed(run_resident)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, timed.last)
     ms_e2e, _, clocks_e2e = timed(run_e2e)
     bad = {'hw_slowdown', 'hw_thermal_slowdown', 'sw_thermal_slowdown'}
     if bad & set(clocks['reasons']):                          # re-measure once (timing rules)
         ms_res, launches, clocks = timed(run_resident)
 
-    # sustained leg (N = 1): >= 5 s of consecutive windows of one long stream, with its own clock record - MEASURED_PEAKS shows
-    # this GPU settling well below its 1965 MHz boost under seconds-long dense load, which a 0.2 s timed region never sees
+    # sustained leg (N = 1): >= 5 s of consecutive windows of one long stream, with its own clock record -
+    # a power-capped GPU can settle below its boost clock under seconds-long dense load, which a 0.2 s timed region never sees
     sustained = None
     if world == 1 and not args.no_sustained:
         n_sus = int(math.ceil(args.sustained_s * 1e3 / (ms_res / K) * 1.15)) + Wm
@@ -704,7 +707,7 @@ def run_ours(args):
                                       f'charged in full to the {K} timed steps; no collective inside the forward',
                        'halo_exchange_ms': halo_ms,
                        'reuse_check': net.Network.reuse_check,
-                       'l2': 'working set per step (~1.5 GB of activations) >> 126 MB L2; no explicit flush',
+                       'l2': 'working set per step (~1.5 GB of activations) >> 50 MB L2; no explicit flush',
                        'match_mode': net.Network.match_mode},
             'e2e': {'value': fps_e2e, 'unit': 'frames/s', 'h2d_bytes_per_step': h2d,
                     'd2h_bytes_per_step': 3 * 16 * H * W * 4, 'ms_per_step': ms_e2e / K,
@@ -714,8 +717,8 @@ def run_ours(args):
                                  'kernel nodes replayed by the per-window CUDA graphs)',
             'clocks': clocks, 'clocks_e2e': clocks_e2e,
             'roofline': dict(roof['conv3x3_lr'], kernel='conv_tc_kernel 3x3 C->C @270x480 (+ReLU+residual)',
-                             peak_source=peaks['source'], traffic=ncu_traffic()),
-            'roofline_other': attach_ncu_traffic({k: v for k, v in roof.items() if k != 'conv3x3_lr'}),
+                             peak_source=peaks['source']),
+            'roofline_other': {k: v for k, v in roof.items() if k != 'conv3x3_lr'},
         }
         if sustained is not None:
             line['sustained'] = sustained
@@ -797,7 +800,11 @@ def main():
     ap.add_argument('--sustained-s', type=float, default=5.0)
     ap.add_argument('--no-graphs', action='store_true', help='eager kernel launches (for ncu launch lists)')
     ap.add_argument('--fuse', action='store_true', help='use the fused residual-block kernel (rv_resblock)')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write what SRNet.forward returned in the last timed step as DIR/<name>.npy (float32)')
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == 'reference':
+        ap.error('--dump-outputs writes what the CUDA path returned; it does not apply to --impl reference')
     args.warmup = max(args.warmup, 3) if args.impl == 'ours' else args.warmup
     if args.impl == 'reference':
         run_reference(args)

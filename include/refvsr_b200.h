@@ -1,5 +1,5 @@
 /*
- * refvsr_b200 — C ABI of the B200 (sm_100a) kernels behind RefVSR's per-frame forward hot path.
+ * refvsr_b200 — C ABI of the H100 (sm_90a) kernels behind RefVSR's per-frame forward hot path.
  *
  * The reference (codeslake/RefVSR) is pure Python: it has no FFI of its own.  Its boundary for this
  * path is the nn.Module contract `SRNet.forward(x, ref, is_first_frame, is_log, is_train)`
@@ -44,7 +44,7 @@ extern "C" {
 #define RV_ACT_CLAMP3 4   /* clamp(-3, 3): affine map of AlignedConv2d (alignment.py:56)            */
 
 #define RV_CONV_IMPL_SIMT 0 /* fp32-accumulate CUDA-core implicit GEMM (any geometry, any dtype)    */
-#define RV_CONV_IMPL_TC 1   /* tcgen05/TMEM implicit GEMM fed by TMA (f16/bf16, stride 1)           */
+#define RV_CONV_IMPL_TC 1   /* wgmma implicit GEMM fed by TMA (f16/bf16, stride 1)                 */
 
 const char* rv_last_error(void);
 int rv_version(void);
@@ -100,17 +100,17 @@ int rv_conv2d(const rv_conv_desc* d, void* stream);
  * per SM.  Returns the previous value.  The engine's own scheduling knob, no counterpart in the reference: the forward-branch
  * step of a window (RefVSR.py:248-277) is independent of its backward branch (RefVSR.py:211-238), so network.py enqueues the two on
  * different streams with half the SMs each - two capped launches overlap each other's prologue / first-box latency / last-tile tail,
- * which a single dependent chain of launches exposes once per layer (profiles/r02_trunk_knockout.md). */
+ * which a single dependent chain of launches exposes once per layer. */
 int rv_set_conv_cta_cap(int cap);
 
 /* Host-only: the launch plan rv_conv2d's tensor-core path would use on a device with `max_smem_optin` bytes of opt-in shared memory
- * per block and `num_sms` SMs -> out8 = {mode, smem slots, stages per barrier group, stages per tile, MMA-issuing warps, TMEM
- * accumulators, nb, dynamic smem bytes}.  No CUDA call is made (pointers in `d` are only tested for null / alignment).  Lets the
+ * per block and `num_sms` SMs -> out8 = {mode, smem slots per consumer, weights resident, stages per tile, consumer
+ * warpgroups, accumulator sets, nb, dynamic smem bytes}.  No CUDA call is made (pointers in `d` are only tested for null / alignment).  Lets the
  * ring invariants (every issuing warp owns its slots and accumulators) be checked without a GPU. */
 int rv_conv2d_tc_plan(const rv_conv_desc* d, int max_smem_optin, int num_sms, int32_t* out8);
 
 /* ------------------------------------------------------------------------------------------------
- * rv_resblock - fused residual block  out = act_post( x + conv2( act_mid( conv1(x) ) ) ), 3x3 / stride 1 / pad 1,
+ * rv_resblock - residual block  out = act_post( x + conv2( act_mid( conv1(x) ) ) ), 3x3 / stride 1 / pad 1,
  * C -> C -> C channels (C <= 64), f16/bf16 NHWC.  One launch instead of two rv_conv2d calls for
  * ResidualBlockNoBN (mmedit/models/common/sr_backbone_utils.py:85-97, act_mid = ReLU) and ResBlock
  * (models/archs/RefVSR_/common.py:33-39, act_mid = LeakyReLU(0.2); act_post = LeakyReLU(0.2) inside
@@ -134,14 +134,15 @@ int rv_resblock(const rv_resblock_desc* d, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * rv_conv_chain - a CHAIN of 3x3 C->C convolutions (+ bias, activation, residual, activation) over a small set of NHWC
- * f16/bf16 buffers of identical geometry, executed by ONE persistent tcgen05 launch with per-tile dependencies between
- * layers and a TMA-store epilogue (refvsr_b200/csrc/conv_chain.cu).  Replaces, launch for launch,
+ * f16/bf16 buffers of identical geometry, executed by ONE persistent wgmma launch with per-tile dependencies between
+ * layers (refvsr_b200/csrc/conv_chain.cu).  Covers
  *   make_layer(ResidualBlockNoBN, num_blocks)  (mmedit/models/common/sr_backbone_utils.py:26-39,85-97; RefVSR.py:346-349)
  *   ResList: N x ResBlock + conv_tail + skip    (RefVSR_/common.py:25-39,64-82; RefVSR.py:48-60,233-234)
  * Layer l computes  buf[dst] = act_post( act_pre( conv3x3(buf[src]) + bias ) + buf[res] )   (res < 0: no residual), zero
  * padding 1.  dst must differ from src.  wpack = the layout-1 tensor-core weight image of rv_conv2d ([9 taps][nb][64]
  * 16-bit, SWIZZLE_128B byte image), bias = nb floats (zero beyond cout).  All buffers: (H, W, C), C % 8 == 0, C <= 48.
- * `flags` is device scratch of >= ceil(H/16) * ceil(W/8) int32 (zeroed by the call, on `stream`).
+ * `flags` is device scratch of >= ceil(H/16) * ceil(W/8) int32, zeroed by the call on `stream`; flags[t] counts the layers tile t
+ * has completed (all = nlayers at the end).
  * Results are bit-identical to the same layers issued one by one through rv_conv2d.
  * ------------------------------------------------------------------------------------------------ */
 #define RV_CHAIN_MAX_LAYERS 64
@@ -161,7 +162,7 @@ typedef struct {
   int32_t nlayers;
   int32_t* flags;
   int32_t max_ctas; /* 0: one persistent CTA per SM.  > 0: cap (leave SMs free for kernels of OTHER streams that must stay
-                       co-resident, e.g. NCCL point-to-point kernels: the chain's CTAs spin on each other's flags and all
+                       co-resident, e.g. NCCL point-to-point kernels: the chain's CTAs wait on each other's flags and all
                        of them have to be resident) */
 } rv_conv_chain_desc;
 int rv_conv_chain(const rv_conv_chain_desc* d, void* stream);
@@ -169,7 +170,7 @@ int rv_conv_chain(const rv_conv_chain_desc* d, void* stream);
 /* space-to-depth by 2: out[(Y,X)][(ry*2+rx)*C + c] = src[(2Y+ry, 2X+rx)][c].  Turns the two stride-2
  * convolutions of the path (ref_encoder2.0.0, RefVSR.py:45; aa2.align.p_conv.0, alignment.py:21) into
  * stride-1 3x3 convolutions over 4C channels (weights re-indexed by packing.s2d_weights), so they run on
- * the tcgen05 kernel.  H, W even; C*elemsize a multiple of 16. */
+ * the tensor-core kernel.  H, W even; C*elemsize a multiple of 16. */
 int rv_space_to_depth2(const void* src, int H, int W, int C, int dtype, void* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
@@ -236,7 +237,7 @@ int rv_patch_pack(const void* feat, int H, int W, int C, int dtype, int mode, vo
                   int kpad, void* stream);
 /* conf[l] = max_r <A[l], B[r]>,  idx[l] = argmax_r (lowest r wins ties)  (attention.py:91).
  * A (P,kpad) fp16, B (R,kpad) fp16, outputs conf (P) fp32, idx (P) int32.
- * impl: 0 = CUDA-core fp32 reference kernel, 1 = tcgen05 (TMA-fed, TMEM accumulators). */
+ * impl: 0 = CUDA-core fp32 reference kernel, 1 = wgmma (TMA-fed, register accumulators). */
 int rv_match_argmax(const void* A, int P, const void* B, int R, int kpad, float out_scale,
                     float* conf, int32_t* idx, int impl, void* stream);
 

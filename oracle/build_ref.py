@@ -5,7 +5,7 @@ The reference is pure Python with no setup.py / pyproject (SURVEY.md section 1),
 this repository's history) but NOT gpurun-ignored, so the staged tree travels to the GPU box, where /root/reference does
 not exist.  Consumers (test infrastructure and bench legs only - never the product):
   * bench.py --impl reference        the reference's own CPU forward on the box's host cores (kind "reference")
-  * bench.py eager_b200 leg          the same unmodified modules in eager PyTorch on the B200
+  * bench.py eager_b200 leg          the same unmodified modules in eager PyTorch on the GPU
   * tests/test_dropin_runpy.py       run.py / eval.py / Trainer.evaluation with and without the drop-in
 Missing third-party packages (mmcv, easydict, termcolor, ...) come from oracle/shims and tests/runpy_env.
 

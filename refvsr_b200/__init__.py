@@ -1,4 +1,4 @@
-"""refvsr_b200 - B200-native (sm_100a) implementation of RefVSR's per-frame forward hot path.
+"""refvsr_b200 - H100-native (sm_90a) implementation of RefVSR's per-frame forward hot path.
 
 Public surface (mirrors the reference's module contract, SURVEY.md 8b):
     SRNet(config).forward(x, ref, is_first_frame=True, is_log=False, is_train=False) -> OrderedDict

@@ -1,4 +1,4 @@
-// Shared helpers for the refvsr_b200 kernels (sm_100a only).
+// Shared helpers for the refvsr_b200 kernels (sm_90a).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>

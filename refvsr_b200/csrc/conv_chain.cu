@@ -1,40 +1,21 @@
-// rv_conv_chain: a whole CHAIN of 3x3 C->C convolutions (the 60-conv trunk of ResidualBlocksWithInputConv, the ResList
-// decoders) in ONE persistent tcgen05 launch, with tile-level instead of grid-level dependencies between layers.
+// rv_conv_chain: a whole CHAIN of 3x3 C->C convolutions (the trunk of ResidualBlocksWithInputConv, the ResList decoders) in
+// ONE persistent wgmma launch, with tile-level instead of grid-level dependencies between layers.
 //
-// Why (profiles/r01_conv_timeline.md): a trunk conv launch spends ~3.6 of its ~12 us outside the MMA-bound middle
-// (prologue + dependency wait, first box latency, last-tile drain), 305 times per window.  Here the CTAs stay resident and
-// walk the layers themselves:
 //   * tile t of layer l+1 may start as soon as the <= 9 tiles around t have finished layer l.  Every tile has ONE monotone
 //     counter in global memory, flags[t] = number of layers completed.  Tiles keep their CTA across layers
 //     (t = cta + k * grid), and each CTA walks (layer, k) in lexicographic order, so the wait graph is acyclic (a CTA
 //     blocked on layer l+1 never holds back a layer-l tile) as long as all CTAs are co-resident: grid <= #SMs, 1 CTA / SM.
 //   * the same condition covers every hazard of ANY layer list over a small set of ping-pong buffers: a layer's source was
 //     last written at some layer <= l-1 (RAW: neighbours' flags >= l), and its destination was last read WITH A HALO by the
-//     neighbours' tiles of some layer <= l-1 (WAR: same flags).  Residual reads have no halo and belong to the tile itself.
-//   * EPILOGUE = TMA STORE: the epilogue group converts its accumulator to the 16-bit storage type, writes the tile into a
-//     128B-swizzled staging buffer and one elected thread issues cp.async.bulk.tensor (global <- shared).  Image borders and
-//     the channel padding (C < 64) are clipped by the tensor map; no per-thread addressing, no 96-byte-stride STG.
-//     That thread later observes completion (cp.async.bulk.wait_group), and publishes flags[t] = l + 1 with a release store.
-//     Publication is deferred to the group's next tile so the store latency is off the critical path - but a group never
-//     blocks on an accumulator while it holds an unpublished flag (bounded try-wait first), which keeps the protocol
-//     deadlock-free for any tile count.
-//   * all global traffic of a layer goes through L2: TMA loads / stores and ld.global.cg residual reads (never the
-//     non-coherent path: the data was written by other SMs during this same launch).
-//   * weights of the next layer replace the current ones as soon as the last MMA of the layer has retired (mbarrier fed by
-//     tcgen05.commit of every issuing warp); up to slots-1 boxes of the next layer are prefetched before that.
-// MEASURED OUTCOME (round 2, B200; profiles/r02_conv_chain.md): bit-identical to the per-layer path at every size, but SLOWER -
-// 20-22 us per 270x480 layer against 9.8 us for one conv_tc launch, 55 vs 32 us at 540x960.  The device timeline shows why:
-// a cross-CTA dependency hop (epilogue -> store complete -> release -> poll -> acquire -> TMA load) costs ~15k cycles on this
-// two-die part (GPU-scope fences 2-4k cycles each), while a CTA has only 7 tiles = ~10k cycles of MMA work per layer to hide
-// it behind, and the neighbourhood of tile k reaches tile k+1 of the previous layer.  The ~3.6 us a launch boundary costs is
-// cheaper than per-tile GPU-scope synchronisation.  The kernel therefore ships OPT-IN (config.b200_conv_chain = True).
-// Geometry = conv_tc.cu MODE 1 (validated in round 1): tile 16 rows x 8 columns = 128 TMEM lanes, ONE 18 x 10 pixel box
-// per tile (64-channel rows, SWIZZLE_128B, out-of-bounds zero fill = conv padding), the 9 taps are row-shifted UMMA
-// descriptor views of it; 512 threads = TMA producer warp, 3 MMA-issuing warps, 3 epilogue groups of 4 warps.
-// Arithmetic (tap order, K slices, fp32 epilogue: bias, act, + residual, act, round) is identical to conv_tc.cu, so a chain
-// is BIT-IDENTICAL to the same layers launched one by one (tests/test_gpu_kernels.py::test_conv_chain_*).
+//     neighbours' tiles of some layer <= l-1 (WAR: same flags).  Residual reads have no halo and belong to the tile itself,
+//     i.e. to this CTA.
+//   * publication: every thread's stores, __threadfence, CTA barrier, then one release store of flags[t] = l + 1.  The
+//     waiting side polls with acquire loads and issues fence.proxy.async before its TMA load reads the data.
+// Geometry = conv_tc.cu MODE 1: tile 16 rows x 8 columns, ONE 18 x 10 pixel box per tile (64-channel rows, SWIZZLE_128B,
+// out-of-bounds zero fill = conv padding), the 9 taps are row-shifted wgmma descriptor views of it; one warpgroup per CTA.
+// The MMA sequence (tap order, K slices, N = NB) and the fp32 epilogue (bias, act, + residual, act, round) are those of
+// conv_tc.cu, so a chain is BIT-IDENTICAL to the same layers launched one by one (tests/test_gpu_kernels.py::test_conv_chain_*).
 #include <algorithm>
-#include <cstdlib>
 
 #include "common.cuh"
 #include "tc_common.cuh"
@@ -43,433 +24,143 @@ namespace rv {
 namespace {
 
 constexpr int CH_MAXL = RV_CHAIN_MAX_LAYERS, CH_MAXB = RV_CHAIN_MAX_BUFFERS;
-constexpr int CH_NACC = 6, CH_NGRP = 3, CH_NMMA = 3, CH_MAXSLOTS = 8;
 constexpr int CH_TH = 16, CH_TW = 8, CH_BW = CH_TW + 2, CH_BH = CH_TH + 2;
 constexpr uint32_t CH_A_TX = CH_BH * CH_BW * 128;              // bytes one activation box delivers (23 040)
-constexpr uint32_t CH_A_BYTES = (CH_A_TX + 1023u) & ~1023u;    // slot pitch (1024-byte swizzle atoms)
-constexpr uint32_t CH_STG_BYTES = 128 * 128;                   // staging tile of one epilogue group: 128 pixels x 128 B
+constexpr uint32_t CH_A_BYTES = (CH_A_TX + 1023u) & ~1023u;    // 1024-byte swizzle atoms
 
 struct ChLayer {
   const uint8_t* wpack;   // layout-1 weight image [9 taps][NB][64], SWIZZLE_128B byte image (packing.pack_tc)
   const float* bias;
   float pre_slope, post_slope;   // act(v) = max(v, v * slope): 1 none, 0 ReLU, 0.1 / 0.2 LeakyReLU
   int src, res, dst;             // buffer indices; res < 0: no residual
-  int res_need;                  // flags[tile] >= res_need  =>  the residual tile has been written (0: external input)
 };
 
 struct ChP {
-  int H, W, C, NB, tiles_x, ntiles, nlayers, slots, nmma, fmt, ksteps;
+  int H, W, C, NB, tiles_x, tiles_y, nlayers, ksteps;
   uint32_t w_bytes;
   int* flags;
-  long long* trace;         // REFVSR_CHAIN_TRACE=<device ptr>: clock64 timeline of CTA `trace_cta` ([7 roles][2048][3])
-  int trace_cta;
-  const void* buf[CH_MAXB];
+  void* buf[CH_MAXB];
   ChLayer layer[CH_MAXL];
 };
 
 struct ChMaps {
   CUtensorMap ld[CH_MAXB];   // box 64 ch x 10 x 18 (tile + halo)
-  CUtensorMap st[CH_MAXB];   // box 64 ch x 8 x 16  (tile)
 };
 
-// ---- bounded waits: a protocol bug must abort the launch (sticky error), never hang the GPU --------------------------
-__device__ __forceinline__ void mbar_wait_wd(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .u32 c;\n\t"
-      "mov.u32 c, 0;\n\t"
-      "CH_WAIT:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra CH_DONE;\n\t"
-      "add.u32 c, c, 1;\n\t"
-      "setp.lt.u32 p, c, 0x1000000;\n\t"
-      "@p bra CH_WAIT;\n\t"
-      "trap;\n\t"
-      "CH_DONE:\n\t}" ::"r"(tc::smem_u32(bar)),
-      "r"(parity)
-      : "memory");
-}
-// coherent at GPU scope, but WITHOUT the L1 invalidation an acquire load carries (CCTL.IVALL per poll iteration evicted the
-// epilogue's read-only data and cost an L2 round trip per tile - profiles/r02_conv_chain.md)
-__device__ __forceinline__ int ld_relaxed(const int* p) {
+__device__ __forceinline__ int ld_acquire(const int* p) {
   int v;
-  asm volatile("ld.relaxed.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
   return v;
 }
-__device__ __forceinline__ uint4 ld_cg16(const void* p) {
-  uint4 v;
-  asm volatile("ld.global.cg.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void group_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, const void* smem, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.tile.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
-                   reinterpret_cast<uint64_t>(m)),
-               "r"(tc::smem_u32(smem)), "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
-  asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-}
-// the calling thread's bulk stores have completed and are visible; then flags[tile] = val is released at GPU scope
-__device__ __forceinline__ void publish(int* flag, int val) {
-  asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-  asm volatile("fence.proxy.async;" ::: "memory");
-  asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(flag), "r"(val) : "memory");
-}
-// same, when exactly one newer bulk store (just issued) may still be in flight
-__device__ __forceinline__ void publish_prev(int* flag, int val) {
-  asm volatile("cp.async.bulk.wait_group 1;" ::: "memory");
-  asm volatile("fence.proxy.async;" ::: "memory");
-  asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(flag), "r"(val) : "memory");
-}
-
-__device__ __forceinline__ uint32_t pack2h(float a, float b, __half) {
-  __half2 h = __floats2half2_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
-__device__ __forceinline__ uint32_t pack2h(float a, float b, __nv_bfloat16) {
-  __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
-__device__ __forceinline__ float2 unpack2h(uint32_t v, __half) { return __half22float2(*reinterpret_cast<__half2*>(&v)); }
-__device__ __forceinline__ float2 unpack2h(uint32_t v, __nv_bfloat16) {
-  return make_float2(__uint_as_float(v << 16), __uint_as_float(v & 0xffff0000u));
-}
-
-// device timeline (tools/chain_trace.py): role r appends (event, n, clock64) triples; one uniform branch when disabled
-#define CH_TRACE(role, ev, nn)                                                                         \
-  do {                                                                                                 \
-    if (p.trace != nullptr && (int)blockIdx.x == p.trace_cta && (threadIdx.x & 31) == 0 && tr_n < 2048) { \
-      long long* _t = p.trace + ((size_t)(role) * 2048 + tr_n) * 3;                                   \
-      _t[0] = (ev); _t[1] = (long long)(nn); _t[2] = clock64(); ++tr_n;                                \
-    }                                                                                                  \
-  } while (0)
-
-template <typename T>
-__global__ void __launch_bounds__(32 * (1 + CH_NMMA) + 128 * CH_NGRP, 1)
-conv_chain_kernel(const __grid_constant__ ChMaps maps, const __grid_constant__ ChP p) {
+template <typename T, int NB>   // NB: rows of the weight image (= p.NB)
+__global__ void __launch_bounds__(128, 1) conv_chain_kernel(const __grid_constant__ ChMaps maps, const __grid_constant__ ChP p) {
+  constexpr bool BF = std::is_same<T, __nv_bfloat16>::value;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ uint64_t bar_full[CH_MAXSLOTS], bar_empty[CH_MAXSLOTS], bar_w, bar_wfree, bar_tfull[CH_NACC], bar_tempty[CH_NACC];
-  __shared__ uint32_t tmem_base_s;
-  __shared__ __align__(16) float bias_s[4][64];     // bias of layer l in slot l & 3 (arrives with the weights, on bar_w)
-
+  __shared__ uint64_t bar_w, bar_in;
+  __shared__ float bias_s[48];
   const uint32_t raw = tc::smem_u32(smem_raw);
-  uint8_t* smemA = smem_raw + (((raw + 1023u) & ~1023u) - raw);
-  uint8_t* smemW = smemA + (size_t)p.slots * CH_A_BYTES;
-  uint8_t* smemS = smemW + p.w_bytes;          // w_bytes = 9 * NB * 128 is a multiple of 1024 for NB % 16 == 0
+  uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
+  uint8_t* smIn = smem;
+  uint8_t* smW = smem + CH_A_BYTES;
+  const int t = threadIdx.x, wq = t >> 5, lane = t & 31;
+  const uint32_t in_a = tc::smem_u32(smIn), w_a = tc::smem_u32(smW);
+  const int ntiles = p.tiles_x * p.tiles_y;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int warp_u = __shfl_sync(0xffffffffu, warp, 0);
-  const int G = gridDim.x;
-  const int ntl = (p.ntiles - (int)blockIdx.x + G - 1) / G;      // local tiles per layer: cta, cta + G, ...
-  const uint32_t total = (uint32_t)p.nlayers * (uint32_t)ntl;    // local (layer, tile) sequence n = l * ntl + k
-  int tr_n = 0;
-  (void)tr_n;
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < p.slots; ++i) {
-      tc::mbar_init(&bar_full[i], 1);
-      tc::mbar_init(&bar_empty[i], 1);
-    }
+  if (t == 0) {
     tc::mbar_init(&bar_w, 1);
-    tc::mbar_init(&bar_wfree, (uint32_t)p.nmma);
-    for (int i = 0; i < CH_NACC; ++i) {
-      tc::mbar_init(&bar_tfull[i], 1);
-      tc::mbar_init(&bar_tempty[i], 4);
-    }
+    tc::mbar_init(&bar_in, 1);
     tc::fence_barrier_init();
   }
-  if (warp == 1 + CH_NMMA) tc::tmem_alloc(&tmem_base_s, 512);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem_base = tmem_base_s;
-
-  if (warp_u < 1 + CH_NMMA) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
-  else asm volatile("setmaxnreg.inc.sync.aligned.u32 152;" ::: "memory");
-
-  if (warp_u == 0) {
-    // ============================ TMA producer ============================
-    uint32_t n = 0;
-    for (int l = 0; l < p.nlayers; ++l) {
-      const int src = p.layer[l].src;
-      const int kws = (l == 0) ? 0 : min(p.slots - 1, ntl - 1);      // boxes of layer l prefetched before its weights
-      int tile = blockIdx.x;
-      uint32_t known = 0;     // bit j: the dependencies of local tile k + j are known to be satisfied
-      for (int k = 0; k < ntl; ++k, ++n, tile += G) {
-        CH_TRACE(0, 0, n);
-        if (k == kws) {
-          if (l > 0) mbar_wait_wd(&bar_wfree, (uint32_t)(l - 1) & 1u);       // every MMA of layer l-1 has retired
-          if (tc::elect_one()) {
-            tc::mbar_expect_tx(&bar_w, p.w_bytes + (uint32_t)p.NB * 4u);
-            tc::bulk_load(p.layer[l].wpack, &bar_w, smemW, p.w_bytes);
-            tc::bulk_load(p.layer[l].bias, &bar_w, &bias_s[l & 3][0], (uint32_t)p.NB * 4u);
+  uint32_t ph_in = 0;
+  for (int l = 0; l < p.nlayers; ++l) {
+    const ChLayer& L = p.layer[l];
+    // weights and bias of layer l replace those of layer l - 1 (whose MMAs have all retired: wait<0> + barrier below)
+    if (t == 0) {
+      tc::mbar_expect_tx(&bar_w, p.w_bytes);
+      tc::bulk_load(L.wpack, &bar_w, smW, p.w_bytes);
+    }
+    if (t < p.NB) bias_s[t] = L.bias[t];
+    __syncthreads();
+    tc::mbar_wait(&bar_w, (uint32_t)l & 1u);
+    const T* res = L.res >= 0 ? reinterpret_cast<const T*>(p.buf[L.res]) : nullptr;
+    T* dst = reinterpret_cast<T*>(p.buf[L.dst]);
+    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ph_in ^= 1u) {
+      const int ty0 = tile / p.tiles_x, tx0 = tile - ty0 * p.tiles_x;
+      if (t == 0) {
+        // RAW on the source and WAR on the destination: the <= 9 tiles around this one have completed layer l - 1
+        for (int dy = -1; dy <= 1; ++dy)
+          for (int dx = -1; dx <= 1; ++dx) {
+            const int y = ty0 + dy, x = tx0 + dx;
+            if (y < 0 || y >= p.tiles_y || x < 0 || x >= p.tiles_x) continue;
+            const int* f = p.flags + y * p.tiles_x + x;
+            while (ld_acquire(f) < l) __nanosleep(64);
           }
-          __syncwarp();
-          CH_TRACE(0, 3, n);
+        asm volatile("fence.proxy.async.global;" ::: "memory");   // generic stores of other CTAs -> this TMA read
+        tc::mbar_expect_tx(&bar_in, CH_A_TX);
+        tc::tma_load_3d(&maps.ld[L.src], &bar_in, smIn, 0, tx0 * CH_TW - 1, ty0 * CH_TH - 1);
+      }
+      tc::mbar_wait(&bar_in, ph_in);
+      float acc[2][NB / 2];
+      tc::wgmma_fence();
+      for (int ky = 0; ky < 3; ++ky)
+        for (int kx = 0; kx < 3; ++kx) {
+          const uint64_t bd = tc::desc_sw128(w_a + (uint32_t)((ky * 3 + kx) * NB * 128));
+          const uint32_t at = in_a + (uint32_t)((ky * CH_BW + kx) * 128);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const uint64_t ad = tc::desc_sw128(at + (uint32_t)h * 8 * CH_BW * 128, CH_BW * 128);
+#pragma unroll
+            for (int k = 0; k < 3; ++k)
+              if (k < p.ksteps) tc::wgmma<NB, BF>(acc[h], ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (ky | kx | k) ? 1u : 0u);
+          }
         }
-        const int ty = tile / p.tiles_x, tx = tile - ty * p.tiles_x;
-        if (l > 0) {
-          // Tile-level dependency: the 3 x 3 tile neighbourhood (incl. the tile itself) has completed l layers.  One poll
-          // round looks at THREE local tiles (lanes 0-8 / 9-17 / 18-26) and remembers which of the next two are already
-          // satisfied, so in steady state there is one L2 round trip per three tiles, yet tile k never waits for the
-          // dependencies of k+1 / k+2.  Polls are relaxed GPU-scope loads; one acquire fence once the tile is cleared.
-          if (!(known & 1u)) {
-            const int j = lane / 9, nbr = lane - j * 9;
-            const int dy = nbr / 3 - 1, dx = nbr - (nbr / 3) * 3 - 1;
-            const int tj = tile + j * G;
-            const int tyj = tj / p.tiles_x, txj = tj - tyj * p.tiles_x;
-            const int tiles_y = p.ntiles / p.tiles_x;
-            const int ny = tyj + dy, nx = txj + dx;
-            const bool need = lane < 27 && (k + j) < ntl && ny >= 0 && ny < tiles_y && nx >= 0 && nx < p.tiles_x;
-            const int* f = p.flags + (need ? ny * p.tiles_x + nx : 0);
-            uint32_t spins = 0;
-            while (true) {
-              const int v = need ? ld_relaxed(f) : l;
-              const uint32_t b = __ballot_sync(0xffffffffu, v >= l);
-              known = ((b & 0x1ffu) == 0x1ffu ? 1u : 0u) | (((b >> 9) & 0x1ffu) == 0x1ffu ? 2u : 0u) |
-                      (((b >> 18) & 0x1ffu) == 0x1ffu ? 4u : 0u);
-              if (known & 1u) break;
-              if (++spins > (1u << 24)) __trap();
+      tc::wgmma_commit();
+      tc::wgmma_wait<0>();
+      // ---- epilogue (the arithmetic of conv_tc.cu) ----
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int r2 = 0; r2 < 2; ++r2) {
+          const int m = 64 * h + 16 * wq + (lane >> 2) + 8 * r2;
+          const int oy = ty0 * CH_TH + (m >> 3), ox = tx0 * CH_TW + (m & 7);
+          if (oy >= p.H || ox >= p.W) continue;
+          const size_t pix = (size_t)oy * p.W + ox;
+#pragma unroll
+          for (int j = 0; j < NB / 8; ++j) {
+            const int n = 8 * j + 2 * (lane & 3);
+            if (n >= p.C) break;
+            float v[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const float x = acc[h][4 * j + 2 * r2 + e] + bias_s[n + e];
+              v[e] = fmaxf(x, x * L.pre_slope);
             }
-            __threadfence();                                   // acquire side of the flags' release stores
-            asm volatile("fence.proxy.async;" ::: "memory");   // ... and the data is read through the async proxy (TMA) next
-          }
-          known >>= 1;
-        }
-        CH_TRACE(0, 1, n);
-        const int slot = (int)(n % (uint32_t)p.slots);
-        const uint32_t ph = (n / (uint32_t)p.slots) & 1u;
-        mbar_wait_wd(&bar_empty[slot], ph ^ 1u);
-        if (tc::elect_one()) {
-          tc::mbar_expect_tx(&bar_full[slot], CH_A_TX);
-          tc::tma_load_3d(&maps.ld[src], &bar_full[slot], smemA + (size_t)slot * CH_A_BYTES, 0, tx * CH_TW - 1, ty * CH_TH - 1);
-        }
-        __syncwarp();
-        CH_TRACE(0, 2, n);
-      }
-    }
-  } else if (warp_u < 1 + CH_NMMA) {
-    // ============================ MMA issuers ==============================
-    const int id = warp_u - 1;
-    if (id < p.nmma) {
-      const uint32_t idesc = tc::umma_idesc(p.fmt, 128, p.NB);
-      const uint64_t adesc0 = tc::umma_desc_sw128(tc::smem_u32(smemA)) + ((uint64_t)((CH_BW * 128 - 1024) >> 4) << 32);
-      const uint64_t bdesc0 = tc::umma_desc_sw128(tc::smem_u32(smemW));
-      const uint32_t a_step = CH_A_BYTES >> 4, b_tap = (uint32_t)(p.NB * 128) >> 4;
-      for (int l = 0; l < p.nlayers; ++l) {
-        bool first = true;
-        for (int k = id; k < ntl; k += p.nmma) {
-          const uint32_t n = (uint32_t)l * (uint32_t)ntl + (uint32_t)k;
-          CH_TRACE(1 + id, 0, n);
-          if (first) {
-            mbar_wait_wd(&bar_w, (uint32_t)l & 1u);            // this layer's weights are resident
-            first = false;
-          }
-          CH_TRACE(1 + id, 1, n);
-          const uint32_t slot = n % (uint32_t)p.slots, ph = (n / (uint32_t)p.slots) & 1u;
-          const uint32_t acc = n % (uint32_t)CH_NACC, accph = (n / (uint32_t)CH_NACC) & 1u;
-          mbar_wait_wd(&bar_tempty[acc], accph ^ 1u);
-          CH_TRACE(1 + id, 2, n);
-          mbar_wait_wd(&bar_full[slot], ph);
-          CH_TRACE(1 + id, 3, n);
-          tc::tc_fence_after();
-          const uint32_t d_tmem = tmem_base + acc * (uint32_t)p.NB;
-          const uint64_t ad = adesc0 + (uint64_t)(slot * a_step);
-          if (tc::elect_one()) {
-#pragma unroll 1
-            for (int ky = 0; ky < 3; ++ky) {
-#pragma unroll
-              for (int kx = 0; kx < 3; ++kx) {
-                const uint64_t a_tap = ad + (uint64_t)((ky * CH_BW + kx) * 8);
-                const uint64_t b_t = bdesc0 + (uint64_t)((ky * 3 + kx) * b_tap);
-#pragma unroll
-                for (int ks = 0; ks < 4; ++ks)
-                  if (ks < p.ksteps)
-                    tc::umma_f16(d_tmem, a_tap + (uint64_t)(ks * 2), b_t + (uint64_t)(ks * 2), idesc, (ky | kx | ks) ? 1u : 0u);
-              }
+            if (res != nullptr) {       // written earlier in this launch by this CTA: coherent (non-.nc) loads
+              uint32_t rw = *reinterpret_cast<const volatile uint32_t*>(res + pix * p.C + n);
+              const T* r = reinterpret_cast<const T*>(&rw);
+              v[0] += to_f(r[0]); v[1] += to_f(r[1]);
             }
-            tc::umma_commit(&bar_empty[slot]);      // frees the activation slot when these MMAs retire
-            tc::umma_commit(&bar_tfull[acc]);       // accumulator complete -> epilogue group acc % 3
-          }
-          __syncwarp();
-          CH_TRACE(1 + id, 4, n);
-        }
-        // this warp's share of layer l has been issued: bar_wfree completes once all issuers' MMAs of the layer retired
-        if (tc::elect_one()) tc::umma_commit(&bar_wfree);
-        __syncwarp();
-      }
-    }
-  } else {
-    // ============================ epilogue (TMA store) ================================
-    const int grp = (warp - 1 - CH_NMMA) >> 2;      // handles n = grp, grp + 3, ...  (accumulators grp and grp + 3)
-    const int q = warp & 3;                         // TMEM lane quarter
-    const int m = q * 32 + lane;                    // tile pixel: row m >> 3, column m & 7
-    const int ty = m >> 3, tx = m & 7;
-    uint8_t* stg = smemS + (size_t)grp * CH_STG_BYTES;
-    uint8_t* stg_row = stg + (size_t)m * 128;
-    const int nch = p.NB >> 4;                      // 16-column chunks (<= 3)
-    const int nvec = p.C >> 3;                      // 16-byte vectors per pixel row in global memory (C % 8 == 0)
-    int pend_tile = -1, pend_val = 0;               // store issued, flag not yet published (tracked by warp q == 0)
-    uint4 rn[6];
-    bool rn_ok = false;
-
-    auto locate = [&](uint32_t n, int& l, int& k) {
-      l = (int)(n / (uint32_t)ntl);
-      k = (int)(n - (uint32_t)l * (uint32_t)ntl);
-    };
-    auto res_ptr = [&](int l, int tile) -> const uint8_t* {
-      const int tyy = tile / p.tiles_x, txx = tile - tyy * p.tiles_x;
-      const int oy = tyy * CH_TH + ty, ox = txx * CH_TW + tx;
-      const bool valid = oy < p.H && ox < p.W;
-      return reinterpret_cast<const uint8_t*>(p.buf[p.layer[l].res]) + (valid ? ((size_t)oy * p.W + ox) * (size_t)p.C * 2 : 0);
-    };
-    // residual vectors of (l, tile) if they can be fetched NOW: the tile that holds them must already be published
-    auto try_fetch = [&](uint32_t n, uint4 (&dst)[6]) -> bool {
-      if (n >= total) return false;
-      int l, k;
-      locate(n, l, k);
-      if (p.layer[l].res < 0) return false;
-      const int tile = blockIdx.x + k * G;
-      const int need = p.layer[l].res_need;
-      if (need > 0 && ld_relaxed(p.flags + tile) < need) return false;      // (the vectors below are L2 reads issued after this test)
-      const uint8_t* r = res_ptr(l, tile);
+            T pr[2];
 #pragma unroll
-      for (int v = 0; v < 6; ++v)
-        if (v < nvec) dst[v] = ld_cg16(r + v * 16);
-      return true;
-    };
-
-    rn_ok = try_fetch((uint32_t)grp, rn);
-    for (uint32_t n = (uint32_t)grp; n < total; n += CH_NGRP) {
-      int l, k;
-      locate(n, l, k);
-      const int tile = blockIdx.x + k * G;
-      const ChLayer& L = p.layer[l];
-      const bool has_res = L.res >= 0;
-      uint4 rp[6];
-      bool rp_ok = rn_ok;
-#pragma unroll
-      for (int v = 0; v < 6; ++v) rp[v] = rn[v];
-      rn_ok = try_fetch(n + CH_NGRP, rn);           // one tile ahead (conv_tc.cu: a prefetch issued later hides nothing)
-
-      const uint32_t acc = n % (uint32_t)CH_NACC, accph = (n / (uint32_t)CH_NACC) & 1u;
-      if (q == 0) CH_TRACE(4 + grp, 0, n);
-      if (q == 0 && pend_tile >= 0) {
-        // never block on an accumulator while holding an unpublished flag (deadlock freedom for any tile count)
-        const bool ready = __all_sync(0xffffffffu, tc::mbar_try_wait(&bar_tfull[acc], accph));
-        if (!ready) {
-          if (lane == 0) publish(p.flags + pend_tile, pend_val);
-          pend_tile = -1;
-        }
-        __syncwarp();
-      }
-      mbar_wait_wd(&bar_tfull[acc], accph);
-      tc::tc_fence_after();
-      if (q == 0) CH_TRACE(4 + grp, 1, n);
-      if (has_res && !rp_ok) {                      // rare: the residual tile was not yet published one tile ago
-        const uint8_t* r = res_ptr(l, tile);        // (now it is: this tile's box was loaded after flags[tile] >= l >= res_need)
-#pragma unroll
-        for (int v = 0; v < 6; ++v)
-          if (v < nvec) rp[v] = ld_cg16(r + v * 16);
-      }
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * (uint32_t)p.NB;
-      uint32_t r[3][16];
-#pragma unroll
-      for (int c = 0; c < 3; ++c)
-        if (c < nch) tc::tmem_ld16(taddr + (uint32_t)c * 16, r[c]);
-      tc::tmem_ld_wait();
-      tc::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&bar_tempty[acc]);        // accumulator back to the MMA warps before the arithmetic
-      if (q == 0) CH_TRACE(4 + grp, 2, n);
-
-      const float pre_slope = L.pre_slope, post_slope = L.post_slope;
-      const int act_pre = (pre_slope == 1.f) ? 0 : (pre_slope == 0.f ? 1 : 2);
-      const int act_post = (post_slope == 1.f) ? 0 : (post_slope == 0.f ? 1 : 2);
-      const float4* bias4 = reinterpret_cast<const float4*>(&bias_s[l & 3][0]);
-      uint32_t ob[3][8];
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        if (c >= nch) break;
-        float v[16];
-#pragma unroll
-        for (int j = 0; j < 16; j += 4) {
-          const float4 b4 = bias4[c * 4 + (j >> 2)];
-          v[j] = __uint_as_float(r[c][j]) + b4.x;
-          v[j + 1] = __uint_as_float(r[c][j + 1]) + b4.y;
-          v[j + 2] = __uint_as_float(r[c][j + 2]) + b4.z;
-          v[j + 3] = __uint_as_float(r[c][j + 3]) + b4.w;
-        }
-        if (act_pre == 1) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f);
-        } else if (act_pre == 2) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], v[j] * pre_slope);
-        }
-        if (has_res && 2 * c < nvec) {               // channels >= C are padding: zero weights, clipped by the store
-          const uint4 ra = rp[2 * c], rb = (2 * c + 1 < nvec) ? rp[2 * c + 1] : make_uint4(0, 0, 0, 0);
-          const uint32_t rw[8] = {ra.x, ra.y, ra.z, ra.w, rb.x, rb.y, rb.z, rb.w};
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float2 r2 = unpack2h(rw[j], T());
-            v[2 * j] += r2.x;
-            v[2 * j + 1] += r2.y;
+            for (int e = 0; e < 2; ++e) pr[e] = from_f<T>(fmaxf(v[e], v[e] * L.post_slope));
+            *reinterpret_cast<uint32_t*>(dst + pix * p.C + n) = *reinterpret_cast<uint32_t*>(pr);
           }
         }
-        if (act_post == 1) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f);
-        } else if (act_post == 2) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], v[j] * post_slope);
-        }
-#pragma unroll
-        for (int j = 0; j < 8; ++j) ob[c][j] = pack2h(v[2 * j], v[2 * j + 1], T());
-      }
-
-      if (q == 0) CH_TRACE(4 + grp, 3, n);
-      // the staging tile is free once the group's previous store has READ it (completion / publication comes later)
-      if (q == 0 && lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-      group_bar(1 + grp);
-      // staging tile = 128 pixel rows of 128 B, 16-byte chunk j of row m at chunk j ^ (m & 7)  (SWIZZLE_128B)
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        if (c >= nch) break;
-        *reinterpret_cast<uint4*>(stg_row + (((2 * c) ^ (m & 7)) << 4)) = make_uint4(ob[c][0], ob[c][1], ob[c][2], ob[c][3]);
-        *reinterpret_cast<uint4*>(stg_row + (((2 * c + 1) ^ (m & 7)) << 4)) = make_uint4(ob[c][4], ob[c][5], ob[c][6], ob[c][7]);
-      }
-      tc::fence_proxy_async();                      // generic smem writes -> visible to the async proxy (TMA store)
-      group_bar(1 + CH_NGRP + grp);
-      if (q == 0) CH_TRACE(4 + grp, 4, n);
-      if (q == 0) {
-        if (lane == 0) {
-          const int tyy = tile / p.tiles_x, txx = tile - tyy * p.tiles_x;
-          tma_store_3d(&maps.st[L.dst], stg, 0, txx * CH_TW, tyy * CH_TH);
-          // the PREVIOUS store of this group has had a whole iteration to complete: publish its flag now, off the other
-          // three warps' path (they are already waiting for / draining the next accumulator)
-          if (pend_tile >= 0) publish_prev(p.flags + pend_tile, pend_val);
-        }
-        pend_tile = tile;
-        pend_val = l + 1;
-        __syncwarp();
-        CH_TRACE(4 + grp, 5, n);
-      }
+      __threadfence();
+      __syncthreads();                 // all stores of the tile done; the input box is free again
+      if (t == 0) asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p.flags + tile), "r"(l + 1) : "memory");
     }
-    if (q == 0 && pend_tile >= 0 && lane == 0) publish(p.flags + pend_tile, pend_val);
   }
-
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 1 + CH_NMMA) tc::tmem_dealloc(tmem_base, 512);
 }
 
-int make_map(CUtensorMap* m, const void* ptr, int C, int W, int H, int box_w, int box_h, int fmt) {
+int make_map(CUtensorMap* m, const void* ptr, int C, int W, int H, int fmt) {
   PFN_tmapEncodeTiled enc = get_tmap_encoder();
   if (!enc) return fail(RV_E_CUDA, "cuTensorMapEncodeTiled entry point not available");
   cuuint64_t gdim[3] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H};
   cuuint64_t gstr[2] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2};
-  cuuint32_t box[3] = {64u, (cuuint32_t)box_w, (cuuint32_t)box_h};
+  cuuint32_t box[3] = {64u, (cuuint32_t)CH_BW, (cuuint32_t)CH_BH};
   cuuint32_t estr[3] = {1, 1, 1};
   CUresult r = enc(m, fmt ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(ptr), gdim, gstr,
                    box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -494,38 +185,22 @@ extern "C" int rv_conv_chain(const rv_conv_chain_desc* d, void* stream) {
   RV_REQUIRE(d->nb >= 16 && d->nb <= 48 && d->nb % 16 == 0 && d->nb >= d->C, "rv_conv_chain: nb=%d must be 16/32/48 and >= C=%d", d->nb, d->C);
   for (int b = 0; b < d->nbuf; ++b)
     RV_REQUIRE(d->buf[b] != nullptr && (uintptr_t)d->buf[b] % 16 == 0, "rv_conv_chain: buffer %d null or not 16-byte aligned", b);
-  static int num_sms = 0, max_smem = 0;
+  static int num_sms = 0;
   if (num_sms == 0) {
     int dev = 0;
     RV_CUDA_OK(cudaGetDevice(&dev));
     RV_CUDA_OK(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
-    RV_CUDA_OK(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
   }
   static ChP p;            // (host-side scratch; the launch copies it by value)
   static ChMaps maps;
   p.H = d->H; p.W = d->W; p.C = d->C; p.NB = d->nb;
   p.tiles_x = (d->W + CH_TW - 1) / CH_TW;
-  const int tiles_y = (d->H + CH_TH - 1) / CH_TH;
-  p.ntiles = p.tiles_x * tiles_y;
+  p.tiles_y = (d->H + CH_TH - 1) / CH_TH;
   p.nlayers = d->nlayers;
-  p.fmt = d->dtype == RV_BF16 ? 1 : 0;
   p.ksteps = (d->C + 15) / 16;
   p.w_bytes = 9u * (uint32_t)d->nb * 128u;
   p.flags = d->flags;
-  { const char* e = getenv("REFVSR_CHAIN_TRACE"); p.trace = e ? (long long*)strtoull(e, nullptr, 0) : nullptr; }
-  { const char* e = getenv("REFVSR_CHAIN_TRACE_CTA"); p.trace_cta = e ? atoi(e) : 70; }
-  const size_t fixed = 1024 + 2048 + (size_t)p.w_bytes + (size_t)CH_NGRP * CH_STG_BYTES;
-  RV_REQUIRE((size_t)max_smem > fixed + 2 * (size_t)CH_A_BYTES, "rv_conv_chain: shared memory too small");
-  p.slots = (int)std::min<size_t>(CH_MAXSLOTS, ((size_t)max_smem - fixed) / CH_A_BYTES);
-  int grid = std::min(num_sms, p.ntiles);
-  if (d->max_ctas > 0) grid = std::min(grid, (int)d->max_ctas);
-  p.nmma = std::max(1, std::min(std::min(CH_NMMA, p.ntiles / grid), p.slots));
-  { const char* e = getenv("REFVSR_CHAIN_NMMA"); if (e && atoi(e) > 0) p.nmma = std::min(p.nmma, atoi(e)); }
-  // every issuer must own its smem slots exclusively (mbarrier parity waits alias across issuers otherwise - conv_tc.cu): slots is
-  // a multiple of the issuer count; CH_NACC = 6 is a multiple of 1, 2 and 3
-  p.slots = (p.slots / p.nmma) * p.nmma;
-  int last_write[CH_MAXB];
-  for (int b = 0; b < CH_MAXB; ++b) { last_write[b] = 0; p.buf[b] = b < d->nbuf ? d->buf[b] : nullptr; }
+  for (int b = 0; b < CH_MAXB; ++b) p.buf[b] = b < d->nbuf ? d->buf[b] : nullptr;
   for (int l = 0; l < d->nlayers; ++l) {
     const rv_chain_layer& s = d->layers[l];
     RV_REQUIRE(s.wpack && s.bias && (uintptr_t)s.wpack % 16 == 0 && (uintptr_t)s.bias % 16 == 0, "rv_conv_chain: layer %d: null / unaligned weights", l);
@@ -536,29 +211,30 @@ extern "C" int rv_conv_chain(const rv_conv_chain_desc* d, void* stream) {
     L.wpack = (const uint8_t*)s.wpack; L.bias = s.bias;
     L.pre_slope = slope_of(s.act_pre); L.post_slope = slope_of(s.act_post);
     L.src = s.src; L.res = s.res < 0 ? -1 : s.res; L.dst = s.dst;
-    L.res_need = L.res >= 0 ? last_write[L.res] : 0;
-    last_write[s.dst] = l + 1;
   }
+  const int fmt = d->dtype == RV_BF16 ? 1 : 0;
   for (int b = 0; b < d->nbuf; ++b) {
-    int rc = make_map(&maps.ld[b], d->buf[b], d->C, d->W, d->H, CH_BW, CH_BH, p.fmt);
-    if (rc) return rc;
-    rc = make_map(&maps.st[b], d->buf[b], d->C, d->W, d->H, CH_TW, CH_TH, p.fmt);
+    const int rc = make_map(&maps.ld[b], d->buf[b], d->C, d->W, d->H, fmt);
     if (rc) return rc;
   }
-  for (int b = d->nbuf; b < CH_MAXB; ++b) { maps.ld[b] = maps.ld[0]; maps.st[b] = maps.st[0]; }
-  const size_t smem = 1024 + (size_t)p.slots * CH_A_BYTES + p.w_bytes + (size_t)CH_NGRP * CH_STG_BYTES;
+  for (int b = d->nbuf; b < CH_MAXB; ++b) maps.ld[b] = maps.ld[0];
+  const int ntiles = p.tiles_x * p.tiles_y;
+  int grid = std::min(num_sms, ntiles);
+  if (d->max_ctas > 0) grid = std::min(grid, (int)d->max_ctas);
+  const size_t smem = 1024 + CH_A_BYTES + p.w_bytes;
   cudaStream_t st = (cudaStream_t)stream;
-  RV_CUDA_OK(cudaMemsetAsync(d->flags, 0, (size_t)p.ntiles * sizeof(int), st));
-  // (one "configured" high-water mark per instantiation: both kernels have the same function-pointer TYPE, so a static inside
-  //  a generic lambda would be shared and the second dtype would launch without its shared-memory attribute)
-  static size_t configured[2] = {0, 0};
-  const int ki = d->dtype == RV_BF16 ? 1 : 0;
-  void (*kern)(ChMaps, ChP) = ki ? conv_chain_kernel<__nv_bfloat16> : conv_chain_kernel<__half>;
-  if (smem > configured[ki]) {
+  RV_CUDA_OK(cudaMemsetAsync(d->flags, 0, (size_t)ntiles * sizeof(int), st));
+  static size_t configured[2][3] = {};
+  const int ni = p.NB / 16 - 1;
+  void (*const kerns[2][3])(ChMaps, ChP) = {
+      {conv_chain_kernel<__half, 16>, conv_chain_kernel<__half, 32>, conv_chain_kernel<__half, 48>},
+      {conv_chain_kernel<__nv_bfloat16, 16>, conv_chain_kernel<__nv_bfloat16, 32>, conv_chain_kernel<__nv_bfloat16, 48>}};
+  void (*kern)(ChMaps, ChP) = kerns[fmt][ni];
+  if (smem > configured[fmt][ni]) {
     RV_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured[ki] = smem;
+    configured[fmt][ni] = smem;
   }
-  kern<<<grid, 32 * (1 + CH_NMMA) + 128 * CH_NGRP, smem, st>>>(maps, p);
+  kern<<<grid, 128, smem, st>>>(maps, p);
   RV_LAUNCH_CHECK("conv_chain");
   return RV_OK;
 }

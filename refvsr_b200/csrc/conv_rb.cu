@@ -1,25 +1,25 @@
-// Fused residual block on tcgen05:   out = post( x + conv2( act( conv1(x) ) ) )      (3x3, C -> C -> C, C <= 64)
+// Fused residual block on wgmma:   out = post( x + conv2( act( conv1(x) ) ) )      (3x3, C -> C -> C, C <= 64)
 //
 // Replaces two rv_conv2d launches per ResidualBlockNoBN / ResBlock
 // (mmedit/models/common/sr_backbone_utils.py:85-97, models/archs/RefVSR_/common.py:33-39): the intermediate
 // activation never leaves the SM and the skip connection is read from the input box that is already in
 // shared memory.
 //
-// Per output tile of 16 rows x 8 columns (one UMMA M=128 tile):
+// Per output tile of 16 rows x 8 columns (M = 128):
 //   * ONE TMA box of the input: 20 rows x 12 columns x 64 channels (2-pixel halo, pitch 12 pixel rows of 128 B,
 //     SWIZZLE_128B, out-of-bounds zero fill = conv1's zero padding).
 //   * conv1 is evaluated on the 18 x 10 halo region, indexed with the same pitch: m1 = yy*12 + xx, so that
-//     input pixel (yy+ky, xx+kx) is simply smem row m1 + ky*12 + kx -> every tap is a row-shifted view of the box
-//     (operand swizzle is a pure function of the smem address, see conv_tc.cu).  216 rows = 2 M-tiles.
-//   * epilogue 1 (8 warps): TMEM -> bias + activation -> 0 outside the image (conv2's zero padding) -> 16-bit ->
-//     written to shared memory in exactly the swizzled K-major operand layout (pitch 12), fence.proxy.async.
+//     input pixel (yy+ky, xx+kx) is simply smem row m1 + ky*12 + kx -> every tap is a row-shifted descriptor view of
+//     the box.  216 rows, computed as four m64 blocks (two per consumer warpgroup; rows >= 216 are never read).
+//   * epilogue 1 (from the accumulator registers): bias + activation -> 0 outside the image (conv2's zero padding) ->
+//     16-bit -> written to shared memory in exactly the swizzled K-major operand layout (pitch 12), fence.proxy.async.
 //   * conv2: M = 128 = 16 x 8, row m2 = ty*8 + tx reads intermediate row (ty+ky)*12 + tx + kx: 8-row groups are
-//     contiguous, consecutive groups 12 rows apart -> SBO = 1536 bytes.
-//   * epilogue 2 (4 warps): TMEM + bias + residual (input box pixel (ty+2, tx+2), de-swizzled from smem) ->
-//     optional post-activation -> NHWC store.
-// Both weight sets stay resident ([9 taps][NB][64] each, host-swizzled); TMEM holds two {D1a, D1b, D2} sets so the
-// MMA warp runs conv1 of tile t+1 while the epilogue groups work on tile t.
-#include <cstdlib>
+//     contiguous, consecutive groups 12 rows apart -> SBO = 1536 bytes; warpgroup g computes tile rows 8g .. 8g + 7.
+//   * epilogue 2: + bias + residual (input box pixel (ty+2, tx+2), de-swizzled from smem) -> optional
+//     post-activation -> NHWC store.
+// Both weight sets stay resident ([9 taps][NB][64] each, host-swizzled).  256 threads = two consumer warpgroups;
+// thread 0 also issues the TMA loads.  Persistent CTAs walk the tile list.
+#include <algorithm>
 
 #include "common.cuh"
 #include "tc_common.cuh"
@@ -30,11 +30,12 @@ static constexpr int RB_TH = 16, RB_TW = 8;      // output tile
 static constexpr int RB_P = 12;                  // pixel-row pitch of the input box and of the intermediate
 static constexpr int RB_IN_ROWS = RB_TH + 4;     // 20 box rows
 static constexpr uint32_t RB_IN_BYTES = RB_IN_ROWS * RB_P * 128;  // 30720
-static constexpr uint32_t RB_MID_BYTES = 256 * 128;               // 2 M-tiles of intermediate rows (216 used)
+// intermediate: 256 rows; conv1's garbage rows (216..255) read the input up to 26 rows past the box, which lands here
+static constexpr uint32_t RB_MID_BYTES = 256 * 128;
 static constexpr int RB_MID_VALID = (RB_TH + 2) * RB_P;           // 216
 
 struct RbP {
-  int H, W, C, cout, NB, tiles_x, tiles_y, fmt;
+  int H, W, C, cout, NB, tiles_x, tiles_y, ksteps;
   uint32_t w_bytes;  // one conv: 9 * NB * 128
   const uint8_t* w1;
   const uint8_t* w2;
@@ -42,290 +43,149 @@ struct RbP {
   const float* b2;
   float mid_slope, post_slope;
   void* out;
-  int out_cs, vec_ok;
-  uint32_t tmem_cols;
+  int out_cs, pair_ok;
 };
 
-template <typename T>
-__global__ void __launch_bounds__(448, 1) conv_rb_kernel(const __grid_constant__ CUtensorMap tmx, const RbP p) {
-  extern __shared__ uint8_t smem_raw[];
-  __shared__ uint64_t bar_in_full[2], bar_in_empty[2], bar_w, bar_d1_full[2], bar_d1_empty[2], bar_mid_full,
-      bar_mid_empty, bar_d2_full[2], bar_d2_empty[2];
-  __shared__ uint32_t tmem_base_s;
-  __shared__ float bias1_s[64], bias2_s[64];
+// byte offset of channel n of row r in a 128B-swizzled K-major tile whose base is 1024-byte aligned
+__device__ __forceinline__ uint32_t sw128_off(int r, int n) {
+  return (uint32_t)r * 128u + ((uint32_t)(((n >> 3) ^ (r & 7)) << 4)) + (uint32_t)((n & 7) * 2);
+}
 
+template <typename T, int NB>   // NB: output channels (= p.NB)
+__global__ void __launch_bounds__(256, 1) conv_rb_kernel(const __grid_constant__ CUtensorMap tmx, const RbP p) {
+  constexpr bool BF = std::is_same<T, __nv_bfloat16>::value;
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ uint64_t bar_w, bar_in;
+  __shared__ float b1_s[64], b2_s[64];
   const uint32_t raw = tc::smem_u32(smem_raw);
   uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
   uint8_t* smW1 = smem;
   uint8_t* smW2 = smW1 + p.w_bytes;
-  uint8_t* smIn = smW2 + p.w_bytes;              // 2 slots
-  uint8_t* smMid = smIn + 2 * RB_IN_BYTES;       // 1 buffer (+ slack rows read by the garbage M rows of conv1)
+  uint8_t* smIn = smW2 + p.w_bytes;
+  uint8_t* smMid = smIn + RB_IN_BYTES;
+  const int g = threadIdx.x >> 7, t = threadIdx.x & 127, wq = t >> 5, lane = t & 31;
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int warp_u = __shfl_sync(0xffffffffu, warp, 0);   // provably warp-uniform copy for the role dispatch
-  const int ntiles = p.tiles_x * p.tiles_y;
-  const int ksteps = (min(p.C, 64) + 15) >> 4;
-
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
   if (threadIdx.x == 0) {
-    for (int i = 0; i < 2; ++i) {
-      tc::mbar_init(&bar_in_full[i], 1);
-      tc::mbar_init(&bar_in_empty[i], 4);    // the 4 epilogue-2 warps (they read the residual last)
-      tc::mbar_init(&bar_d1_full[i], 1);
-      tc::mbar_init(&bar_d1_empty[i], 8);    // the 8 epilogue-1 warps
-      tc::mbar_init(&bar_d2_full[i], 1);
-      tc::mbar_init(&bar_d2_empty[i], 4);
-    }
     tc::mbar_init(&bar_w, 1);
-    tc::mbar_init(&bar_mid_full, 8);
-    tc::mbar_init(&bar_mid_empty, 1);
+    tc::mbar_init(&bar_in, 1);
     tc::fence_barrier_init();
     tc::prefetch_tmap(&tmx);
   }
-  if (warp == 2) tc::tmem_alloc(&tmem_base_s, p.tmem_cols);
-  for (int i = threadIdx.x; i < 64; i += blockDim.x) {
-    bias1_s[i] = (i < p.cout) ? p.b1[i] : 0.f;
-    bias2_s[i] = (i < p.cout) ? p.b2[i] : 0.f;
+  if (threadIdx.x < 64) {
+    b1_s[threadIdx.x] = (int)threadIdx.x < p.cout ? p.b1[threadIdx.x] : 0.f;
+    b2_s[threadIdx.x] = (int)threadIdx.x < p.cout ? p.b2[threadIdx.x] : 0.f;
   }
-  tc::tc_fence_before();
+  // intermediate channels the epilogue never writes (NB .. 63) are read by conv2's K slices only with zero weights, but
+  // must not hold NaN patterns
+  for (int i = threadIdx.x; i < (int)(RB_MID_BYTES / 16); i += blockDim.x) reinterpret_cast<uint4*>(smMid)[i] = make_uint4(0, 0, 0, 0);
+  tc::fence_proxy_async();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem_base = tmem_base_s;
-  const uint32_t set_stride = 3u * (uint32_t)p.NB;   // {D1 tile0, D1 tile1, D2}
+  if (threadIdx.x == 0) {
+    tc::mbar_expect_tx(&bar_w, 2 * p.w_bytes);
+    tc::bulk_load(p.w1, &bar_w, smW1, p.w_bytes);
+    tc::bulk_load(p.w2, &bar_w, smW2, p.w_bytes);
+  }
+  tc::mbar_wait(&bar_w, 0);
 
-  // Producer and MMA warps: warp-uniform control flow, one elected lane issues (see tc::elect_one).
-  if (warp_u == 0) {
-    // ===================== TMA producer =====================
-    if (tc::elect_one()) {
-      tc::mbar_expect_tx(&bar_w, 2u * p.w_bytes);
-      tc::bulk_load(p.w1, &bar_w, smW1, p.w_bytes);
-      tc::bulk_load(p.w2, &bar_w, smW2, p.w_bytes);
+  const uint32_t in_a = tc::smem_u32(smIn), mid_a = tc::smem_u32(smMid);
+  const uint32_t w1_a = tc::smem_u32(smW1), w2_a = tc::smem_u32(smW2);
+  T* out = reinterpret_cast<T*>(p.out);
+  const int ntiles = p.tiles_x * p.tiles_y;
+  uint32_t ph = 0;
+  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ph ^= 1u) {
+    const int ty0 = tile / p.tiles_x, tx0 = tile - ty0 * p.tiles_x;
+    if (threadIdx.x == 0) {
+      tc::mbar_expect_tx(&bar_in, RB_IN_BYTES);
+      tc::tma_load_3d(&tmx, &bar_in, smIn, 0, tx0 * RB_TW - 2, ty0 * RB_TH - 2);
     }
-    __syncwarp();
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      const int slot = it & 1;
-      const uint32_t ph = (it >> 1) & 1u;
-      tc::mbar_wait(&bar_in_empty[slot], ph ^ 1u);
-      if (tc::elect_one()) {
-        tc::mbar_expect_tx(&bar_in_full[slot], RB_IN_BYTES);
-        const int ty0 = tile / p.tiles_x, tx0 = tile - ty0 * p.tiles_x;
-        tc::tma_load_3d(&tmx, &bar_in_full[slot], smIn + (size_t)slot * RB_IN_BYTES, 0, tx0 * RB_TW - 2, ty0 * RB_TH - 2);
+    tc::mbar_wait(&bar_in, ph);
+
+    // ---- conv1 over the 18 x 10 halo region: m64 blocks 2g and 2g + 1 ----
+    float acc1[2][NB / 2];
+    tc::wgmma_fence();
+    for (int ky = 0; ky < 3; ++ky)
+      for (int kx = 0; kx < 3; ++kx) {
+        const uint64_t bd = tc::desc_sw128(w1_a + (uint32_t)((ky * 3 + kx) * NB * 128));
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint64_t ad = tc::desc_sw128(in_a + (uint32_t)((64 * (2 * g + h) + ky * RB_P + kx) * 128));
+#pragma unroll
+          for (int k = 0; k < 4; ++k)
+            if (k < p.ksteps) tc::wgmma<NB, BF>(acc1[h], ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (ky | kx | k) ? 1u : 0u);
+        }
       }
-      __syncwarp();
-    }
-  } else if (warp_u == 1) {
-    // ===================== MMA issuer =====================
-    {
-      const uint32_t idesc = tc::umma_idesc(p.fmt, 128, p.NB);
-      const uint64_t in_desc0 = tc::umma_desc_sw128(tc::smem_u32(smIn));                     // SBO 1024
-      const uint64_t mid_desc = tc::umma_desc_sw128(tc::smem_u32(smMid)) +
-                                ((uint64_t)((RB_P * 128 - 1024) >> 4) << 32);                // SBO 1536
-      const uint64_t w1_desc = tc::umma_desc_sw128(tc::smem_u32(smW1));
-      const uint64_t w2_desc = tc::umma_desc_sw128(tc::smem_u32(smW2));
-      const uint32_t b_tap = (uint32_t)(p.NB * 128) >> 4;
-      tc::mbar_wait(&bar_w, 0);
-
-      auto conv1 = [&](uint32_t t) {           // both M-tiles of the halo region of local tile t
-        const int slot = t & 1;
-        const uint32_t ph = (t >> 1) & 1u;
-        tc::mbar_wait(&bar_in_full[slot], ph);
-        tc::mbar_wait(&bar_d1_empty[slot], ph ^ 1u);
-        tc::tc_fence_after();
-        if (tc::elect_one()) {
-          const uint64_t a0 = in_desc0 + (uint64_t)((uint32_t)slot * (RB_IN_BYTES >> 4));
-          const uint32_t d0 = tmem_base + (uint32_t)slot * set_stride;
+    tc::wgmma_commit();
+    tc::wgmma_wait<0>();
+    // ---- epilogue 1 -> swizzled 16-bit intermediate ----
 #pragma unroll
-          for (int j = 0; j < 2; ++j) {
+    for (int h = 0; h < 2; ++h)
 #pragma unroll
-            for (int ky = 0; ky < 3; ++ky)
+      for (int r2 = 0; r2 < 2; ++r2) {
+        const int m1 = 64 * (2 * g + h) + 16 * wq + (lane >> 2) + 8 * r2;
+        if (m1 >= RB_MID_VALID) continue;
+        const int yy = m1 / RB_P, xx = m1 - yy * RB_P;
+        const int iy = ty0 * RB_TH - 1 + yy, ix = tx0 * RB_TW - 1 + xx;
+        const bool inside = xx < RB_TW + 2 && iy >= 0 && iy < p.H && ix >= 0 && ix < p.W;
 #pragma unroll
-              for (int kx = 0; kx < 3; ++kx)
+        for (int j = 0; j < NB / 8; ++j) {
+          const int n = 8 * j + 2 * (lane & 3);
+          float v[2];
 #pragma unroll
-                for (int k = 0; k < 4; ++k)
-                  if (k < ksteps)
-                    tc::umma_f16(d0 + (uint32_t)j * p.NB, a0 + (uint64_t)((j * 128 + ky * RB_P + kx) * 8 + k * 2),
-                                 w1_desc + (uint64_t)((ky * 3 + kx) * b_tap + k * 2), idesc, (ky | kx | k) ? 1u : 0u);
+          for (int e = 0; e < 2; ++e) {
+            const float x = acc1[h][4 * j + 2 * r2 + e] + b1_s[n + e];
+            v[e] = inside ? fmaxf(x, x * p.mid_slope) : 0.f;
           }
-          tc::umma_commit(&bar_d1_full[slot]);
+          T pr[2] = {from_f<T>(v[0]), from_f<T>(v[1])};
+          *reinterpret_cast<uint32_t*>(smMid + sw128_off(m1, n)) = *reinterpret_cast<uint32_t*>(pr);
         }
-        __syncwarp();
-      };
-      auto conv2 = [&](uint32_t t) {
-        const int slot = t & 1;
-        const uint32_t ph = (t >> 1) & 1u;
-        tc::mbar_wait(&bar_mid_full, t & 1u);
-        tc::mbar_wait(&bar_d2_empty[slot], ph ^ 1u);
-        tc::tc_fence_after();
-        if (tc::elect_one()) {
-          const uint32_t d2 = tmem_base + (uint32_t)slot * set_stride + 2u * p.NB;
-#pragma unroll
-          for (int ky = 0; ky < 3; ++ky)
-#pragma unroll
-            for (int kx = 0; kx < 3; ++kx)
-#pragma unroll
-              for (int k = 0; k < 4; ++k)
-                if (k < ksteps)
-                  tc::umma_f16(d2, mid_desc + (uint64_t)((ky * RB_P + kx) * 8 + k * 2),
-                               w2_desc + (uint64_t)((ky * 3 + kx) * b_tap + k * 2), idesc, (ky | kx | k) ? 1u : 0u);
-          tc::umma_commit(&bar_mid_empty);        // intermediate buffer free once these MMAs retire
-          tc::umma_commit(&bar_d2_full[slot]);
-        }
-        __syncwarp();
-      };
-      uint32_t nloc = 0;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) ++nloc;
-      if (nloc > 0) conv1(0);
-      for (uint32_t t = 0; t < nloc; ++t) {
-        if (t + 1 < nloc) conv1(t + 1);          // tensor core stays busy while epilogue 1 of tile t runs
-        conv2(t);
       }
-    }
-  } else if (warp_u < 10) {
-    // ===================== epilogue 1: D1 -> act -> swizzled smem operand =====================
-    const int g = (warp - 2) >> 2;       // M-tile of the halo region
-    const int q = warp & 3;
-    const int m1 = g * 128 + q * 32 + lane;
-    const int yy = m1 / RB_P, xx = m1 - yy * RB_P;
-    const bool row_ok = (m1 < RB_MID_VALID) && (xx < RB_TW + 2);
-    uint8_t* dst_row = smMid + (size_t)m1 * 128;
-    const int sw = m1 & 7;
-    uint32_t t = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++t) {
-      const int slot = t & 1;
-      const uint32_t ph = (t >> 1) & 1u;
-      const int ty0 = tile / p.tiles_x, tx0 = tile - ty0 * p.tiles_x;
-      const int iy = ty0 * RB_TH - 1 + yy, ix = tx0 * RB_TW - 1 + xx;
-      const bool inside = (iy >= 0) && (iy < p.H) && (ix >= 0) && (ix < p.W);
-      tc::mbar_wait(&bar_d1_full[slot], ph);
-      tc::mbar_wait(&bar_mid_empty, (t & 1u) ^ 1u);      // conv2 of the previous tile has consumed the buffer
-      tc::tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)slot * set_stride + (uint32_t)g * p.NB;
+    tc::fence_proxy_async();                           // generic smem writes -> visible to the wgmma operand reads
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+
+    // ---- conv2: tile rows 8g .. 8g + 7 ----
+    float acc2[NB / 2];
+    tc::wgmma_fence();
+    for (int ky = 0; ky < 3; ++ky)
+      for (int kx = 0; kx < 3; ++kx) {
+        const uint64_t bd = tc::desc_sw128(w2_a + (uint32_t)((ky * 3 + kx) * NB * 128));
+        const uint64_t ad = tc::desc_sw128(mid_a + (uint32_t)(((8 * g + ky) * RB_P + kx) * 128), RB_P * 128);
 #pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        if (c * 16 >= p.NB) break;
-        uint32_t r[16];
-        tc::tmem_ld16(taddr + c * 16, r);
-        tc::tmem_ld_wait();
-        if (!row_ok) continue;
-        uint4 lo, hi;
-        T* tl = reinterpret_cast<T*>(&lo);
-        T* th = reinterpret_cast<T*>(&hi);
+        for (int k = 0; k < 4; ++k)
+          if (k < p.ksteps) tc::wgmma<NB, BF>(acc2, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (ky | kx | k) ? 1u : 0u);
+      }
+    tc::wgmma_commit();
+    tc::wgmma_wait<0>();
+    // ---- epilogue 2: + bias + residual from the input box -> NHWC ----
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          float a = __uint_as_float(r[j]) + bias1_s[c * 16 + j];
-          float b = __uint_as_float(r[8 + j]) + bias1_s[c * 16 + 8 + j];
-          a = fmaxf(a, a * p.mid_slope);
-          b = fmaxf(b, b * p.mid_slope);
-          tl[j] = from_f<T>(inside ? a : 0.f);
-          th[j] = from_f<T>(inside ? b : 0.f);
-        }
-        // 16-byte chunk index 2c / 2c+1 of this row, stored at chunk ^ (row % 8)  (SWIZZLE_128B)
-        *reinterpret_cast<uint4*>(dst_row + (((2 * c) ^ sw) << 4)) = lo;
-        *reinterpret_cast<uint4*>(dst_row + (((2 * c + 1) ^ sw) << 4)) = hi;
-      }
-      tc::fence_proxy_async();          // generic-proxy smem writes -> visible to the tensor core (async proxy)
-      tc::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        tc::mbar_arrive(&bar_mid_full);
-        tc::mbar_arrive(&bar_d1_empty[slot]);
-      }
-    }
-  } else {
-    // ===================== epilogue 2: D2 + bias + skip -> global =====================
-    const int q = warp & 3;
-    const int m2 = q * 32 + lane;
-    const int ty = m2 >> 3, tx = m2 & 7;
-    const int res_row = (ty + 2) * RB_P + tx + 2;        // input box pixel under this output pixel
-    const int rsw = res_row & 7;
-    T* out = reinterpret_cast<T*>(p.out);
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    uint32_t t = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++t) {
-      const int slot = t & 1;
-      const uint32_t ph = (t >> 1) & 1u;
-      const int ty0 = tile / p.tiles_x, tx0 = tile - ty0 * p.tiles_x;
+    for (int r2 = 0; r2 < 2; ++r2) {
+      const int m2 = 64 * g + 16 * wq + (lane >> 2) + 8 * r2;
+      const int ty = m2 >> 3, tx = m2 & 7;
       const int oy = ty0 * RB_TH + ty, ox = tx0 * RB_TW + tx;
-      const bool valid = (oy < p.H) && (ox < p.W);
-      const size_t pix = (size_t)oy * p.W + ox;
-      const uint8_t* res_src = smIn + (size_t)slot * RB_IN_BYTES + (size_t)res_row * 128;
-      tc::mbar_wait(&bar_in_full[slot], ph);     // acquire the TMA-written box (already complete; skip connection)
-      tc::mbar_wait(&bar_d2_full[slot], ph);
-      tc::tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)slot * set_stride + 2u * p.NB;
+      if (oy >= p.H || ox >= p.W) continue;
+      const int rrow = (ty + 2) * RB_P + tx + 2;
 #pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        if (c * 16 >= p.NB) break;
-        uint32_t r[16];
-        tc::tmem_ld16(taddr + c * 16, r);
-        tc::tmem_ld_wait();
-        const int n0 = c * 16;
-        if (!valid || n0 >= p.cout) continue;
-        const uint4 rlo = *reinterpret_cast<const uint4*>(res_src + (((2 * c) ^ rsw) << 4));
-        const uint4 rhi = *reinterpret_cast<const uint4*>(res_src + (((2 * c + 1) ^ rsw) << 4));
-        const T* xl = reinterpret_cast<const T*>(&rlo);
-        const T* xh = reinterpret_cast<const T*>(&rhi);
-        float v[16];
+      for (int j = 0; j < NB / 8; ++j) {
+        const int n = 8 * j + 2 * (lane & 3);
+        if (n >= p.cout) break;
+        const T* rs = reinterpret_cast<const T*>(smIn + sw128_off(rrow, n));
+        float v[2];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          float a = __uint_as_float(r[j]) + bias2_s[n0 + j] + to_f(xl[j]);
-          float b = __uint_as_float(r[8 + j]) + bias2_s[n0 + 8 + j] + to_f(xh[j]);
-          v[j] = fmaxf(a, a * p.post_slope);
-          v[8 + j] = fmaxf(b, b * p.post_slope);
+        for (int e = 0; e < 2; ++e) {
+          const float x = acc2[4 * j + 2 * r2 + e] + b2_s[n + e] + to_f(rs[e]);
+          v[e] = fmaxf(x, x * p.post_slope);
         }
-        if (n0 + 16 <= p.cout && p.vec_ok) {
-          uint4 o0, o1;
-          T* t0 = reinterpret_cast<T*>(&o0);
-          T* t1 = reinterpret_cast<T*>(&o1);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) { t0[j] = from_f<T>(v[j]); t1[j] = from_f<T>(v[8 + j]); }
-          uint4* o = reinterpret_cast<uint4*>(out + pix * p.out_cs + n0);
-          o[0] = o0;
-          o[1] = o1;
+        T* o = out + ((size_t)oy * p.W + ox) * p.out_cs + n;
+        if (p.pair_ok && n + 1 < p.cout) {
+          T pr[2] = {from_f<T>(v[0]), from_f<T>(v[1])};
+          *reinterpret_cast<uint32_t*>(o) = *reinterpret_cast<uint32_t*>(pr);
         } else {
-#pragma unroll
-          for (int j = 0; j < 16; ++j)
-            if (n0 + j < p.cout) out[pix * p.out_cs + n0 + j] = from_f<T>(v[j]);
+          o[0] = from_f<T>(v[0]);
+          if (n + 1 < p.cout) o[1] = from_f<T>(v[1]);
         }
-      }
-      tc::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        tc::mbar_arrive(&bar_d2_empty[slot]);
-        tc::mbar_arrive(&bar_in_empty[slot]);      // skip connection read: the input box may be overwritten
       }
     }
+    __syncthreads();                                   // input box and intermediate are free for the next tile
   }
-
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tc::tmem_dealloc(tmem_base, p.tmem_cols);
-}
-
-template <typename T>
-static int launch_rb(const CUtensorMap& tm, const RbP& p, int grid, size_t smem, cudaStream_t st) {
-  auto kern = conv_rb_kernel<T>;
-  static size_t configured = 0;
-  if (smem > configured) {
-    RV_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured = smem;
-  }
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(448);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  static const bool use_pdl = getenv("REFVSR_NO_PDL") == nullptr;
-  cfg.attrs = attr;
-  cfg.numAttrs = use_pdl ? 1 : 0;
-  RV_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tm, p));
-  RV_LAUNCH_CHECK("conv_rb");
-  return RV_OK;
 }
 
 }  // namespace rv
@@ -339,6 +199,7 @@ extern "C" int rv_resblock(const rv_resblock_desc* d, void* stream) {
   RV_REQUIRE(d->nb % 16 == 0 && d->nb >= 16 && d->nb <= 64 && d->nb >= d->cout, "rv_resblock: nb=%d", d->nb);
   RV_REQUIRE(d->H > 0 && d->W > 0, "rv_resblock: bad geometry");
   RV_REQUIRE(((uintptr_t)d->src % 16 == 0) && ((uintptr_t)d->w1 % 16 == 0) && ((uintptr_t)d->w2 % 16 == 0), "rv_resblock: 16-byte alignment");
+  RV_REQUIRE(d->act_mid != RV_ACT_CLAMP3 && d->act_post != RV_ACT_CLAMP3, "rv_resblock: clamp3 not supported");
   static int num_sms = 0, max_smem = 0;
   if (num_sms == 0) {
     int dev = 0;
@@ -349,20 +210,15 @@ extern "C" int rv_resblock(const rv_resblock_desc* d, void* stream) {
   RbP p;
   p.H = d->H; p.W = d->W; p.C = d->c; p.cout = d->cout; p.NB = d->nb;
   p.tiles_x = (d->W + RB_TW - 1) / RB_TW; p.tiles_y = (d->H + RB_TH - 1) / RB_TH;
-  p.fmt = d->dtype == RV_BF16 ? 1 : 0;
+  p.ksteps = (d->c + 15) / 16;      // K slices of the input (conv1) and of the intermediate (conv2; zero weights beyond cout)
   p.w_bytes = 9u * (uint32_t)p.NB * 128u;
   p.w1 = (const uint8_t*)d->w1; p.w2 = (const uint8_t*)d->w2; p.b1 = d->b1; p.b2 = d->b2;
   auto slope = [](int act) { return act == RV_ACT_RELU ? 0.f : act == RV_ACT_LRELU01 ? 0.1f : act == RV_ACT_LRELU02 ? 0.2f : 1.f; };
-  RV_REQUIRE(d->act_mid != RV_ACT_CLAMP3 && d->act_post != RV_ACT_CLAMP3, "rv_resblock: clamp3 not supported");
   p.mid_slope = slope(d->act_mid); p.post_slope = slope(d->act_post);
   p.out = d->out; p.out_cs = d->out_cs;
-  p.vec_ok = ((uintptr_t)d->out % 16 == 0) && ((d->out_cs * 2) % 16 == 0);
-  uint32_t cols = 32;
-  while (cols < 6u * p.NB) cols <<= 1;
-  p.tmem_cols = cols;
-  // + 4 KB slack after the intermediate: conv1's garbage M rows (216..255) read up to 26 rows past their tile
-  const size_t smem = 1024 + 2 * (size_t)p.w_bytes + 2 * (size_t)RB_IN_BYTES + RB_MID_BYTES + 4096;
-  RV_REQUIRE(smem + 4096 <= (size_t)max_smem, "rv_resblock: %zu bytes of shared memory do not fit", smem);
+  p.pair_ok = ((uintptr_t)d->out % 4 == 0) && (d->out_cs % 2 == 0);
+  const size_t smem = 1024 + 2 * (size_t)p.w_bytes + RB_IN_BYTES + RB_MID_BYTES;
+  RV_REQUIRE(smem <= (size_t)max_smem, "rv_resblock: %zu bytes of shared memory do not fit", smem);
   PFN_tmapEncodeTiled enc = get_tmap_encoder();
   if (!enc) return fail(RV_E_CUDA, "cuTensorMapEncodeTiled entry point not available");
   CUtensorMap tm;
@@ -370,12 +226,24 @@ extern "C" int rv_resblock(const rv_resblock_desc* d, void* stream) {
   cuuint64_t gstr[2] = {(cuuint64_t)d->c * 2, (cuuint64_t)d->W * d->c * 2};
   cuuint32_t box[3] = {64, (cuuint32_t)RB_P, (cuuint32_t)RB_IN_ROWS};
   cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(&tm, p.fmt ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3,
+  CUresult r = enc(&tm, d->dtype == RV_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3,
                    const_cast<void*>(d->src), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(RV_E_CUDA, "cuTensorMapEncodeTiled(resblock) failed (%d)", (int)r);
-  const int ntiles = p.tiles_x * p.tiles_y;
-  const int grid = std::min(ntiles, num_sms);
-  if (d->dtype == RV_F16) return launch_rb<__half>(tm, p, grid, smem, (cudaStream_t)stream);
-  return launch_rb<__nv_bfloat16>(tm, p, grid, smem, (cudaStream_t)stream);
+  const int grid = std::min(p.tiles_x * p.tiles_y, num_sms);
+  cudaStream_t st = (cudaStream_t)stream;
+  static size_t configured[2][4] = {};
+  const int ki = d->dtype == RV_BF16 ? 1 : 0, ni = p.NB / 16 - 1;
+  void (*const kerns[2][4])(CUtensorMap, RbP) = {
+      {conv_rb_kernel<__half, 16>, conv_rb_kernel<__half, 32>, conv_rb_kernel<__half, 48>, conv_rb_kernel<__half, 64>},
+      {conv_rb_kernel<__nv_bfloat16, 16>, conv_rb_kernel<__nv_bfloat16, 32>, conv_rb_kernel<__nv_bfloat16, 48>,
+       conv_rb_kernel<__nv_bfloat16, 64>}};
+  void (*kern)(CUtensorMap, RbP) = kerns[ki][ni];
+  if (smem > configured[ki][ni]) {
+    RV_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    configured[ki][ni] = smem;
+  }
+  kern<<<grid, 256, smem, st>>>(tm, p);
+  RV_LAUNCH_CHECK("conv_rb");
+  return RV_OK;
 }

@@ -1,5 +1,5 @@
 // CUDA-core implicit-GEMM convolution with the same fused prologue/epilogue contract as the
-// tcgen05 path (conv_tc.cu).  It is the geometry-complete implementation (any kernel size, stride,
+// wgmma path (conv_tc.cu).  It is the geometry-complete implementation (any kernel size, stride,
 // channel count, dtype incl. fp32) and the numerical yardstick the tensor-core kernel is tested
 // against on the GPU.  fp32 accumulation in the reference's k-order (ky, kx, c).
 //

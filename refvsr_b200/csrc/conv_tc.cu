@@ -1,23 +1,22 @@
-// tcgen05 / TMEM implicit-GEMM convolution for NHWC f16/bf16 activations (stride 1, "same"-style
-// zero padding), the tensor-core implementation of rv_conv2d.
+// wgmma implicit-GEMM convolution for NHWC f16/bf16 activations (stride 1, "same"-style zero padding), the
+// tensor-core implementation of rv_conv2d (sm_90a).
 //
-// GEMM view per CTA tile: M = 128 output pixels, N = NB output channels (3 * NB in the kx-folded mode), K = taps x
-// 64-channel chunks of src0|src1 in UMMA_K = 16 steps.  There is no im2col buffer:
+// GEMM view per CTA tile: M = 128 output pixels, N = NB output channels, K = taps x 64-channel chunks of src0|src1 in
+// K = 16 steps.  There is no im2col buffer:
 //   * A operand: TMA box loads of the tile + halo, 64 channels wide.  TMA's out-of-bounds zero fill implements the
 //     convolution's zero padding and the channel padding to 64.  The box lands in shared memory as 128-byte pixel rows
-//     with the 128B swizzle, i.e. directly in the canonical K-major UMMA layout, and the taps are row-shifted
-//     descriptor views of it (the swizzle is a pure function of the shared-memory address, so any view that starts
-//     on a 128-byte row is valid with base_offset 0 - measured, profiles/r01_umma_base_offset_experiment.log).
-//     Layout 0: one box per (kx, chunk), tile 8 x 16; layout 1 (default): ONE box per (tile, chunk), tile 16 x 8,
-//     all kh x kw taps are views; MODE 3: tile 4 x 30 on a 4 x 32 grid, kx folded into N (see the kernel comment).
+//     with the 128B swizzle, i.e. directly in the canonical K-major wgmma layout, and the taps are row-shifted
+//     descriptor views of it.
+//     MODE 0: one box per (kx, chunk), tile 8 x 16 (y-halo only; tap views start on 1024-byte swizzle atoms);
+//     MODE 1: ONE box per (tile, chunk), tile 16 x 8, all kh x kw taps are views (layouts 1 and 3 of the weights);
+//     MODE 2: 32B-swizzled 16-channel quads per kx, one K = 16 slice per row (layout 2).
 //   * B operand: weights pre-packed on the host in exactly the swizzled shared-memory image, fetched with plain bulk
-//     copies; resident for the whole CTA lifetime when they fit, otherwise streamed through the same ring as A.
-//   * D: fp32 accumulators in TMEM (3 or 6 buffers).  Persistent CTAs walk the tile list round-robin.
-// Warp roles (512 threads): warp 0 = TMA producer, warps 1-3 = MMA issuers (alternate tiles; warp-uniform control flow,
-// an elected lane issues - see tc::elect_one), warps 4-15 = three epilogue groups of four warps; group g drains the
-// tiles t = g, g + 3, ... (tcgen05.ld -> bias/act/gate/residual -> NHWC or pixel-shuffled store).  setmaxnreg moves
-// registers from the four role warps (40) to the epilogue warps (152).  How this shape was arrived at, with device
-// timelines and knock-outs: profiles/r01_conv_timeline.md.
+//     copies; resident for the whole CTA lifetime when they fit, otherwise streamed through the ring with A.
+//   * D: fp32 accumulators in the registers of the consumer warpgroup (two m64nNk16 halves of the 128-pixel tile).
+// Warp roles (384 threads): warp 0 = TMA producer (warps 1-3 idle), warpgroups 1 and 2 = consumers.  Consumer c owns the
+// CTA's local tiles c, c + 2, ... and its own ring of shared-memory slots, so one consumer's MMAs overlap the other's
+// epilogue (bias / act / gate / residual / act / NHWC or pixel-shuffled store straight from the accumulator registers).
+#include <algorithm>
 #include <cstdlib>
 
 #include "common.cuh"
@@ -26,974 +25,282 @@
 namespace rv {
 
 static constexpr int TH = 8, TW = 16;
-static constexpr int MAX_SLOTS = 8;
-static constexpr int NACC = 3;      // epilogue warp groups
-static constexpr int MAX_MMA = 3;   // MMA-issuing warps (warps 1..3; warp 0 = TMA producer, warps 4..15 = epilogue)
-static constexpr int MAX_ACC = 6;   // TMEM accumulator buffers in flight (p.nacc = 3 or 6): the MMA warp may run this many
-                                    // tiles ahead of the epilogue groups; an accumulator is busy for MMA time + epilogue time
+static constexpr int NCONS = 2;      // consumer warpgroups
+static constexpr int MAX_SLOTS = 6;  // ring slots per consumer
+static constexpr int MAX_NB = 96;
 
 struct TcP {
   int Ho, Wo, kh, kw, pad;
   int nch0, nch1, c0, c1;
   int S, NB, cout, tiles_x, tiles_y, slots, resident;
-  uint32_t a_bytes, w_bytes, a_tx;   // a_tx = bytes one A-stage TMA box delivers (<= a_bytes, the slot pitch)
+  uint32_t a_bytes, w_bytes, a_tx, slot_bytes;   // a_tx = bytes one A-stage TMA load delivers (<= a_bytes)
+  int th, tw, tw_shift, bw;                      // tile rows / columns, box width in pixels
+  int mode;                                      // 0, 1, 2 (see the file comment)
+  int nq0, nq1;                                  // MODE 2: 16-channel quads of src0 / src1
+  uint32_t q_bytes;                              // MODE 2: bytes of one quad sub-buffer of an A stage
   const uint8_t* wpack;
   const float* bias;
-  float pre_slope, post_slope;   // act(v) = v > 0 ? v : v * slope  (none: 1, relu: 0, lrelu: 0.1 / 0.2)
+  float pre_slope, post_slope;   // act(v) = max(v, v * slope)  (none: 1, relu: 0, lrelu: 0.1 / 0.2)
   int post_clamp3;               // clamp(-3, 3) after everything (AlignedConv2d affine map)
   const void* gate;
   int gate_cs;
   const void* res;
   int res_cs;
   void* out;
-  int out_cs, pixel_shuffle, fmt, vec_ok;
-  uint32_t tmem_cols, acc_stride;
-  // tile geometry: mode 0 = 8 rows x 16 cols, one box per (kx, chunk) stage (y-halo only);
-  //                mode 1 = 16 rows x 8 cols, ONE box per (chunk) stage with x- and y-halo, taps = shifted views
-  int single_box, th, tw, tw_shift, bw;   // bw = box width in pixels (mode 1: tile + halo, mode 3: 32)
-  int bo_force;                           // experiment hook: constant base_offset for kx != 0 taps (-1 = kx)
-  // layout 2: operands staged with SWIZZLE_32B in 16-channel quads (32-byte rows): one UMMA_K = 16 slice is a
-  // whole row (built to test an operand over-fetch hypothesis; measured no faster, kept as a validated variant)
-  int nacc;                               // accumulator buffers in TMEM (3 or 6)
-  int fold;                               // mode 3: the 3 kx taps folded into N = 3 * NB (see conv_tc_kernel MODE 3)
-  int fast;                               // streamlined epilogue (all-16-bit, vector stores, full 16-channel chunks)
-  int colsplit;                           // fast epilogue, NB = 48: the three groups share a tile, one 16-column chunk each (1 every tile, 2 the CTA's last)
-  int vlast;                              // 16-byte vectors of the LAST 16-column chunk that exist in memory (2, or 1 when cout = NB - 8)
-  int nmma;                               // MMA-issuing warps in use (1..MAX_MMA), tiles dealt round-robin
-  int grp;                                // consecutive stages that share one full/empty barrier pair (1 or S)
-  int sw32, nq0, nq1;
-  uint32_t q_bytes;                       // bytes of one quad sub-buffer of an A stage
-  long long* trace;                       // experiment hook: device timeline buffer (REFVSR_CONV_TRACE=<ptr>)
-  int dbg;                                // experiment hook (REFVSR_CONV_DBG): 1 no MMA, 2 no epilogue global traffic,
-                                          // 4 no TMEM loads, 8 no TMA box loads
+  int out_cs, pixel_shuffle, pair_ok, fmt;
 };
 
-template <typename T>
-__device__ __forceinline__ void load16(const T* p, float v[16], bool vec) {
-  if (vec) {
-    if constexpr (sizeof(T) == 2) {
-      uint4 a = __ldg(reinterpret_cast<const uint4*>(p));
-      uint4 b = __ldg(reinterpret_cast<const uint4*>(p) + 1);
-      const T* ta = reinterpret_cast<const T*>(&a);
-      const T* tb = reinterpret_cast<const T*>(&b);
+// All MMAs of one pipeline stage into both 64-row halves.  Descriptor start addresses are in 16-byte units: +2 per
+// K = 16 slice of a 128-byte row, whole rows per tap.
+template <int MODE, bool BF, int NB>
+__device__ __forceinline__ void issue_stage(const TcP& p, float (&acc)[2][NB / 2], uint32_t a_addr, uint32_t b_addr,
+                                            int s, int ksteps) {
+  if constexpr (MODE == 2) {
+    const int nq = p.nq0 + p.nq1;
+    for (int ky = 0; ky < p.kh; ++ky)
+      for (int qd = 0; qd < nq; ++qd) {
+        const uint64_t bd = tc::desc_sw32(b_addr + (uint32_t)((ky * nq + qd) * NB * 32));
 #pragma unroll
-      for (int i = 0; i < 8; ++i) { v[i] = to_f(ta[i]); v[8 + i] = to_f(tb[i]); }
-    } else {
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        float4 a = __ldg(reinterpret_cast<const float4*>(p) + q);
-        v[4 * q] = a.x; v[4 * q + 1] = a.y; v[4 * q + 2] = a.z; v[4 * q + 3] = a.w;
-      }
-    }
-  } else {
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = to_f(p[i]);
-  }
-}
-
-template <typename T>
-__device__ __forceinline__ void store16(T* p, const float v[16]) {
-  if constexpr (sizeof(T) == 2) {
-    uint4 a, b;
-    T* ta = reinterpret_cast<T*>(&a);
-    T* tb = reinterpret_cast<T*>(&b);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) { ta[i] = from_f<T>(v[i]); tb[i] = from_f<T>(v[8 + i]); }
-    reinterpret_cast<uint4*>(p)[0] = a;
-    reinterpret_cast<uint4*>(p)[1] = b;
-  } else {
-#pragma unroll
-    for (int q = 0; q < 4; ++q)
-      reinterpret_cast<float4*>(p)[q] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-  }
-}
-
-// packed 16-bit pairs <-> fp32 (one F2FP / two bit ops per pair)
-__device__ __forceinline__ uint32_t pack2(float a, float b, __half) {
-  __half2 h = __floats2half2_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
-__device__ __forceinline__ uint32_t pack2(float a, float b, __nv_bfloat16) {
-  __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
-__device__ __forceinline__ float2 unpack2(uint32_t v, __half) { return __half22float2(*reinterpret_cast<__half2*>(&v)); }
-__device__ __forceinline__ float2 unpack2(uint32_t v, __nv_bfloat16) {
-  return make_float2(__uint_as_float(v << 16), __uint_as_float(v & 0xffff0000u));
-}
-__device__ __forceinline__ uint32_t pack2(float, float, float) { return 0; }          // never instantiated on the fast path
-__device__ __forceinline__ float2 unpack2(uint32_t, float) { return make_float2(0.f, 0.f); }
-
-// all MMAs of one pipeline stage: KH vertical taps x ksteps (<= 4) K-slices of 16 channels.  Descriptor
-// start addresses advance by +2 (32 bytes) per K-slice and by one tile row block per tap.
-template <int KH>
-__device__ __forceinline__ void issue_taps(uint32_t d_tmem, uint64_t ad, uint64_t bd, uint32_t idesc, int ksteps,
-                                           uint32_t b_tap, uint32_t acc0, uint32_t alt = 0) {
-#pragma unroll
-  for (int ky = 0; ky < KH; ++ky) {
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      if (k < ksteps) {
-        // alt != 0 (timing experiment only): consecutive MMAs hit different accumulators -> no RAW chain on D
-        // acc0 = 0 only for the first stage of a tile: its first MMA overwrites the accumulator
-        tc::umma_f16(d_tmem + (((ky * 4 + k) % 3) * alt), ad + (uint64_t)(ky * (TW * 128 / 16) + k * 2),
-                     bd + (uint64_t)(ky * b_tap + k * 2), idesc, (ky | k) ? 1u : acc0);
-      }
-    }
-  }
-}
-
-// mode 1: all KH x KW taps of one channel chunk read the same box.  Tap (ky,kx) starts (ky*bw + kx) pixel
-// rows (128 B each) into the box; 8-row groups of the M dimension are bw rows apart (SBO).  The start is
-// then not 1024-byte aligned, which is fine: see the base_offset note below.
-template <int KH>
-__device__ __forceinline__ void issue_taps_box(uint32_t d_tmem, uint64_t ad, uint64_t bd, uint32_t idesc, int ksteps,
-                                               uint32_t b_tap, int bw, int bo_force, uint32_t acc0) {
-#pragma unroll 1
-  for (int ky = 0; ky < KH; ++ky) {
-#pragma unroll
-    for (int kx = 0; kx < KH; ++kx) {
-      // base_offset (bits [49,52)) stays 0: measured on B200, the operand swizzle is a pure function of the
-      // absolute shared-memory address bits, so a view that starts kx rows into a 1024-byte atom reads exactly
-      // what TMA wrote; a non-zero base_offset shifts the XOR phase and corrupts the operand (experiment hook).
-      const int bo = (bo_force >= 0 && kx != 0) ? bo_force : 0;
-      const uint64_t a_tap = ad + (uint64_t)((ky * bw + kx) * 8) + ((uint64_t)bo << 49);
-      const uint64_t b_t = bd + (uint64_t)((ky * KH + kx) * b_tap);
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        if (k < ksteps) {
-          tc::umma_f16(d_tmem, a_tap + (uint64_t)(k * 2), b_t + (uint64_t)(k * 2), idesc, (ky | kx | k) ? 1u : acc0);
+        for (int h = 0; h < 2; ++h) {
+          const uint64_t ad = tc::desc_sw32(a_addr + (uint32_t)(qd * p.q_bytes + (h * 4 + ky) * TW * 32));
+          tc::wgmma<NB, BF>(acc[h], ad, bd, (s | ky | qd) ? 1u : 0u);
         }
       }
+  } else if constexpr (MODE == 1) {
+    const uint32_t sbo = (uint32_t)p.bw * 128;        // 8-row groups of M = consecutive tile rows of the box
+    for (int ky = 0; ky < p.kh; ++ky)
+      for (int kx = 0; kx < p.kw; ++kx) {
+        const uint64_t bd = tc::desc_sw128(b_addr + (uint32_t)((ky * p.kw + kx) * NB * 128));
+        const uint32_t at = a_addr + (uint32_t)((ky * p.bw + kx) * 128);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint64_t ad = tc::desc_sw128(at + (uint32_t)h * 8 * sbo, sbo);
+#pragma unroll
+          for (int k = 0; k < 4; ++k)
+            if (k < ksteps) tc::wgmma<NB, BF>(acc[h], ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (s | ky | kx | k) ? 1u : 0u);
+        }
+      }
+  } else {
+    for (int ky = 0; ky < p.kh; ++ky) {
+      const uint64_t bd = tc::desc_sw128(b_addr + (uint32_t)(ky * NB * 128));
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint64_t ad = tc::desc_sw128(a_addr + (uint32_t)((h * 4 + ky) * TW * 128));
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          if (k < ksteps) tc::wgmma<NB, BF>(acc[h], ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (s | ky | k) ? 1u : 0u);
+      }
     }
   }
 }
 
-// The tiles of one epilogue group, walked without integer divisions: tile index, tile coordinates, and the TMEM
-// accumulator (tile t lives in accumulator t % nacc, phase (t / nacc) & 1; consecutive tiles of a group are NACC apart).
-struct TileIter {
-  int tile, ty, tx, step, dty, dtx;
-  uint32_t acc, accph;
-  __device__ __forceinline__ void init(int first, int step_, int tiles_x, int grp) {
-    tile = first; step = step_;
-    ty = first / tiles_x; tx = first - ty * tiles_x;
-    dty = step_ / tiles_x; dtx = step_ - dty * tiles_x;
-    acc = (uint32_t)grp; accph = 0;
+template <typename T>
+__device__ __forceinline__ float2 ld2(const T* q, bool pair) {
+  if constexpr (sizeof(T) == 2) {
+    if (pair) {
+      if constexpr (std::is_same<T, __half>::value) return __half22float2(*reinterpret_cast<const __half2*>(q));
+      else return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(q));
+    }
+  } else {
+    if (pair) return *reinterpret_cast<const float2*>(q);
   }
-  __device__ __forceinline__ void next(int tiles_x, int nacc) {
-    tile += step; tx += dtx; ty += dty;
-    if (tx >= tiles_x) { tx -= tiles_x; ++ty; }
-    acc += NACC;
-    if (acc >= (uint32_t)nacc) { acc -= (uint32_t)nacc; accph ^= 1u; }
+  return make_float2(to_f(q[0]), 0.f);
+}
+
+template <typename T>
+__device__ __forceinline__ void st2(T* q, float a, float b, bool pair) {
+  if constexpr (sizeof(T) == 2) {
+    if (pair) {
+      if constexpr (std::is_same<T, __half>::value) *reinterpret_cast<__half2*>(q) = __floats2half2_rn(a, b);
+      else *reinterpret_cast<__nv_bfloat162*>(q) = __floats2bfloat162_rn(a, b);
+      return;
+    }
+  } else {
+    if (pair) { *reinterpret_cast<float2*>(q) = make_float2(a, b); return; }
   }
-};
+  q[0] = from_f<T>(a);
+}
 
-// MODE: 0 = 128B-swizzled boxes per (kx, chunk); 1 = single box per (tile, chunk); 2 = 32B-swizzled quads per kx;
-// 3 = "kx-folded" 3x3: tile = 4 rows x 30 columns computed on a 4 x 32 pixel grid (M = 128, one warp per row).  One MMA
-//     per (ky, 16-channel slice) multiplies the grid by the weights of ALL three kx taps at once (N = 3 * NB, the taps
-//     are adjacent row blocks of the layout-1 weight image), so accumulator column block kx of grid pixel b holds the
-//     tap-kx partial sum of INPUT column b; the epilogue adds the three blocks across lanes (out[j] = D0[j] + D1[j+1]
-//     + D2[j+2], two warp shuffles per value).  9 MMAs per tile instead of 27 and the 4 KB A-operand slice is read
-//     from shared memory once per (ky, slice) instead of three times - the SS-mode MMAs of this kernel are bound by
-//     shared-memory operand bandwidth (~55 cycles per N = 48 MMA measured, 24 by tensor math).
-// One instantiation per mode keeps the (register-critical) epilogue free of the other modes' code.
-#ifdef RV_CONV_EXPERIMENTS
-#define RV_DBG(p, bit) ((p).dbg & (bit))
-// kernel-level marks of CTA 0 (role 7): 0 = entry, 1 = prologue done (barriers, TMEM, bias), 2 = exit
-#define RV_MARK(ev)                                                                                \
-  do {                                                                                             \
-    if (p.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) {            \
-      long long* _t = p.trace + ((size_t)7 * 1000 + (ev)) * 3;                                     \
-      _t[0] = (ev); _t[1] = 0; _t[2] = clock64();                                                  \
-    }                                                                                              \
-  } while (0)
-// device-side timeline of CTA 0: role r writes (event, tile, clock64) triples into its own region of p.trace
-#define RV_TRACE(role, ev, tile)                                                                   \
-  do {                                                                                             \
-    if (p.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && tr_n < 1000 && ((threadIdx.x & 31) == 0 || (role) >= 2)) {                 \
-      long long* _t = p.trace + ((size_t)(role) * 1000 + tr_n) * 3;                                \
-      _t[0] = (ev); _t[1] = (tile); _t[2] = clock64(); ++tr_n;                                     \
-    }                                                                                              \
-  } while (0)
-#else
-#define RV_DBG(p, bit) 0
-#define RV_MARK(ev) do { } while (0)
-#define RV_TRACE(role, ev, tile) do { } while (0)
-#endif
-
-template <typename TI, typename TR, typename TO, int MODE, bool PS = false>   // PS: pixel-shuffle stores on the fast epilogue
-__global__ void __launch_bounds__(32 * (1 + MAX_MMA) + 128 * NACC, 1)
-conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1,
-               const TcP p) {
+template <typename TI, typename TR, typename TO, int MODE, int NB>   // NB: output channels per CTA (= p.NB)
+__global__ void __launch_bounds__(128 * (1 + NCONS), 1)
+conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1, const TcP p) {
+  constexpr bool BF = std::is_same<TI, __nv_bfloat16>::value;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ uint64_t bar_full[MAX_SLOTS], bar_empty[MAX_SLOTS], bar_w, bar_tfull[MAX_ACC], bar_tempty[MAX_ACC];
-  __shared__ uint32_t tmem_base_s;
-  __shared__ __align__(16) float bias_s[256];
+  __shared__ uint64_t bar_full[NCONS][MAX_SLOTS], bar_empty[NCONS][MAX_SLOTS], bar_w;
+  __shared__ __align__(16) float bias_s[MAX_NB];
 
   const uint32_t raw = tc::smem_u32(smem_raw);
   uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
-  uint8_t* smemA = smem;
-  uint8_t* smemW = smem + (size_t)p.slots * p.grp * p.a_bytes;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int warp_u = __shfl_sync(0xffffffffu, warp, 0);   // same value, provably warp-uniform for the compiler
+  uint8_t* smemW = smem;                                            // resident weights (S stages)
+  uint8_t* ring = smem + (p.resident ? (size_t)p.S * p.w_bytes : 0);  // consumer c: slots x slot_bytes
+  const int warp = threadIdx.x >> 5;
+  const int warp_u = __shfl_sync(0xffffffffu, warp, 0);
   const int nblk = blockIdx.y;
   const int ntiles = p.tiles_x * p.tiles_y;
   const int nchunks = p.nch0 + p.nch1;
 
-  // Programmatic dependent launch: let the next kernel of the stream start its own prologue as soon as SMs free
-  // up; everything below that reads or writes activations sits behind griddepcontrol.wait, while barrier init,
-  // TMEM allocation, bias and the (constant) weight fetch overlap the previous kernel's tail.
-  RV_MARK(0);
+  // Programmatic dependent launch: the next kernel of the stream may start its prologue now; activations are read and
+  // written only after griddepcontrol.wait, while barrier init, bias and the (constant) weight fetch overlap the tail
+  // of the previous kernel.
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-
-  // barrier init spread over the threads of warp 0 (one slot / accumulator each) instead of ~25 serial inits by thread 0: the
-  // prologue is on every launch's critical path (profiles/r02_trunk_knockout.md)
-  if (threadIdx.x < 32) {
-    const int i = threadIdx.x;
-    if (i < p.slots) {
-      tc::mbar_init(&bar_full[i], 1);
-      tc::mbar_init(&bar_empty[i], 1);
-    }
-    if (i < MAX_ACC) {
-      tc::mbar_init(&bar_tfull[i], 1);
-      tc::mbar_init(&bar_tempty[i], p.colsplit == 1 ? 4 * NACC : 4);      // one arrival per epilogue warp that drains the accumulator
-    }
-    if (i == 31) {
-      tc::mbar_init(&bar_w, 1);
-      tc::prefetch_tmap(&tm0);
-      if (p.nch1) tc::prefetch_tmap(&tm1);
-    }
+  if (threadIdx.x == 0) {
+    for (int c = 0; c < NCONS; ++c)
+      for (int i = 0; i < p.slots; ++i) {
+        tc::mbar_init(&bar_full[c][i], 1);
+        tc::mbar_init(&bar_empty[c][i], 4);   // one arrival per consumer warp
+      }
+    tc::mbar_init(&bar_w, 1);
     tc::fence_barrier_init();
+    tc::prefetch_tmap(&tm0);
+    if (p.nch1 || p.nq1) tc::prefetch_tmap(&tm1);
   }
-  if (warp == 1 + MAX_MMA) tc::tmem_alloc(&tmem_base_s, p.tmem_cols);
   for (int i = threadIdx.x; i < p.NB; i += blockDim.x) {
-    int n = nblk * p.NB + i;
+    const int n = nblk * p.NB + i;
     bias_s[i] = (n < p.cout) ? p.bias[n] : 0.f;
   }
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem_base = tmem_base_s;
-  RV_MARK(1);
-
-  // Register re-balancing (512 threads x 128 registers at launch): the four single-thread role warps (warpgroup 0)
-  // hand registers to the three epilogue warpgroups, whose 16-column drain + prefetch loop otherwise spills.
-  if (warp_u < 1 + MAX_MMA) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
-  else asm volatile("setmaxnreg.inc.sync.aligned.u32 152;" ::: "memory");
 
   if (warp_u == 0) {
     // ============================ TMA producer ============================
-    // warp-uniform control flow (all lanes wait on the barriers), one elected lane issues the copies
-    {
-      const uint8_t* wsrc = p.wpack + (size_t)nblk * p.S * p.w_bytes;
-      if (p.resident && tc::elect_one()) {
-        tc::mbar_expect_tx(&bar_w, (uint32_t)p.S * p.w_bytes);
-        for (int s = 0; s < p.S; ++s)
-          tc::bulk_load(wsrc + (size_t)s * p.w_bytes, &bar_w, smemW + (size_t)s * p.w_bytes, p.w_bytes);
-      }
-      __syncwarp();
-      asm volatile("griddepcontrol.wait;" ::: "memory");   // activations of the previous kernel are now visible
-      const uint32_t tx_bytes = p.a_tx + (p.resident ? 0u : p.w_bytes);
-      int slot = 0;
-      uint32_t ph = 0;
-      int tr_n = 0; (void)tr_n;
-      int ty0 = blockIdx.x / p.tiles_x, tx0 = blockIdx.x - ty0 * p.tiles_x;   // tile coordinates, advanced incrementally
-      const int dty = gridDim.x / p.tiles_x, dtx = gridDim.x - dty * p.tiles_x;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-        const int yc = ty0 * p.th - p.pad, xc = tx0 * p.tw - p.pad;
-        int kx = 0, ch = 0;
-        for (int s = 0, sub = 0; s < p.S; ++s) {
-          RV_TRACE(0, 0, tile);
-          if (sub == 0) tc::mbar_wait(&bar_empty[slot], ph ^ 1u);
-          RV_TRACE(0, 1, tile);
-          if (tc::elect_one()) {
-            if (RV_DBG(p, 8)) {
-              if (sub + 1 == p.grp) tc::mbar_arrive(&bar_full[slot]);
-            } else {
-              if (sub == 0) tc::mbar_expect_tx(&bar_full[slot], tx_bytes * (uint32_t)p.grp);
-              uint8_t* dstA = smemA + ((size_t)slot * p.grp + sub) * p.a_bytes;
-              if constexpr (MODE == 2) {
-                // stage = kx; one 16-channel box per quad of src0 | src1
-                for (int qd = 0; qd < p.nq0 + p.nq1; ++qd) {
-                  if (qd < p.nq0)
-                    tc::tma_load_3d(&tm0, &bar_full[slot], dstA + (size_t)qd * p.q_bytes, qd * 16, xc + kx, yc);
-                  else
-                    tc::tma_load_3d(&tm1, &bar_full[slot], dstA + (size_t)qd * p.q_bytes, (qd - p.nq0) * 16, xc + kx, yc);
-                }
-              } else {
-                if (ch < p.nch0)
-                  tc::tma_load_3d(&tm0, &bar_full[slot], dstA, ch * 64, xc + kx, yc);
-                else
-                  tc::tma_load_3d(&tm1, &bar_full[slot], dstA, (ch - p.nch0) * 64, xc + kx, yc);
-              }
-              if (!p.resident)
-                tc::bulk_load(wsrc + (size_t)s * p.w_bytes, &bar_full[slot], smemW + (size_t)slot * p.w_bytes, p.w_bytes);
-            }
-          }
-          __syncwarp();
-          // stage order: mode 0 = (kx, chunk), mode 1 = (chunk), mode 2 = (kx)
-          if (MODE == 2) ++kx;
-          else if (++ch == nchunks) { ch = 0; kx += (MODE == 1 || MODE == 3) ? 0 : 1; }
-          if (++sub == p.grp) {
-            sub = 0;
-            if (++slot == p.slots) { slot = 0; ph ^= 1u; }
-          }
-        }
-        tx0 += dtx; ty0 += dty;
-        if (tx0 >= p.tiles_x) { tx0 -= p.tiles_x; ++ty0; }
-      }
+    const uint8_t* wsrc = p.wpack + (size_t)nblk * p.S * p.w_bytes;
+    if (p.resident && tc::elect_one()) {
+      tc::mbar_expect_tx(&bar_w, (uint32_t)p.S * p.w_bytes);
+      for (int s = 0; s < p.S; ++s) tc::bulk_load(wsrc + (size_t)s * p.w_bytes, &bar_w, smemW + (size_t)s * p.w_bytes, p.w_bytes);
     }
-  } else if (warp_u < 1 + MAX_MMA) {
-    // ============================ MMA issuers ==============================
-    // Device timelines (profiles/r01_conv_timeline.md) show the issuing THREAD is the critical resource of this
-    // kernel: every tcgen05.mma holds it ~140 cycles while the tensor pipe and the epilogue groups idle.  So up to
-    // MAX_MMA warps issue, each owning the local tiles id, id + nmma, ... (own smem slots, own TMEM accumulator);
-    // the tensor pipe interleaves the independent instruction streams.  Per thread the stream is kept minimal:
-    // descriptors are 64-bit bases plus small immediates, the tap loop is unrolled per kernel height.
-    const int id = warp_u - 1;
-    // warp-uniform control flow: all 32 lanes run the loop, an elected lane issues (see tc::umma_f16_elect)
-    if (id < p.nmma) {
-      const uint32_t idesc = tc::umma_idesc(p.fmt, 128, (MODE == 3) ? 3 * p.NB : p.NB);
-      // SBO (bits [32,46)): 1024 B between 8-row groups in mode 0, bw*128 B (next tile row) in mode 1
-      const uint64_t adesc0 = (MODE == 2) ? tc::umma_desc_sw32(tc::smem_u32(smemA))
-                                          : tc::umma_desc_sw128(tc::smem_u32(smemA)) +
-                                                ((MODE == 1) ? ((uint64_t)((p.bw * 128 - 1024) >> 4) << 32) : 0ull);
-      // (mode 3: the 4 x 32 grid rows are contiguous in the box, 8-row groups 1024 B apart like mode 0)
-      const uint64_t bdesc0 = (MODE == 2) ? tc::umma_desc_sw32(tc::smem_u32(smemW)) : tc::umma_desc_sw128(tc::smem_u32(smemW));
-      const uint32_t a_step = p.a_bytes >> 4, w_step = p.w_bytes >> 4, b_tap = (uint32_t)(p.NB * 128) >> 4;
-      const uint32_t ngrp = (uint32_t)(p.S / p.grp);   // barrier groups (smem slots) per tile: 1 or S
-      if (p.resident) tc::mbar_wait(&bar_w, 0);
-      int tr_n = 0; (void)tr_n;
-      const int trole = (id == 0) ? 1 : 4 + id; (void)trole;
-      uint32_t tl = (uint32_t)id;
-      for (int tile = blockIdx.x + id * gridDim.x; tile < ntiles; tile += p.nmma * gridDim.x, tl += (uint32_t)p.nmma) {
-        const uint32_t g0 = tl * ngrp;
-        int slot = (int)(g0 % (uint32_t)p.slots);
-        uint32_t ph = (g0 / (uint32_t)p.slots) & 1u;
-        const uint32_t acc = tl % (uint32_t)p.nacc, accph = (tl / (uint32_t)p.nacc) & 1u;
-        RV_TRACE(trole, 0, tile);
-        tc::mbar_wait(&bar_tempty[acc], accph ^ 1u);
-        tc::tc_fence_after();
-        RV_TRACE(trole, 1, tile);
-        const uint32_t d_tmem = tmem_base + acc * p.acc_stride;
-        int ch = 0;
-        for (int s = 0, sub = 0; s < p.S; ++s) {
-          const int crem = (ch < p.nch0) ? (p.c0 - ch * 64) : (p.c1 - (ch - p.nch0) * 64);
-          const int ksteps = (min(crem, 64) + 15) >> 4;
-          const uint32_t abuf = (uint32_t)(slot * p.grp + sub);
-          const uint64_t ad = adesc0 + (uint64_t)(abuf * a_step);
-          const uint64_t bd = bdesc0 + (uint64_t)((uint32_t)(p.resident ? s : slot) * w_step);
-          if (sub == 0) {
-            tc::mbar_wait(&bar_full[slot], ph);
-            tc::tc_fence_after();
-          }
-          RV_TRACE(trole, 2, tile);
-          if (tc::elect_one()) {
-          if (RV_DBG(p, 1)) {
-          } else if constexpr (MODE == 2) {
-            const int nq = p.nq0 + p.nq1;
-            const uint32_t q_step = p.q_bytes >> 4, bq = (uint32_t)(p.NB * 32) >> 4;
-            for (int ky = 0; ky < p.kh; ++ky)
-              for (int qd = 0; qd < nq; ++qd) {
-                tc::umma_f16(d_tmem, ad + (uint64_t)(qd * q_step + ky * (TW * 32 / 16)), bd + (uint64_t)((ky * nq + qd) * bq),
-                             idesc, (s | ky | qd) ? 1u : 0u);
-              }
-          } else if constexpr (MODE == 3) {
-            // stage = channel chunk; A view for tap row ky starts ky grid rows (32 pixels = 4096 B) into the box
-#pragma unroll
-            for (int ky = 0; ky < 3; ++ky)
-#pragma unroll
-              for (int k = 0; k < 4; ++k)
-                if (k < ksteps)
-                  tc::umma_f16(d_tmem, ad + (uint64_t)(ky * 256 + k * 2), bd + (uint64_t)(ky * 3 * b_tap + k * 2), idesc,
-                               (s | ky | k) ? 1u : 0u);
-          } else if constexpr (MODE == 1) {
-            switch (p.kh) {
-              case 1: issue_taps_box<1>(d_tmem, ad, bd, idesc, ksteps, b_tap, p.bw, p.bo_force, s ? 1u : 0u); break;
-              case 3: issue_taps_box<3>(d_tmem, ad, bd, idesc, ksteps, b_tap, p.bw, p.bo_force, s ? 1u : 0u); break;
-              case 5: issue_taps_box<5>(d_tmem, ad, bd, idesc, ksteps, b_tap, p.bw, p.bo_force, s ? 1u : 0u); break;
-              default: issue_taps_box<7>(d_tmem, ad, bd, idesc, ksteps, b_tap, p.bw, p.bo_force, s ? 1u : 0u); break;
+    __syncwarp();
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    const uint32_t tx_bytes = p.a_tx + (p.resident ? 0u : p.w_bytes);
+    int slot[NCONS] = {0, 0};
+    uint32_t ph[NCONS] = {0u, 0u};
+    int cons = 0;
+    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+      const int ty0 = tile / p.tiles_x, tx0 = tile - ty0 * p.tiles_x;
+      const int yc = ty0 * p.th - p.pad, xc = tx0 * p.tw - p.pad;
+      int kx = 0, ch = 0;
+      for (int s = 0; s < p.S; ++s) {
+        const int sl = slot[cons];
+        tc::mbar_wait(&bar_empty[cons][sl], ph[cons] ^ 1u);
+        if (tc::elect_one()) {
+          uint64_t* bar = &bar_full[cons][sl];
+          uint8_t* dst = ring + ((size_t)cons * p.slots + sl) * p.slot_bytes;
+          tc::mbar_expect_tx(bar, tx_bytes);
+          if constexpr (MODE == 2) {
+            for (int qd = 0; qd < p.nq0 + p.nq1; ++qd) {
+              if (qd < p.nq0) tc::tma_load_3d(&tm0, bar, dst + (size_t)qd * p.q_bytes, qd * 16, xc + kx, yc);
+              else tc::tma_load_3d(&tm1, bar, dst + (size_t)qd * p.q_bytes, (qd - p.nq0) * 16, xc + kx, yc);
             }
           } else {
-            switch (p.kh) {
-              case 1: issue_taps<1>(d_tmem, ad, bd, idesc, ksteps, b_tap, s ? 1u : 0u); break;
-              case 3: issue_taps<3>(RV_DBG(p, 16) ? tmem_base : d_tmem, ad, bd, idesc, ksteps, b_tap, s ? 1u : 0u, RV_DBG(p, 16) ? p.acc_stride : 0); break;
-              case 5: issue_taps<5>(d_tmem, ad, bd, idesc, ksteps, b_tap, s ? 1u : 0u); break;
-              case 7: issue_taps<7>(d_tmem, ad, bd, idesc, ksteps, b_tap, s ? 1u : 0u); break;
-              default:
-                for (int ky = 0; ky < p.kh; ++ky)
-                  for (int k = 0; k < ksteps; ++k) {
-                    tc::umma_f16(d_tmem, ad + (uint64_t)(ky * (TW * 128 / 16) + k * 2), bd + (uint64_t)(ky * b_tap + k * 2), idesc, (s | ky | k) ? 1u : 0u);
-                  }
-            }
+            if (ch < p.nch0) tc::tma_load_3d(&tm0, bar, dst, ch * 64, xc + kx, yc);
+            else tc::tma_load_3d(&tm1, bar, dst, (ch - p.nch0) * 64, xc + kx, yc);
           }
-          if (sub + 1 == p.grp) tc::umma_commit(&bar_empty[slot]);   // frees the smem slot when these MMAs retire
-          if (s + 1 == p.S) tc::umma_commit(&bar_tfull[acc]);        // accumulator complete -> epilogue group
-          }
-          __syncwarp();
-          RV_TRACE(trole, 3, tile);
-          if (++ch == nchunks) ch = 0;
-          if (++sub == p.grp) {
-            sub = 0;
-            if (++slot == p.slots) { slot = 0; ph ^= 1u; }
-          }
+          if (!p.resident) tc::bulk_load(wsrc + (size_t)s * p.w_bytes, bar, dst + p.a_bytes, p.w_bytes);
         }
-        RV_TRACE(trole, 5, tile);
+        __syncwarp();
+        // stage order: mode 0 = (kx, chunk), mode 1 = (chunk), mode 2 = (kx)
+        if (MODE == 2) ++kx;
+        else if (++ch == nchunks) { ch = 0; kx += (MODE == 1) ? 0 : 1; }
+        if (++slot[cons] == p.slots) { slot[cons] = 0; ph[cons] ^= 1u; }
       }
+      if (++cons == NCONS) cons = 0;
     }
-  } else {
-    // ============================ epilogue ================================
-    const int grp = (warp - 1 - MAX_MMA) >> 2;  // accumulator buffer / tile parity owned by this group
-    const int q = warp & 3;           // TMEM lane quarter this warp may access
-    const int m = q * 32 + lane;
-    const int ty = m >> p.tw_shift, tx = m & (p.tw - 1);
+  } else if (warp_u >= 4) {
+    // ============================ consumers ================================
+    const int cons = (warp_u >> 2) - 1;
+    const int t = threadIdx.x & 127, wq = t >> 5, lane = t & 31;
     const TI* gate = reinterpret_cast<const TI*>(p.gate);
     const TR* res = reinterpret_cast<const TR*>(p.res);
     TO* out = reinterpret_cast<TO*>(p.out);
-    const float pre_slope = p.pre_slope, post_slope = p.post_slope;
+    const uint32_t ring_addr = tc::smem_u32(ring + (size_t)cons * p.slots * p.slot_bytes);
+    const uint32_t w_addr = tc::smem_u32(smemW);
+    if (p.resident) tc::mbar_wait(&bar_w, 0);
     asm volatile("griddepcontrol.wait;" ::: "memory");     // gate / residual reads and all stores come after this
-    constexpr int PRE = 3;  // chunks whose residual / gate vectors are prefetched before the accumulator wait
-    // group g drains local tiles t = g, g + 3, g + 6, ...; tile t lives in accumulator t % nacc
-    uint32_t tl = (uint32_t)grp;
-    int tr_n = (q == 0 && lane == 0) ? 0 : 1000000; (void)tr_n;
-    if constexpr (MODE == 3 && sizeof(TI) == 2 && sizeof(TR) == 2 && sizeof(TO) == 2) {
-      // ---- kx-folded tile: warp q = grid row, lane = grid column b (input column tile_x0 - pad + b) ----
-      const int nch = p.NB >> 4;
-      const int act_pre = (pre_slope == 1.f) ? 0 : (pre_slope == 0.f ? 1 : 2);
-      const int act_post = (post_slope == 1.f) ? 0 : (post_slope == 0.f ? 1 : 2);
-      // Residual vectors are fetched ONE TILE AHEAD: once the epilogue (not the MMAs) paces the kernel the accumulator
-      // is already complete when a group comes back for its next tile, so a prefetch issued just before the tfull wait
-      // hides nothing and the L2 / HBM latency of the 96-byte-strided loads lands on the critical path.
-      const int nbase = nblk * p.NB;
-      auto tile_pixel = [&](const TileIter& it, bool& valid) -> size_t {
-        const int oy = it.ty * p.th + q, ox = it.tx * p.tw + lane;
-        valid = (it.tile < ntiles) && (lane < p.tw) && (oy < p.Ho) && (ox < p.Wo);
-        return valid ? (size_t)oy * p.Wo + ox : 0;
-      };
-      uint4 rp[3][2], rn[3][2];                 // residual vectors of the current / next tile
-      auto fetch_res = [&](size_t pix, uint4 (&dst)[3][2]) {
-        if (res != nullptr) {
-#pragma unroll
-          for (int c = 0; c < 3; ++c)
-            if (c < nch) {
-              const uint4* q4 = reinterpret_cast<const uint4*>(res + pix * p.res_cs + nbase + c * 16);
-              dst[c][0] = __ldg(q4);
-              dst[c][1] = (c + 1 < nch || p.vlast == 2) ? __ldg(q4 + 1) : make_uint4(0, 0, 0, 0);
-            }
+    int slot = 0;
+    uint32_t ph = 0;
+    float acc[2][NB / 2];
+    for (int tile = blockIdx.x + cons * gridDim.x; tile < ntiles; tile += NCONS * gridDim.x) {
+      int ch = 0, prev = -1;
+      for (int s = 0; s < p.S; ++s) {
+        int ksteps = 4;
+        if (MODE != 2) {
+          const int crem = (ch < p.nch0) ? (p.c0 - ch * 64) : (p.c1 - (ch - p.nch0) * 64);
+          ksteps = (min(crem, 64) + 15) >> 4;
+          if (++ch == nchunks) ch = 0;
         }
-      };
-      TileIter it;
-      it.init(blockIdx.x + grp * gridDim.x, NACC * gridDim.x, p.tiles_x, grp);
-      {
-        bool v0;
-        fetch_res(tile_pixel(it, v0), rn);
-      }
-      for (; it.tile < ntiles; it.next(p.tiles_x, p.nacc)) {
-        const int tile = it.tile; (void)tile;
-        const uint32_t acc = it.acc, accph = it.accph;
-        bool valid, valid_next;
-        const size_t pix = tile_pixel(it, valid);
-#pragma unroll
-        for (int c = 0; c < 3; ++c) { rp[c][0] = rn[c][0]; rp[c][1] = rn[c][1]; }
-        TileIter nx = it;
-        nx.next(p.tiles_x, p.nacc);
-        fetch_res(tile_pixel(nx, valid_next), rn);
-        RV_TRACE(2 + grp, 0, tile);
-        tc::mbar_wait(&bar_tfull[acc], accph);
-        tc::tc_fence_after();
-        RV_TRACE(2 + grp, 1, tile);
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * p.acc_stride;
-#pragma unroll
-        for (int c = 0; c < 3; ++c) {          // 9 * NB <= 512 -> at most 3 chunks; unrolled so rp[] stays in registers
-          if (c >= nch) break;
-          const int n0 = c * 16;
-          uint32_t d0[16], d1[16], d2[16];
-          tc::tmem_ld16(taddr + (uint32_t)n0, d0);
-          tc::tmem_ld16(taddr + (uint32_t)(p.NB + n0), d1);
-          tc::tmem_ld16(taddr + (uint32_t)(2 * p.NB + n0), d2);
-          tc::tmem_ld_wait();
-          if (c + 1 == nch) {
-            tc::tc_fence_before();
-            __syncwarp();
-            if (lane == 0) tc::mbar_arrive(&bar_tempty[acc]);
-          }
-          RV_TRACE(2 + grp, 2, tile);
-          float v[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const float s1 = __shfl_down_sync(0xffffffffu, __uint_as_float(d1[j]), 1);
-            const float s2 = __shfl_down_sync(0xffffffffu, __uint_as_float(d2[j]), 2);
-            v[j] = (__uint_as_float(d0[j]) + s1) + (s2 + bias_s[n0 + j]);
-          }
-          if (act_pre == 1) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f);
-          } else if (act_pre == 2) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], v[j] * pre_slope);
-          }
-          if (gate != nullptr) {
-            const uint4* g4 = reinterpret_cast<const uint4*>(gate + pix * p.gate_cs + nbase + n0);
-            const uint4 ga = __ldg(g4), gb = (c + 1 < nch || p.vlast == 2) ? __ldg(g4 + 1) : make_uint4(0, 0, 0, 0);
-            const uint32_t gw[8] = {ga.x, ga.y, ga.z, ga.w, gb.x, gb.y, gb.z, gb.w};
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float2 g2 = unpack2(gw[j], TI());
-              v[2 * j] *= g2.x;
-              v[2 * j + 1] *= g2.y;
-            }
-          }
-          if (res != nullptr) {
-            uint4 ra, rb;
-            if (c < 3) { ra = rp[c < 3 ? c : 0][0]; rb = rp[c < 3 ? c : 0][1]; }
-            else {
-              const uint4* q4 = reinterpret_cast<const uint4*>(res + pix * p.res_cs + nbase + n0);
-              ra = __ldg(q4); rb = (c + 1 < nch || p.vlast == 2) ? __ldg(q4 + 1) : make_uint4(0, 0, 0, 0);
-            }
-            const uint32_t rw[8] = {ra.x, ra.y, ra.z, ra.w, rb.x, rb.y, rb.z, rb.w};
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float2 r2 = unpack2(rw[j], TR());
-              v[2 * j] += r2.x;
-              v[2 * j + 1] += r2.y;
-            }
-          }
-          if (act_post == 1) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f);
-          } else if (act_post == 2) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], v[j] * post_slope);
-          }
-          if (p.post_clamp3) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = fminf(fmaxf(v[j], -3.f), 3.f);
-          }
-          if (valid) {
-            uint4 o0, o1;
-            o0.x = pack2(v[0], v[1], TO()); o0.y = pack2(v[2], v[3], TO()); o0.z = pack2(v[4], v[5], TO()); o0.w = pack2(v[6], v[7], TO());
-            o1.x = pack2(v[8], v[9], TO()); o1.y = pack2(v[10], v[11], TO()); o1.z = pack2(v[12], v[13], TO()); o1.w = pack2(v[14], v[15], TO());
-            uint4* o = reinterpret_cast<uint4*>(out + pix * p.out_cs + nbase + n0);
-            o[0] = o0;
-            if (c + 1 < nch || p.vlast == 2) o[1] = o1;
-          }
-        }
-        RV_TRACE(2 + grp, 3, tile);
-      }
-      tl = 0x7fffffffu;
-    } else if constexpr (sizeof(TI) == 2 && sizeof(TR) == 2 && sizeof(TO) == 2) {
-      if (p.fast) {
-        // ---- fast path: 16-bit in / residual / out, NB = 16 * nch full chunks, 32-byte vector accesses ----
-        // The generic loop below costs ~450 SASS instructions per 16-column chunk (runtime layout / tail handling);
-        // with only 3 epilogue warps per scheduler that made the EPILOGUE the pacing stage once the MMA issue was
-        // fixed (profiles/r01_conv_timeline.md).  Here: all TMEM loads of a tile in flight at once, packed
-        // conversions, uniform branches hoisted out of the per-value loops.
-        const int nch = p.NB >> 4;
-        const int act_pre = (pre_slope == 1.f) ? 0 : (pre_slope == 0.f ? 1 : 2);
-        const int act_post = (post_slope == 1.f) ? 0 : (post_slope == 0.f ? 1 : 2);
-        // p.colsplit (NB = 48): 1 = every tile of the CTA, 2 = only its LAST tile is drained by all three groups together, one
-        // 16-column chunk each (second block below); the per-tile loop here then stops before that tile
-        const int ntl = (ntiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;     // local tiles of this CTA (>= 1)
-        const int last_tile = (int)blockIdx.x + (ntl - 1) * (int)gridDim.x;
-        const int split = PS ? 0 : p.colsplit;
-        const int tile_end = (split == 1) ? 0 : (split == 2 ? last_tile : ntiles);
-        // residual vectors are fetched one tile ahead (see the MODE 3 branch above)
-        const int nbase = nblk * p.NB;
-        auto tile_pixel = [&](const TileIter& it, bool& valid) -> size_t {
-          const int oy = it.ty * p.th + ty, ox = it.tx * p.tw + tx;
-          valid = (it.tile < tile_end) && (oy < p.Ho) && (ox < p.Wo);
-          return valid ? (size_t)oy * p.Wo + ox : 0;          // out-of-image lanes read pixel 0, never store
-        };
-        uint4 rp[3][2], rn[3][2];               // residual vectors of the current / next tile
-        auto fetch_res = [&](size_t pix, uint4 (&dst)[3][2]) {
-          if (RV_DBG(p, 128)) {
-#pragma unroll
-            for (int c = 0; c < 3; ++c) dst[c][0] = dst[c][1] = make_uint4(0, 0, 0, 0);
-          } else if (res != nullptr) {
-#pragma unroll
-            for (int c = 0; c < 3; ++c)
-              if (c < nch) {
-                const uint4* q4 = reinterpret_cast<const uint4*>(res + pix * p.res_cs + nbase + c * 16);
-                dst[c][0] = __ldg(q4);
-                dst[c][1] = (c + 1 < nch || p.vlast == 2) ? __ldg(q4 + 1) : make_uint4(0, 0, 0, 0);
-              }
-          }
-        };
-        TileIter it;
-        it.init(blockIdx.x + grp * gridDim.x, NACC * gridDim.x, p.tiles_x, grp);
-        {
-          bool v0;
-          fetch_res(tile_pixel(it, v0), rn);
-        }
-        for (; it.tile < tile_end; it.next(p.tiles_x, p.nacc)) {
-          const int tile = it.tile; (void)tile;
-          const uint32_t acc = it.acc, accph = it.accph;
-          bool valid, valid_next;
-          const size_t pix = tile_pixel(it, valid);
-#pragma unroll
-          for (int c = 0; c < 3; ++c) { rp[c][0] = rn[c][0]; rp[c][1] = rn[c][1]; }
-          TileIter nx = it;
-          nx.next(p.tiles_x, p.nacc);
-          fetch_res(tile_pixel(nx, valid_next), rn);
-          RV_TRACE(2 + grp, 0, tile);
-          tc::mbar_wait(&bar_tfull[acc], accph);
-          tc::tc_fence_after();
-          RV_TRACE(2 + grp, 1, tile);
-          const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * p.acc_stride;
-          // pixel shuffle: the (a, b) sub-pixel of this thread's pixel receives channels c = n / 4; one 16-n chunk gives it
-          // 4 channels = 8 bytes.  All chunks are packed into ob[] first so each sub-pixel row is written as whole
-          // 16-byte vectors (complete 32-byte sectors) instead of 8-byte pieces.
-          uint32_t ob[PS ? 4 : 1][PS ? 12 : 1];
-          (void)ob;
-#pragma unroll
-          for (int bb = 0; bb < 2; ++bb) {       // NB <= 96: at most two batches of three 16-column chunks
-            const int c3 = bb * 3;
-            if (c3 >= nch) break;
-            uint32_t r[3][16];
-#pragma unroll
-            for (int c = 0; c < 3; ++c)
-              if (c3 + c < nch) tc::tmem_ld16(taddr + (uint32_t)(c3 + c) * 16, r[c]);
-            tc::tmem_ld_wait();
-            if (c3 + 3 >= nch) {
-              // accumulator fully in registers: hand it back to the MMA warps before the arithmetic and the stores
-              tc::tc_fence_before();
-              __syncwarp();
-              if (lane == 0) tc::mbar_arrive(&bar_tempty[acc]);
-            }
-            RV_TRACE(2 + grp, 2, tile);
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-              if (c3 + c >= nch) break;
-              const int n0 = (c3 + c) * 16;
-              float v[16];
-#pragma unroll
-              for (int j = 0; j < 16; j += 4) {
-                const float4 b4 = RV_DBG(p, 32) ? make_float4(0.f, 0.f, 0.f, 0.f) : *reinterpret_cast<const float4*>(&bias_s[n0 + j]);
-                v[j] = __uint_as_float(r[c][j]) + b4.x;
-                v[j + 1] = __uint_as_float(r[c][j + 1]) + b4.y;
-                v[j + 2] = __uint_as_float(r[c][j + 2]) + b4.z;
-                v[j + 3] = __uint_as_float(r[c][j + 3]) + b4.w;
-              }
-              if (act_pre == 1) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f);
-              } else if (act_pre == 2) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], v[j] * pre_slope);
-              }
-              if (gate != nullptr) {
-                const uint4* g4 = reinterpret_cast<const uint4*>(gate + pix * p.gate_cs + nbase + n0);
-                const uint4 ga = __ldg(g4), gb = (c3 + c + 1 < nch || p.vlast == 2) ? __ldg(g4 + 1) : make_uint4(0, 0, 0, 0);
-                const uint32_t gw[8] = {ga.x, ga.y, ga.z, ga.w, gb.x, gb.y, gb.z, gb.w};
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  const float2 g2 = unpack2(gw[j], TI());
-                  v[2 * j] *= g2.x;
-                  v[2 * j + 1] *= g2.y;
-                }
-              }
-              if (res != nullptr) {
-                uint4 ra, rb;
-                if (c3 == 0) { ra = rp[c][0]; rb = rp[c][1]; }
-                else {
-                  const uint4* q4 = reinterpret_cast<const uint4*>(res + pix * p.res_cs + nbase + n0);
-                  ra = __ldg(q4); rb = (c3 + c + 1 < nch || p.vlast == 2) ? __ldg(q4 + 1) : make_uint4(0, 0, 0, 0);
-                }
-                const uint32_t rw[8] = {ra.x, ra.y, ra.z, ra.w, rb.x, rb.y, rb.z, rb.w};
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                  const float2 r2 = unpack2(rw[j], TR());
-                  v[2 * j] += r2.x;
-                  v[2 * j + 1] += r2.y;
-                }
-              }
-              if (act_post == 1) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f);
-              } else if (act_post == 2) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], v[j] * post_slope);
-              }
-              if (p.post_clamp3) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) v[j] = fminf(fmaxf(v[j], -3.f), 3.f);
-              }
-              if (valid && !RV_DBG(p, 64)) {
-                if constexpr (PS) {
-                  // n = 4c + 2a + b: value v[4 * cc + ab] is channel (n0 / 4 + cc) of sub-pixel ab
-#pragma unroll
-                  for (int ab = 0; ab < 4; ++ab) {
-                    ob[ab][2 * (bb * 3 + c)] = pack2(v[ab], v[4 + ab], TO());
-                    ob[ab][2 * (bb * 3 + c) + 1] = pack2(v[8 + ab], v[12 + ab], TO());
-                  }
-                } else {
-                  uint4 o0, o1;
-                  o0.x = pack2(v[0], v[1], TO()); o0.y = pack2(v[2], v[3], TO()); o0.z = pack2(v[4], v[5], TO()); o0.w = pack2(v[6], v[7], TO());
-                  o1.x = pack2(v[8], v[9], TO()); o1.y = pack2(v[10], v[11], TO()); o1.z = pack2(v[12], v[13], TO()); o1.w = pack2(v[14], v[15], TO());
-                  uint4* o = reinterpret_cast<uint4*>(out + pix * p.out_cs + nbase + n0);
-                  o[0] = o0;
-                  if (c3 + c + 1 < nch || p.vlast == 2) o[1] = o1;
-                }
-              }
-            }
-          }
-          if constexpr (PS) {
-            if (valid && !RV_DBG(p, 64)) {
-              const int oy = it.ty * p.th + ty, ox = it.tx * p.tw + tx;
-#pragma unroll
-              for (int ab = 0; ab < 4; ++ab) {
-                TO* o = out + ((size_t)(2 * oy + (ab >> 1)) * (2 * p.Wo) + (2 * ox + (ab & 1))) * p.out_cs + (nbase >> 2);
-#pragma unroll
-                for (int k = 0; k < 3; ++k)          // 2 chunks = 8 channels = 16 bytes per vector
-                  if (2 * k + 1 < nch) reinterpret_cast<uint4*>(o)[k] = make_uint4(ob[ab][4 * k], ob[ab][4 * k + 1], ob[ab][4 * k + 2], ob[ab][4 * k + 3]);
-              }
-            }
-          }
-          RV_TRACE(2 + grp, 3, tile);
-        }
-        if (split != 0) {
-        // ---- column-split tiles (NB = 48, the C -> C convs of the propagation trunks and of RAP) ----
-        // All three groups drain the same tile, group g the 16-column chunk g: a warp handles 32 pixels x 16 channels (one
-        // tcgen05.ld.x16, 32 bytes of residual, 32 bytes of output per thread).  Same values as the per-tile loop above; what
-        // changes is the latency of that tile's epilogue (~1/3): the LAST tile of the CTA no longer keeps one group busy for
-        // ~1.8k cycles while the other two idle (7 tiles per CTA, ~10 us per launch: profiles/r02_trunk_knockout.md).  Splitting
-        // EVERY tile (split == 1) was measured slower (10.3 vs 9.8 us per trunk conv): three times the per-tile fixed work.
-        const int n0 = grp * 16;
-        const int nbase = nblk * p.NB + n0;
-        float bias_r[16];
-#pragma unroll
-        for (int j = 0; j < 16; j += 4) {
-          const float4 b4 = RV_DBG(p, 32) ? make_float4(0.f, 0.f, 0.f, 0.f) : *reinterpret_cast<const float4*>(&bias_s[n0 + j]);
-          bias_r[j] = b4.x; bias_r[j + 1] = b4.y; bias_r[j + 2] = b4.z; bias_r[j + 3] = b4.w;
-        }
-        // local tiles 0, 1, 2, ... of this CTA: tile t lives in accumulator t % nacc, phase (t / nacc) & 1
-        int tile = (split == 1) ? (int)blockIdx.x : last_tile;
-        int tyi = tile / p.tiles_x, txi = tile - tyi * p.tiles_x;
-        const int dty = gridDim.x / p.tiles_x, dtx = gridDim.x - dty * p.tiles_x;
-        const uint32_t tl0 = (split == 1) ? 0u : (uint32_t)(ntl - 1);
-        uint32_t acc = tl0 % (uint32_t)p.nacc, accph = (tl0 / (uint32_t)p.nacc) & 1u;
-        auto pixel_of = [&](int tl_, int tyy, int txx, bool& valid) -> size_t {
-          const int oy = tyy * p.th + ty, ox = txx * p.tw + tx;
-          valid = (tl_ < ntiles) && (oy < p.Ho) && (ox < p.Wo);
-          return valid ? (size_t)oy * p.Wo + ox : 0;          // out-of-image lanes read pixel 0, never store
-        };
-        uint4 rp0, rp1, rn0 = make_uint4(0, 0, 0, 0), rn1 = make_uint4(0, 0, 0, 0);     // residual of the current / next tile
-        auto fetch_res = [&](size_t pix, uint4& a, uint4& b) {
-          if (RV_DBG(p, 128)) { a = b = make_uint4(0, 0, 0, 0); }
-          else if (res != nullptr) {
-            const uint4* q4 = reinterpret_cast<const uint4*>(res + pix * p.res_cs + nbase);
-            a = __ldg(q4); b = __ldg(q4 + 1);
-          }
-        };
-        {
-          bool v0;
-          fetch_res(pixel_of(tile, tyi, txi, v0), rn0, rn1);
-        }
-        for (; tile < ntiles; tile += gridDim.x) {
-          bool valid, valid_next;
-          const size_t pix = pixel_of(tile, tyi, txi, valid);
-          rp0 = rn0; rp1 = rn1;
-          txi += dtx; tyi += dty;
-          if (txi >= p.tiles_x) { txi -= p.tiles_x; ++tyi; }
-          fetch_res(pixel_of(tile + (int)gridDim.x, tyi, txi, valid_next), rn0, rn1);
-          RV_TRACE(2 + grp, 0, tile);
-          tc::mbar_wait(&bar_tfull[acc], accph);
-          tc::tc_fence_after();
-          RV_TRACE(2 + grp, 1, tile);
-          uint32_t r[16];
-          tc::tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + acc * p.acc_stride + (uint32_t)n0, r);
-          tc::tmem_ld_wait();
-          tc::tc_fence_before();
-          __syncwarp();
-          if (split == 1 && lane == 0) tc::mbar_arrive(&bar_tempty[acc]);     // (nobody waits for the last tile's accumulator)
-          if (++acc == (uint32_t)p.nacc) { acc = 0; accph ^= 1u; }
-          RV_TRACE(2 + grp, 2, tile);
-          float v[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = __uint_as_float(r[j]) + bias_r[j];
-          if (act_pre == 1) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f);
-          } else if (act_pre == 2) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], v[j] * pre_slope);
-          }
-          if (gate != nullptr) {
-            const uint4* g4 = reinterpret_cast<const uint4*>(gate + pix * p.gate_cs + nbase);
-            const uint4 ga = __ldg(g4), gb = __ldg(g4 + 1);
-            const uint32_t gw[8] = {ga.x, ga.y, ga.z, ga.w, gb.x, gb.y, gb.z, gb.w};
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float2 g2 = unpack2(gw[j], TI());
-              v[2 * j] *= g2.x;
-              v[2 * j + 1] *= g2.y;
-            }
-          }
-          if (res != nullptr) {
-            const uint32_t rw[8] = {rp0.x, rp0.y, rp0.z, rp0.w, rp1.x, rp1.y, rp1.z, rp1.w};
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float2 r2 = unpack2(rw[j], TR());
-              v[2 * j] += r2.x;
-              v[2 * j + 1] += r2.y;
-            }
-          }
-          if (act_post == 1) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], 0.f);
-          } else if (act_post == 2) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = fmaxf(v[j], v[j] * post_slope);
-          }
-          if (p.post_clamp3) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[j] = fminf(fmaxf(v[j], -3.f), 3.f);
-          }
-          if (valid && !RV_DBG(p, 64)) {
-            uint4 o0, o1;
-            o0.x = pack2(v[0], v[1], TO()); o0.y = pack2(v[2], v[3], TO()); o0.z = pack2(v[4], v[5], TO()); o0.w = pack2(v[6], v[7], TO());
-            o1.x = pack2(v[8], v[9], TO()); o1.y = pack2(v[10], v[11], TO()); o1.z = pack2(v[12], v[13], TO()); o1.w = pack2(v[14], v[15], TO());
-            uint4* o = reinterpret_cast<uint4*>(out + pix * p.out_cs + nbase);
-            o[0] = o0;
-            o[1] = o1;
-          }
-          RV_TRACE(2 + grp, 3, tile);
-        }
-        }
-        tl = 0x7fffffffu;   // generic loop below is skipped
-      }
-    }
-    for (int tile = (tl == 0x7fffffffu) ? ntiles : blockIdx.x + grp * gridDim.x; tile < ntiles; tile += NACC * gridDim.x, tl += NACC) {
-      const uint32_t acc = tl % (uint32_t)p.nacc, accph = (tl / (uint32_t)p.nacc) & 1u;
-      const int oy = (tile / p.tiles_x) * p.th + ty, ox = (tile % p.tiles_x) * p.tw + tx;
-      const bool valid = (oy < p.Ho) && (ox < p.Wo);
-      const size_t pix = (size_t)oy * p.Wo + ox;
-      // ---- prefetch: one DRAM round trip per tile, overlapped with the MMAs of this tile ----
-      uint4 rp[PRE][2], gp[PRE][2];
-      bool pre_ok[PRE];
-#pragma unroll
-      for (int c = 0; c < PRE; ++c) {
-        const int n0 = nblk * p.NB + c * 16;
-        pre_ok[c] = valid && (c * 16 < p.NB) && (n0 + 16 <= p.cout) && p.vec_ok && !RV_DBG(p, 2);
-        if (pre_ok[c] && res != nullptr && sizeof(TR) == 2) {
-          const uint4* q4 = reinterpret_cast<const uint4*>(res + pix * p.res_cs + n0);
-          rp[c][0] = __ldg(q4);
-          rp[c][1] = __ldg(q4 + 1);
-        }
-        if (pre_ok[c] && gate != nullptr) {
-          const uint4* q4 = reinterpret_cast<const uint4*>(gate + pix * p.gate_cs + n0);
-          gp[c][0] = __ldg(q4);
-          gp[c][1] = __ldg(q4 + 1);
-        }
-      }
-      RV_TRACE(2 + grp, 0, tile);
-      tc::mbar_wait(&bar_tfull[acc], accph);
-      tc::tc_fence_after();
-      RV_TRACE(2 + grp, 1, tile);
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * p.acc_stride;
-#pragma unroll
-      for (int c = 0; c < 6; ++c) {
-        const int c0 = c * 16;
-        if (c0 >= p.NB) break;
-        const int n0 = nblk * p.NB + c0;
-        const bool live = valid && n0 < p.cout && !RV_DBG(p, 2);
-        const bool full = (n0 + 16 <= p.cout);
-        const bool vec = full && p.vec_ok;
-        const bool pre = (c < PRE) && pre_ok[c < PRE ? c : 0];
-        if (RV_DBG(p, 4)) continue;
-        float g[16], rr[16];
-        if (live && gate) {
-          if (pre) {
-            const TI* tg = reinterpret_cast<const TI*>(&gp[c < PRE ? c : 0][0]);
-#pragma unroll
-            for (int j = 0; j < 16; ++j) g[j] = to_f(tg[j]);
-          } else if (vec) {
-            load16<TI>(gate + pix * p.gate_cs + n0, g, true);
-          } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) g[j] = (n0 + j < p.cout) ? to_f(gate[pix * p.gate_cs + n0 + j]) : 0.f;
-          }
-        }
-        if (live && res) {
-          if (pre && sizeof(TR) == 2) {
-            const TR* tr = reinterpret_cast<const TR*>(&rp[c < PRE ? c : 0][0]);
-#pragma unroll
-            for (int j = 0; j < 16; ++j) rr[j] = to_f(tr[j]);
-          } else if (vec) {
-            load16<TR>(res + pix * p.res_cs + n0, rr, true);
-          } else {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) rr[j] = (n0 + j < p.cout) ? to_f(res[pix * p.res_cs + n0 + j]) : 0.f;
-          }
-        }
-        uint32_t r[16];
-        tc::tmem_ld16(taddr + c0, r);
-        tc::tmem_ld_wait();
-        RV_TRACE(2 + grp, 2, tile);
-        if (!live) continue;
-        float v[16];
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          float x = __uint_as_float(r[j]) + bias_s[c0 + j];
-          x = fmaxf(x, x * pre_slope);      // slope in [0,1]: identity / ReLU / LeakyReLU without a select
-          if (gate) x *= g[j];
-          if (res) x += rr[j];
-          x = fmaxf(x, x * post_slope);
-          v[j] = x;
-        }
-        if (p.post_clamp3) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = fminf(fmaxf(v[j], -3.f), 3.f);
-        }
-        if (p.pixel_shuffle) {
-          // n = 4c + 2a + b  ->  out[(2oy+a, 2ox+b)][c]; 16 n's = 4 consecutive c for each (a,b)
-          const int cb = n0 >> 2;
-#pragma unroll
-          for (int ab = 0; ab < 4; ++ab) {
-            const int a = ab >> 1, b = ab & 1;
-            TO* o = out + ((size_t)(2 * oy + a) * (2 * p.Wo) + (2 * ox + b)) * p.out_cs + cb;
-            if (vec && sizeof(TO) == 2) {
-              TO pk[4];
-#pragma unroll
-              for (int cc = 0; cc < 4; ++cc) pk[cc] = from_f<TO>(v[4 * cc + ab]);
-              *reinterpret_cast<uint2*>(o) = *reinterpret_cast<const uint2*>(pk);
-            } else {
-#pragma unroll
-              for (int cc = 0; cc < 4; ++cc)
-                if (n0 + 4 * cc + ab < p.cout) o[cc] = from_f<TO>(v[4 * cc + ab]);
-            }
-          }
-        } else if (vec) {
-          store16<TO>(out + pix * p.out_cs + n0, v);
+        tc::mbar_wait(&bar_full[cons][slot], ph);
+        const uint32_t a_addr = ring_addr + (uint32_t)slot * p.slot_bytes;
+        const uint32_t b_addr = p.resident ? w_addr + (uint32_t)s * p.w_bytes : a_addr + p.a_bytes;
+        tc::wgmma_fence();
+        issue_stage<MODE, BF, NB>(p, acc, a_addr, b_addr, s, ksteps);
+        tc::wgmma_commit();
+        if (p.slots == 1) {
+          // a single slot is refilled only after these MMAs have read it
+          tc::wgmma_wait<0>();
+          if (lane == 0) tc::mbar_arrive(&bar_empty[cons][slot]);
         } else {
+          // the previous stage's MMAs have retired once at most this stage's group is in flight: free its slot
+          tc::wgmma_wait<1>();
+          if (prev >= 0 && lane == 0) tc::mbar_arrive(&bar_empty[cons][prev]);
+          prev = slot;
+        }
+        if (++slot == p.slots) { slot = 0; ph ^= 1u; }
+      }
+      tc::wgmma_wait<0>();
+      if (prev >= 0 && lane == 0) tc::mbar_arrive(&bar_empty[cons][prev]);
+
+      // ---- epilogue: thread t holds rows 64 h + 16 wq + lane / 4 (+ 8) and column pairs 8 j + 2 (lane % 4) ----
+      const int ty0 = tile / p.tiles_x, tx0 = tile - ty0 * p.tiles_x;
 #pragma unroll
-          for (int j = 0; j < 16; ++j)
-            if (n0 + j < p.cout) out[pix * p.out_cs + n0 + j] = from_f<TO>(v[j]);
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int r2 = 0; r2 < 2; ++r2) {
+          const int m = 64 * h + 16 * wq + (lane >> 2) + 8 * r2;
+          const int oy = ty0 * p.th + (m >> p.tw_shift), ox = tx0 * p.tw + (m & (p.tw - 1));
+          if (oy >= p.Ho || ox >= p.Wo) continue;
+          const size_t pix = (size_t)oy * p.Wo + ox;
+#pragma unroll
+          for (int j = 0; j < NB / 8; ++j) {
+            const int nl = 8 * j + 2 * (lane & 3);
+            const int n = nblk * NB + nl;
+            if (n >= p.cout) continue;
+            const bool pair = p.pair_ok && (n + 1 < p.cout);
+            float v[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              float x = acc[h][4 * j + 2 * r2 + e] + bias_s[nl + e];
+              v[e] = fmaxf(x, x * p.pre_slope);     // slope in [0,1]: identity / ReLU / LeakyReLU without a select
+            }
+            if (gate != nullptr) {
+              float2 g = ld2<TI>(gate + pix * p.gate_cs + n, pair);
+              if (!pair && n + 1 < p.cout) g.y = to_f(gate[pix * p.gate_cs + n + 1]);
+              v[0] *= g.x; v[1] *= g.y;
+            }
+            if (res != nullptr) {
+              float2 r = ld2<TR>(res + pix * p.res_cs + n, pair);
+              if (!pair && n + 1 < p.cout) r.y = to_f(res[pix * p.res_cs + n + 1]);
+              v[0] += r.x; v[1] += r.y;
+            }
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              v[e] = fmaxf(v[e], v[e] * p.post_slope);
+              if (p.post_clamp3) v[e] = fminf(fmaxf(v[e], -3.f), 3.f);
+            }
+            if (p.pixel_shuffle) {
+              // n = 4c + 2a + b  ->  out[(2oy+a, 2ox+b)][c]; the pair (n, n+1) is b = 0, 1 of one (c, a)
+              const int cc = n >> 2, a = (n >> 1) & 1;
+              TO* o = out + ((size_t)(2 * oy + a) * (2 * p.Wo) + 2 * ox) * p.out_cs + cc;
+              o[0] = from_f<TO>(v[0]);
+              if (n + 1 < p.cout) o[p.out_cs] = from_f<TO>(v[1]);
+            } else {
+              TO* o = out + pix * p.out_cs + n;
+              st2<TO>(o, v[0], v[1], pair);
+              if (!pair && n + 1 < p.cout) o[1] = from_f<TO>(v[1]);
+            }
+          }
         }
       }
-      RV_TRACE(2 + grp, 3, tile);
-      tc::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&bar_tempty[acc]);
-      RV_TRACE(2 + grp, 4, tile);
     }
   }
-
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 1 + MAX_MMA) tc::tmem_dealloc(tmem_base, p.tmem_cols);
-  RV_MARK(2);
 }
-
-#ifdef RV_WATCHDOG
-}  // namespace rv
-extern "C" int rv_set_watchdog_buffer(void* host_mapped) {
-  unsigned long long* p = (unsigned long long*)host_mapped;
-  return cudaMemcpyToSymbol(rv::tc::rv_wd_buf, &p, sizeof(p)) == cudaSuccess ? 0 : -2;
-}
-namespace rv {
-#endif
 
 PFN_tmapEncodeTiled get_tmap_encoder() {
   static PFN_tmapEncodeTiled fn = nullptr;
@@ -1029,10 +336,10 @@ static int g_max_smem = 0;
 static int g_cta_cap = 0;          // rv_set_conv_cta_cap: upper bound of the persistent grid (0 = one CTA per SM)
 int set_conv_cta_cap(int cap) { const int old = g_cta_cap; g_cta_cap = cap > 0 ? cap : 0; return old; }
 
-template <typename TI, typename TR, typename TO, int MODE, bool PS = false>
+template <typename TI, typename TR, typename TO, int MODE, int NB>
 static int launch_tc_mode(const CUtensorMap& tm0, const CUtensorMap& tm1, const TcP& p, dim3 grid, size_t smem,
-                     cudaStream_t st) {
-  auto kern = conv_tc_kernel<TI, TR, TO, MODE, PS>;
+                          cudaStream_t st) {
+  auto kern = conv_tc_kernel<TI, TR, TO, MODE, NB>;
   static size_t configured = 0;   // per template instantiation
   if (smem > configured) {
     RV_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1040,7 +347,7 @@ static int launch_tc_mode(const CUtensorMap& tm0, const CUtensorMap& tm1, const 
   }
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
-  cfg.blockDim = dim3(32 * (1 + MAX_MMA) + 128 * NACC);
+  cfg.blockDim = dim3(128 * (1 + NCONS));
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
   cudaLaunchAttribute attr[1];
@@ -1054,28 +361,39 @@ static int launch_tc_mode(const CUtensorMap& tm0, const CUtensorMap& tm1, const 
   return RV_OK;
 }
 
-template <typename TI, typename TR, typename TO>
-static int launch_tc(const CUtensorMap& tm0, const CUtensorMap& tm1, const TcP& p, dim3 grid, size_t smem, cudaStream_t st) {
-  if (p.sw32) return launch_tc_mode<TI, TR, TO, 2>(tm0, tm1, p, grid, smem, st);
-  if (p.fold) return launch_tc_mode<TI, TR, TO, 3>(tm0, tm1, p, grid, smem, st);
-  if constexpr (sizeof(TO) == 2) {
-    if (p.fast && p.pixel_shuffle && p.single_box) return launch_tc_mode<TI, TR, TO, 1, true>(tm0, tm1, p, grid, smem, st);
+template <typename TI, typename TR, typename TO, int NB>
+static int launch_tc_nb(const CUtensorMap& tm0, const CUtensorMap& tm1, const TcP& p, dim3 grid, size_t smem, cudaStream_t st) {
+  switch (p.mode) {
+    case 2: return launch_tc_mode<TI, TR, TO, 2, NB>(tm0, tm1, p, grid, smem, st);
+    case 1: return launch_tc_mode<TI, TR, TO, 1, NB>(tm0, tm1, p, grid, smem, st);
+    default: return launch_tc_mode<TI, TR, TO, 0, NB>(tm0, tm1, p, grid, smem, st);
   }
-  if (p.single_box) return launch_tc_mode<TI, TR, TO, 1>(tm0, tm1, p, grid, smem, st);
-  return launch_tc_mode<TI, TR, TO, 0>(tm0, tm1, p, grid, smem, st);
 }
 
-// Everything about a launch that does not need a device: geometry, layout mode, shared-memory ring, accumulators, issuers.
-// (rv_conv2d_tc_plan exposes it so that the ring / issuer invariants are checked on a machine without a GPU.)
+template <typename TI, typename TR, typename TO>
+static int launch_tc(const CUtensorMap& tm0, const CUtensorMap& tm1, const TcP& p, dim3 grid, size_t smem, cudaStream_t st) {
+  switch (p.NB) {
+    case 16: return launch_tc_nb<TI, TR, TO, 16>(tm0, tm1, p, grid, smem, st);
+    case 32: return launch_tc_nb<TI, TR, TO, 32>(tm0, tm1, p, grid, smem, st);
+    case 48: return launch_tc_nb<TI, TR, TO, 48>(tm0, tm1, p, grid, smem, st);
+    case 64: return launch_tc_nb<TI, TR, TO, 64>(tm0, tm1, p, grid, smem, st);
+    case 80: return launch_tc_nb<TI, TR, TO, 80>(tm0, tm1, p, grid, smem, st);
+    default: return launch_tc_nb<TI, TR, TO, 96>(tm0, tm1, p, grid, smem, st);
+  }
+}
+
+// Everything about a launch that does not need a device: geometry, layout mode and the shared-memory rings.
+// (rv_conv2d_tc_plan exposes it so that the ring invariants are checked on a machine without a GPU.)
 static int plan_tc(const rv_conv_desc* d, TcP& p, size_t& smem_out, int& nblk_out) {
   RV_REQUIRE(d->stride == 1, "rv_conv2d(tc): stride must be 1 (got %d)", d->stride);
   RV_REQUIRE(d->in_dtype == RV_F16 || d->in_dtype == RV_BF16, "rv_conv2d(tc): activations must be f16/bf16");
   RV_REQUIRE(d->c0 % 8 == 0 && (!d->src1 || d->c1 % 8 == 0), "rv_conv2d(tc): channel counts must be multiples of 8");
   RV_REQUIRE(((uintptr_t)d->src0 % 16 == 0) && ((uintptr_t)d->src1 % 16 == 0) && ((uintptr_t)d->wpack % 16 == 0),
              "rv_conv2d(tc): src/wpack must be 16-byte aligned");
-  RV_REQUIRE(d->nb >= 16 && d->nb <= 96 && d->nb % 16 == 0, "rv_conv2d(tc): nb=%d must be a multiple of 16 in [16,96]", d->nb);
+  RV_REQUIRE(d->nb >= 16 && d->nb <= MAX_NB && d->nb % 16 == 0, "rv_conv2d(tc): nb=%d must be a multiple of 16 in [16,96]", d->nb);
   RV_REQUIRE(d->kh >= 1 && d->kh <= 7 && d->kw >= 1 && d->kw <= 7, "rv_conv2d(tc): kernel size up to 7x7");
   RV_REQUIRE(!d->pixel_shuffle || d->cout % 4 == 0, "rv_conv2d: pixel_shuffle needs cout %% 4 == 0");
+  RV_REQUIRE(d->layout >= 0 && d->layout <= 3, "rv_conv2d(tc): unknown layout %d", d->layout);
   RV_REQUIRE(g_num_sms > 0 && g_max_smem > 0, "rv_conv2d(tc): device limits not set");
   p.Ho = d->H + 2 * d->pad - d->kh + 1;
   p.Wo = d->W + 2 * d->pad - d->kw + 1;
@@ -1083,57 +401,20 @@ static int plan_tc(const rv_conv_desc* d, TcP& p, size_t& smem_out, int& nblk_ou
   p.kh = d->kh; p.kw = d->kw; p.pad = d->pad;
   p.c0 = d->c0; p.c1 = d->src1 ? d->c1 : 0;
   p.nch0 = (p.c0 + 63) / 64; p.nch1 = (p.c1 + 63) / 64;
+  p.nq0 = p.nq1 = 0; p.q_bytes = 0;
   p.NB = d->nb; p.cout = d->cout;
   const int nblk = (d->cout + p.NB - 1) / p.NB;
-  const size_t budget = (size_t)g_max_smem - 1024 /*alignment*/ - 4096 /*static: barriers, bias*/;
-  { const char* e = getenv("REFVSR_BO_FORCE"); p.bo_force = e ? atoi(e) : -1; }
-  { const char* e = getenv("REFVSR_CONV_DBG"); p.dbg = e ? atoi(e) : 0; }
-  { const char* e = getenv("REFVSR_CONV_TRACE"); p.trace = e ? (long long*)strtoull(e, nullptr, 0) : nullptr; }
-  const int rdt = d->res ? d->res_dtype : d->out_dtype;
-  auto al16 = [](const void* q, int cs, int dt) { return q == nullptr || (((uintptr_t)q % 16 == 0) && ((cs * dtype_size(dt)) % 16 == 0)); };
-  p.vec_ok = al16(d->out, d->out_cs, d->out_dtype) && al16(d->gate, d->gate_cs, d->in_dtype) && al16(d->res, d->res_cs, rdt);
-  static const bool fast_ok = getenv("REFVSR_NO_FAST_EPILOGUE") == nullptr;
-  // (pixel-shuffle outputs: 8-byte stores of 4 channels, so (cout / 4) channels per pixel must keep them 8-byte aligned)
-  const bool ps_ok = !d->pixel_shuffle || ((d->layout == 1 || d->layout == 3) && p.NB % 32 == 0 && p.NB <= 96 && (d->out_cs * 2) % 16 == 0 && d->res == nullptr && d->gate == nullptr && (d->out_cs * 2) % 8 == 0 && ((uintptr_t)d->out % 8) == 0);
-  // cout = NB - 8 with a single column block (the small models' 24-channel maps, NB = 32): the last chunk holds one 16-byte vector
-  // per pixel instead of two; the padding columns compute zeros (zero weights and bias) and are simply not stored / not read
-  const bool ragged_ok = (nblk == 1) && (d->cout == p.NB - 8) && !d->pixel_shuffle && d->out_cs == d->cout &&
-                         (!d->res || d->res_cs == d->cout) && (!d->gate || d->gate_cs == d->cout);
-  p.vlast = (d->cout % p.NB == 0) ? 2 : 1;
-  p.fast = fast_ok && p.vec_ok && ps_ok && (d->cout % p.NB == 0 || ragged_ok) && d->out_dtype != RV_F32 && rdt != RV_F32 &&
-           d->out_dtype == d->in_dtype && rdt == d->in_dtype && (p.dbg & 22) == 0;   // knock-out bits 1 / 8 / 32 / 64 / 128 also work on the fast path, 2 / 4 / 16 need the generic one
-  // mode 1 (single box per tile and chunk) when the whole weight set stays resident next to >= 2 boxes
-  p.single_box = 0; p.sw32 = 0; p.nq0 = p.nq1 = 0; p.q_bytes = 0; p.fold = 0; p.colsplit = 0;
-  if (d->layout == 1 || d->layout == 3) {
+  const size_t budget = (size_t)g_max_smem - 1024 /*alignment*/ - 2048 /*static: barriers, bias*/;
+  p.mode = (d->layout == 1 || d->layout == 3) ? 1 : d->layout;
+  if (p.mode == 1) {
     RV_REQUIRE(d->kh == d->kw && (d->kh == 1 || d->kh == 3 || d->kh == 5 || d->kh == 7), "rv_conv2d(tc): layout 1 needs a square 1/3/5/7 kernel");
-    p.single_box = 1;
-    // mode 3 (kx-folded N = 3 * NB) shares the layout-1 weight image; it needs the streamlined 16-bit epilogue
-    static const bool fold_ok = getenv("REFVSR_NO_KXFOLD") == nullptr;
-    const size_t w_fold = (size_t)(p.nch0 + p.nch1) * 9 * p.NB * 128;
-    // measured (profiles/r01_conv_timeline.md): folding wins where the MMA phase dominates - two 64-channel chunks or
-    // narrow outputs (NB <= 32, where N = NB under-uses each A-operand read most) - and loses on the single-chunk
-    // 48 -> 48 convs, whose epilogue (heavier when folded: 3x TMEM reads + shuffles) already paces the kernel
-    static const bool fold_all = getenv("REFVSR_KXFOLD_ALL") != nullptr;
-    const bool fold_pays = fold_all || (p.nch0 + p.nch1) >= 2 || p.NB <= 32;
-    p.fold = fold_ok && fold_pays && !d->pixel_shuffle && d->layout == 1 && d->kh == 3 && p.fast && p.dbg == 0 && 9 * p.NB <= 512 /* three N = 3 * NB accumulators in TMEM */ && w_fold + 3 * (size_t)(6 * 32 * 128) <= budget;
-  }
-  if (p.fold) {
-    p.th = 4; p.tw = 30; p.tw_shift = 0;
-    p.bw = 32;                           // the 4 x 32 pixel grid of a tile: input columns tile_x0 - pad .. + 31
-    p.S = p.nch0 + p.nch1;
-    p.a_tx = (uint32_t)(p.th + d->kh - 1) * p.bw * 128;
-    p.a_bytes = p.a_tx;
-    p.w_bytes = (uint32_t)d->kh * d->kw * p.NB * 128;
-  } else if (p.single_box) {
     p.th = 16; p.tw = 8; p.tw_shift = 3;
     p.bw = p.tw + d->kw - 1;            // box = tile + halo; rows of the box are bw pixels (bw * 128 B) apart
     p.S = p.nch0 + p.nch1;
     p.a_tx = (uint32_t)(p.th + d->kh - 1) * p.bw * 128;
     p.a_bytes = (p.a_tx + 1023u) & ~1023u;   // slots stay 1024-byte aligned (swizzle atom)
     p.w_bytes = (uint32_t)d->kh * d->kw * p.NB * 128;
-    RV_REQUIRE((size_t)p.S * p.w_bytes + 2 * (size_t)p.a_bytes <= budget, "rv_conv2d(tc): layout 1 weights do not fit in shared memory");
-  } else if (d->layout == 2) {
-    p.sw32 = 1;
+  } else if (p.mode == 2) {
     p.th = TH; p.tw = TW; p.tw_shift = 4; p.bw = TW;
     p.nq0 = (p.c0 + 15) / 16; p.nq1 = (p.c1 + 15) / 16;
     p.S = d->kw;
@@ -1149,31 +430,21 @@ static int plan_tc(const rv_conv_desc* d, TcP& p, size_t& smem_out, int& nblk_ou
     p.w_bytes = (uint32_t)d->kh * p.NB * 128;
   }
   p.tiles_x = (p.Wo + p.tw - 1) / p.tw; p.tiles_y = (p.Ho + p.th - 1) / p.th;
-  {
-    static const int colsplit_mode = getenv("REFVSR_COLSPLIT") ? atoi(getenv("REFVSR_COLSPLIT")) : 0;      // 0 off (default: neither variant paid, see the kernel), 1 all tiles, 2 last tile
-    p.colsplit = (p.fast && !p.fold && !d->pixel_shuffle && p.NB == 16 * NACC && p.vlast == 2) ? colsplit_mode : 0;
-  }
-  // shared-memory plan: weights resident when they leave room for >= 3 A slots
+  // shared-memory plan: weights resident when they leave room for two slots per consumer (layout 1: one), else streamed with
+  // A; a consumer with a single slot still overlaps with the other consumer's ring
   const size_t w_all = (size_t)p.S * p.w_bytes;
-  p.grp = 1;
-  static const bool group_stages = getenv("REFVSR_NO_STAGE_GROUPS") == nullptr;
-  if (group_stages && p.S > 1 && w_all + 2 * (size_t)p.S * p.a_bytes <= budget) {
-    // all stages of a tile behind ONE full / empty barrier pair: the MMA-issuing thread (the serial resource of
-    // the kernel) pays one wait + one tcgen05.commit per tile instead of one per stage
+  if (w_all + (size_t)NCONS * (p.mode == 1 ? 1 : 2) * p.a_bytes <= budget) {
     p.resident = 1;
-    p.grp = p.S;
-    p.slots = (int)std::min<size_t>(MAX_SLOTS, (budget - w_all) / ((size_t)p.S * p.a_bytes));
-  } else if (p.single_box || w_all + 3 * (size_t)p.a_bytes <= budget) {
-    p.resident = 1;
-    p.slots = (int)std::min<size_t>(MAX_SLOTS, (budget - w_all) / p.a_bytes);
+    p.slot_bytes = p.a_bytes;
+    p.slots = (int)std::min<size_t>(MAX_SLOTS, (budget - w_all) / ((size_t)NCONS * p.a_bytes));
   } else {
+    RV_REQUIRE(p.mode != 1, "rv_conv2d(tc): layout 1 weights do not fit in shared memory");
     p.resident = 0;
-    p.slots = (int)std::min<size_t>(MAX_SLOTS, budget / ((size_t)p.a_bytes + p.w_bytes));
-    RV_REQUIRE(p.slots >= 2, "rv_conv2d(tc): stage of %u bytes does not fit twice in shared memory",
-               p.a_bytes + p.w_bytes);
+    p.slot_bytes = p.a_bytes + p.w_bytes;
+    p.slots = (int)std::min<size_t>(MAX_SLOTS, budget / ((size_t)NCONS * p.slot_bytes));
+    RV_REQUIRE(p.slots >= 1, "rv_conv2d(tc): stage of %u bytes does not fit once per consumer in shared memory", p.slot_bytes);
   }
-  if (p.grp == 1) p.slots = std::min(p.slots, std::max(2, p.single_box ? 6 * p.S : 3 * p.S));
-  const size_t smem = 1024 + (size_t)p.slots * p.grp * p.a_bytes + (p.resident ? w_all : (size_t)p.slots * p.w_bytes);
+  const size_t smem = 1024 + (p.resident ? w_all : 0) + (size_t)NCONS * p.slots * p.slot_bytes;
   p.wpack = (const uint8_t*)d->wpack; p.bias = d->bias;
   auto slope = [](int act) { return act == RV_ACT_RELU ? 0.f : act == RV_ACT_LRELU01 ? 0.1f : act == RV_ACT_LRELU02 ? 0.2f : 1.f; };
   RV_REQUIRE(d->act_pre != RV_ACT_CLAMP3, "rv_conv2d(tc): clamp3 is only supported as act_post");
@@ -1181,36 +452,11 @@ static int plan_tc(const rv_conv_desc* d, TcP& p, size_t& smem_out, int& nblk_ou
   p.post_clamp3 = d->act_post == RV_ACT_CLAMP3;
   p.gate = d->gate; p.gate_cs = d->gate_cs; p.res = d->res; p.res_cs = d->res_cs;
   p.out = d->out; p.out_cs = d->out_cs; p.pixel_shuffle = d->pixel_shuffle;
+  // channel pairs (n, n + 1), n even, are one 4- / 8-byte access when every row stride keeps them aligned
+  const int rdt = d->res ? d->res_dtype : d->out_dtype;
+  auto al = [](const void* q, int cs, int dt) { return q == nullptr || (((uintptr_t)q % (2 * dtype_size(dt)) == 0) && cs % 2 == 0); };
+  p.pair_ok = al(d->out, d->out_cs, d->out_dtype) && al(d->gate, d->gate_cs, d->in_dtype) && al(d->res, d->res_cs, rdt);
   p.fmt = d->in_dtype == RV_BF16 ? 1 : 0;
-  p.acc_stride = (uint32_t)(p.fold ? 3 * p.NB : p.NB);
-  uint32_t cols = 32;
-  // accumulator t % nacc must always belong to the same epilogue group (t % 3): nacc is 3 or 6
-  p.nacc = (6 * p.acc_stride <= 512) ? 6 : 3;
-  // Issuers: as many as there are whole tiles in flight in shared memory (and accumulators to write to) - and every issuer
-  // must OWN its smem slots and accumulators.  All waits are mbarrier PARITY waits: a warp that waits for the k-th fill of a
-  // slot passes as soon as the barrier's completed-phase count has the right parity, i.e. also when it is still TWO fills
-  // short.  That cannot happen to the warp that consumed fill k-1 itself, but it does happen to ANOTHER issuer that reaches the
-  // slot `slots` tiles later while the earlier fill (a TMA box with a long-tail latency: cold DRAM page / TLB miss on a
-  // > 100 MB map) is still in flight - it then multiplies stale data, commits, and the barrier phases are off by two for good
-  // (round 2: 48 -> 192 pixel-shuffle conv at 1080x1920, 4 slots / 3 issuers, dead-lock in ~1 of 20 launches;
-  // profiles/r02_8k.md).  With tiles-in-flight and accumulators both multiples of the issuer count, consecutive uses of a slot /
-  // accumulator always belong to the same issuer and the parity wait is exact.
-#ifdef RV_CONV_EXPERIMENTS
-  const int nmma_env = getenv("REFVSR_NMMA") ? atoi(getenv("REFVSR_NMMA")) : 0;          // (re-read per launch: tools/trunk_bench.py)
-#else
-  static const int nmma_env = getenv("REFVSR_NMMA") ? atoi(getenv("REFVSR_NMMA")) : 0;
-#endif
-  {
-    const int unit = (p.grp == p.S) ? 1 : p.S;                 // smem slots (barrier pairs) per tile
-    int tif = p.slots / unit;                                  // whole tiles in flight
-    p.nmma = std::max(1, std::min(std::min((int)MAX_MMA, tif), p.nacc));
-    if (nmma_env > 0) p.nmma = std::min(p.nmma, nmma_env);
-    while (p.nmma > 1 && (p.nacc % p.nmma != 0 || tif / p.nmma == 0)) --p.nmma;
-    if (p.nmma > 1) p.slots = (tif / p.nmma) * p.nmma * unit;     // (a single issuer keeps whatever ring it has, even < 1 tile)
-  }
-  while (cols < (uint32_t)p.nacc * p.acc_stride) cols <<= 1;
-  p.tmem_cols = cols;
-
   smem_out = smem;
   nblk_out = nblk;
   return RV_OK;
@@ -1231,11 +477,12 @@ int conv2d_tc(const rv_conv_desc* d, cudaStream_t st) {
     if (rc0) return rc0;
   }
   const int rdt = d->res ? d->res_dtype : d->out_dtype;
+  const int sw32 = p.mode == 2;
   CUtensorMap tm0, tm1;
-  int rc = make_act_tmap(&tm0, d->src0, p.c0, d->W, d->H, p.bw, p.th + d->kh - 1, p.fmt, p.sw32);
+  int rc = make_act_tmap(&tm0, d->src0, p.c0, d->W, d->H, p.mode == 1 ? p.tw + d->kw - 1 : p.tw, p.th + d->kh - 1, p.fmt, sw32);
   if (rc) return rc;
-  if (p.nch1) {
-    rc = make_act_tmap(&tm1, d->src1, p.c1, d->W, d->H, p.bw, p.th + d->kh - 1, p.fmt, p.sw32);
+  if (p.c1) {
+    rc = make_act_tmap(&tm1, d->src1, p.c1, d->W, d->H, p.mode == 1 ? p.tw + d->kw - 1 : p.tw, p.th + d->kh - 1, p.fmt, sw32);
     if (rc) return rc;
   } else {
     tm1 = tm0;
@@ -1251,8 +498,9 @@ int conv2d_tc(const rv_conv_desc* d, cudaStream_t st) {
   return fail(RV_E_UNSUPPORTED, "rv_conv2d(tc): unsupported dtype combination in=%d res=%d out=%d", d->in_dtype, rdt, d->out_dtype);
 }
 
-// host-only: the launch plan of rv_conv2d (tensor-core path) for given device limits -> out[8] = {mode, slots, grp, S, nmma, nacc,
-// nb, smem bytes}.  mode: 0 boxes per (kx, chunk), 1 single box, 2 32B-swizzled quads, 3 kx-folded.
+// host-only: the launch plan of rv_conv2d (tensor-core path) for given device limits -> out[8] = {mode, slots per consumer,
+// weights resident, S, consumer warpgroups, accumulator sets, nb, smem bytes}.  mode: 0 boxes per (kx, chunk), 1 single box,
+// 2 32B-swizzled quads.
 int conv2d_tc_plan(const rv_conv_desc* d, int max_smem, int num_sms, int* out) {
   const int s0 = g_num_sms, s1 = g_max_smem;
   g_num_sms = num_sms; g_max_smem = max_smem;
@@ -1262,8 +510,8 @@ int conv2d_tc_plan(const rv_conv_desc* d, int max_smem, int num_sms, int* out) {
   const int rc = plan_tc(d, p, smem, nblk);
   g_num_sms = s0; g_max_smem = s1;
   if (rc) return rc;
-  out[0] = p.sw32 ? 2 : (p.fold ? 3 : (p.single_box ? 1 : 0));
-  out[1] = p.slots; out[2] = p.grp; out[3] = p.S; out[4] = p.nmma; out[5] = p.nacc; out[6] = p.NB; out[7] = (int)smem;
+  out[0] = p.mode;
+  out[1] = p.slots; out[2] = p.resident; out[3] = p.S; out[4] = NCONS; out[5] = NCONS; out[6] = p.NB; out[7] = (int)smem;
   return RV_OK;
 }
 

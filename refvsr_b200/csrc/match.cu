@@ -1,8 +1,8 @@
 // LR <-> Ref patch matching: conf[l] = max_r <A[l], B[r]>, idx[l] = argmax_r  (attention.py:83-91)
 // The reference materialises the (R x P) similarity matrix (16.8 GB fp32 at 270x480) and then
-// reduces it; here the GEMM tiles never leave the SM: accumulators live in TMEM and each epilogue
-// thread owns one LR pixel (= one TMEM lane), so the max/argmax over reference patches is a purely
-// thread-local running reduction over the N dimension - no shuffles, no atomics.
+// reduces it; here the GEMM tiles never leave the SM: accumulators live in the registers of the
+// consumer warpgroups and the max/argmax over reference patches is a running reduction over the N
+// dimension, four threads per LR pixel - no atomics.
 //
 // Operands are fp16 rows produced by rv_patch_pack (pre-scaled by 2^6).  In "split" mode each row is
 // [hi|lo|hi] x [hi|hi|lo], which makes the fp16 tensor-core product equal to the fp32 product up to
@@ -82,9 +82,13 @@ __global__ void __launch_bounds__(256) match_simt_kernel(const __half* __restric
 }
 
 // ------------------------------------------------------------------------------------------------
-// tcgen05 streaming argmax GEMM
+// wgmma streaming argmax GEMM
 // ------------------------------------------------------------------------------------------------
-static constexpr int MT_BM = 128, MT_BN = 256, MT_MAXCH = 7, MT_SLOTS_MAX = 6;
+// 384 threads: warp 0 = TMA producer, warpgroups 1 and 2 = consumers, consumer c multiplies LR rows 64 c .. 64 c + 63 of
+// the CTA's 128-row A block (resident in shared memory) by every 128-row B tile streamed through the ring.  Thread t
+// of a consumer holds rows 16 (t / 32) + (t % 32) / 4 (+ 8) and the column pairs 8 j + 2 (t % 4) of the tile: a running
+// max / argmax per row and thread over the N dimension, then the four threads of a row combine theirs (shuffles).
+static constexpr int MT_BM = 128, MT_BN = 128, MT_MAXCH = 7, MT_SLOTS_MAX = 6;
 
 struct MtP {
   int P, R, nk, slots, ntiles_n;
@@ -93,12 +97,11 @@ struct MtP {
   int32_t* idx;
 };
 
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(384, 1)
 match_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                 const MtP p) {
   extern __shared__ uint8_t smem_raw[];
-  __shared__ uint64_t bar_full[MT_SLOTS_MAX], bar_empty[MT_SLOTS_MAX], bar_a, bar_tfull[2], bar_tempty[2];
-  __shared__ uint32_t tmem_base_s;
+  __shared__ uint64_t bar_full[MT_SLOTS_MAX], bar_empty[MT_SLOTS_MAX], bar_a;
   const uint32_t raw = tc::smem_u32(smem_raw);
   uint8_t* smem = smem_raw + (((raw + 1023u) & ~1023u) - raw);
   constexpr uint32_t A_CH = MT_BM * 128, B_ST = MT_BN * 128;
@@ -109,21 +112,14 @@ match_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   const int m0 = blockIdx.x * MT_BM;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < p.slots; ++i) { tc::mbar_init(&bar_full[i], 1); tc::mbar_init(&bar_empty[i], 1); }
+    for (int i = 0; i < p.slots; ++i) { tc::mbar_init(&bar_full[i], 1); tc::mbar_init(&bar_empty[i], 8); }
     tc::mbar_init(&bar_a, 1);
-    for (int i = 0; i < 2; ++i) { tc::mbar_init(&bar_tfull[i], 1); tc::mbar_init(&bar_tempty[i], 4); }
     tc::fence_barrier_init();
     tc::prefetch_tmap(&tmA);
     tc::prefetch_tmap(&tmB);
   }
-  if (warp == 2) tc::tmem_alloc(&tmem_base_s, 512);
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem_base = tmem_base_s;
 
-  // Producer and MMA warps run warp-uniform control flow with one elected lane issuing (tc::elect_one): the compiler
-  // then keeps descriptors / barrier addresses in uniform registers instead of a per-instruction broadcast waterfall.
   if (warp_u == 0) {
     if (tc::elect_one()) {
       tc::mbar_expect_tx(&bar_a, (uint32_t)p.nk * A_CH);
@@ -142,87 +138,59 @@ match_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         __syncwarp();
         if (++slot == p.slots) { slot = 0; ph ^= 1u; }
       }
-  } else if (warp_u == 1) {
-    const uint32_t idesc = tc::umma_idesc(0, MT_BM, MT_BN);
-    const uint64_t adesc0 = tc::umma_desc_sw128(tc::smem_u32(smemA)), bdesc0 = tc::umma_desc_sw128(tc::smem_u32(smemB));
+  } else if (warp_u >= 4) {
+    const int cons = (warp_u >> 2) - 1, wq = warp_u & 3;
+    const uint32_t a0 = tc::smem_u32(smemA) + (uint32_t)cons * 64 * 128, b0 = tc::smem_u32(smemB);
+    float best[2] = {-INFINITY, -INFINITY};
+    int bidx[2] = {0, 0};
+    float acc[MT_BN / 2];
     tc::mbar_wait(&bar_a, 0);
-    int slot = 0;
+    int slot = 0, prev = -1;
     uint32_t ph = 0;
     for (int nt = 0; nt < p.ntiles_n; ++nt) {
-      const uint32_t acc = nt & 1u, accph = (nt >> 1) & 1u;
-      tc::mbar_wait(&bar_tempty[acc], accph ^ 1u);
-      tc::tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * MT_BN;
       for (int c = 0; c < p.nk; ++c) {
         tc::mbar_wait(&bar_full[slot], ph);
-        tc::tc_fence_after();
-        if (tc::elect_one()) {
-          const uint64_t ad = adesc0 + (uint64_t)((uint32_t)c * (A_CH >> 4));
-          const uint64_t bd = bdesc0 + (uint64_t)((uint32_t)slot * (B_ST >> 4));
+        const uint64_t ad = tc::desc_sw128(a0 + (uint32_t)c * A_CH), bd = tc::desc_sw128(b0 + (uint32_t)slot * B_ST);
+        tc::wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < 4; ++k) tc::umma_f16(d_tmem, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), idesc, (c | k) ? 1u : 0u);
-          tc::umma_commit(&bar_empty[slot]);
-          if (c + 1 == p.nk) tc::umma_commit(&bar_tfull[acc]);
-        }
-        __syncwarp();
+        for (int k = 0; k < 4; ++k) tc::wgmma<MT_BN, false>(acc, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (c | k) ? 1u : 0u);
+        tc::wgmma_commit();
+        tc::wgmma_wait<1>();
+        if (prev >= 0 && lane == 0) tc::mbar_arrive(&bar_empty[prev]);
+        prev = slot;
         if (++slot == p.slots) { slot = 0; ph ^= 1u; }
       }
+      tc::wgmma_wait<0>();
+      if (lane == 0) tc::mbar_arrive(&bar_empty[prev]);
+      prev = -1;
+      // columns in increasing order with a strict > keep the earliest maximum of this thread
+      const int rbase = nt * MT_BN + 2 * (lane & 3);
+      const int nvalid = p.R - rbase;
+#pragma unroll
+      for (int j = 0; j < MT_BN / 8; ++j)
+#pragma unroll
+        for (int r2 = 0; r2 < 2; ++r2)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const float v = acc[4 * j + 2 * r2 + e];
+            if (8 * j + e < nvalid && v > best[r2]) { best[r2] = v; bidx[r2] = rbase + 8 * j + e; }
+          }
     }
-  } else {
-    const int q = warp & 3;
-    const int m = m0 + q * 32 + lane;
-    float best = -INFINITY;
-    int bidx = 0;
-    for (int nt = 0; nt < p.ntiles_n; ++nt) {
-      const uint32_t acc = nt & 1u, accph = (nt >> 1) & 1u;
-      tc::mbar_wait(&bar_tfull[acc], accph);
-      tc::tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + acc * MT_BN;
-      const int rbase = nt * MT_BN;
-      const int nvalid = min(MT_BN, p.R - rbase);
-      for (int c0 = 0; c0 < MT_BN; c0 += 32) {
-        uint32_t r[32];
-        tc::tmem_ld32(taddr + c0, r);
-        tc::tmem_ld_wait();
-        if (c0 + 32 <= nvalid) {
-          // chunk maximum first (a tree of independent FMNMX), index search only when it beats the running best:
-          // a serial `if (v > best)` scan is one dependent compare-select chain per element and made this loop,
-          // not the MMAs, the pacing stage in single-pass mode.  Same result: strict > keeps the earliest maximum
-          // across chunks, the search below takes the first position inside the chunk.
-          float m8[8];
 #pragma unroll
-          for (int j = 0; j < 8; ++j)
-            m8[j] = fmaxf(fmaxf(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1])),
-                          fmaxf(__uint_as_float(r[4 * j + 2]), __uint_as_float(r[4 * j + 3])));
-          const float mx = fmaxf(fmaxf(fmaxf(m8[0], m8[1]), fmaxf(m8[2], m8[3])), fmaxf(fmaxf(m8[4], m8[5]), fmaxf(m8[6], m8[7])));
-          if (mx > best) {
-            best = mx;
-            int jj = 31;
+    for (int r2 = 0; r2 < 2; ++r2) {
 #pragma unroll
-            for (int j = 30; j >= 0; --j)
-              if (__uint_as_float(r[j]) == mx) jj = j;
-            bidx = rbase + c0 + jj;
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            float v = __uint_as_float(r[j]);
-            if (c0 + j < nvalid && v > best) { best = v; bidx = rbase + c0 + j; }
-          }
-        }
+      for (int off = 1; off < 4; off <<= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, best[r2], off);
+        const int oi = __shfl_xor_sync(0xffffffffu, bidx[r2], off);
+        if (ov > best[r2] || (ov == best[r2] && oi < bidx[r2])) { best[r2] = ov; bidx[r2] = oi; }
       }
-      tc::tc_fence_before();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&bar_tempty[acc]);
-    }
-    if (m < p.P) {
-      p.conf[m] = best * p.out_scale;
-      p.idx[m] = bidx;
+      const int m = m0 + cons * 64 + 16 * wq + (lane >> 2) + 8 * r2;
+      if ((lane & 3) == 0 && m < p.P) {
+        p.conf[m] = best[r2] * p.out_scale;
+        p.idx[m] = bidx[r2];
+      }
     }
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tc::tmem_dealloc(tmem_base, 512);
 }
 
 static int make_rows_tmap(CUtensorMap* m, const void* ptr, int kpad, int rows, int box_rows) {
@@ -264,7 +232,7 @@ static int match_tc(const void* A, int P, const void* B, int R, int kpad, float 
     RV_CUDA_OK(cudaFuncSetAttribute(match_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     configured = smem;
   }
-  match_tc_kernel<<<cdiv(P, MT_BM), 192, smem, st>>>(tmA, tmB, p);
+  match_tc_kernel<<<cdiv(P, MT_BM), 384, smem, st>>>(tmA, tmB, p);
   RV_LAUNCH_CHECK("match_tc");
   return RV_OK;
 }

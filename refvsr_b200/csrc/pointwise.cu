@@ -10,10 +10,10 @@
 namespace rv {
 
 #ifndef RV_W3_TILE_DEFAULT
-#define RV_W3_TILE_DEFAULT 0     // 8 x 16 pixels: 32.3 us vs 35.0 (4 x 16) / 38.1 (2 x 16): the flow-tile prologue is exposed per CTA
+#define RV_W3_TILE_DEFAULT 0     // 8 x 16 pixels (see launch_warp3 for the measured shapes)
 #endif
 #ifndef RV_AS_TILE_DEFAULT
-#define RV_AS_TILE_DEFAULT 1     // 4 x 16 cells: measured 25.4 us vs 28.2 us (8 x 16) at 270x480x48 bf16, profiles/r02_pointwise_tiles.md
+#define RV_AS_TILE_DEFAULT 1     // 4 x 16 cells: 41.2 us vs 43.0 us (8 x 16) at 270x480x48 bf16 (H100 80GB HBM3, 400 W limit)
 #endif
 
 // ---------------------------------------------------------------------------------------------
@@ -64,10 +64,13 @@ __device__ __forceinline__ void stvi(T* base, int i, const Vec<T, V>& r) {
 
 // ---------------------------------------------------------------------------------------------
 // 4-tap blend of one channel vector: r = a * w.x + b * w.y + c * w.z + d * w.w in fp32, evaluated for every element as
-// fma(d, w.w, fma(c, w.z, fma(b, w.y, a * w.x))).  The gather kernels are issue-bound as much as HBM-bound (ncu: ~65 % issue
-// utilisation), so the arithmetic runs on packed pairs (sm_100 FFMA2: one issue slot per two lanes' worth of FMAs) and the
-// 16-bit <-> fp32 conversions are done on packed words.
+// fma(d, w.w, fma(c, w.z, fma(b, w.y, a * w.x))).  The gather kernels spend many issue slots per byte, so the 16-bit <-> fp32 conversions are done on packed words.  sm_90 has no packed fp32 FMA: each pair is
+// two round-to-nearest FFMAs, the same values a packed instruction gives.
 // ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
 template <typename T>
 __device__ __forceinline__ float2 unpack2(const T* p);
 template <>
@@ -97,10 +100,10 @@ __device__ __forceinline__ Vec<T, V> blend4(const Vec<T, V>& a, const Vec<T, V>&
   Vec<T, V> r;
 #pragma unroll
   for (int k = 0; k < V; k += 2) {
-    float2 acc = __fmul2_rn(unpack2<T>(&a.v[k]), wx);
-    acc = __ffma2_rn(unpack2<T>(&b.v[k]), wy, acc);
-    acc = __ffma2_rn(unpack2<T>(&c.v[k]), wz, acc);
-    acc = __ffma2_rn(unpack2<T>(&d.v[k]), ww, acc);
+    float2 acc = fmul2(unpack2<T>(&a.v[k]), wx);
+    acc = ffma2(unpack2<T>(&b.v[k]), wy, acc);
+    acc = ffma2(unpack2<T>(&c.v[k]), wz, acc);
+    acc = ffma2(unpack2<T>(&d.v[k]), ww, acc);
     pack2<T>(&r.v[k], acc);
   }
   return r;
@@ -1063,7 +1066,7 @@ static int warp_launch(const void* src, int Hi, int Wi, int C, const float* flow
   constexpr int VMAX = 16 / sizeof(T);
   long long px = (long long)(up2 ? 4 : 1) * hf * wf;
   bool aligned = ((uintptr_t)src % 16 == 0) && ((uintptr_t)out % 16 == 0);
-  if (false && C % (2 * VMAX) == 0 && aligned && C / (2 * VMAX) <= 256) {   // 32 B / thread measured slower (40.2 vs 35.6 us)
+  if (false && C % (2 * VMAX) == 0 && aligned && C / (2 * VMAX) <= 256) {   // 32 B / thread variant: disabled
     const int cv = C / (2 * VMAX), ppb = 256 / cv;   // pixels per block, 32 bytes per thread
     warp_vec_kernel<T, VMAX, 2><<<cdiv(px, ppb), 256, 0, st>>>((const T*)src, Hi, Wi, C, flow, hf, wf, up2, (T*)out, ppb);
   } else if (C % VMAX == 0 && aligned && C / VMAX <= 256) {
@@ -1091,9 +1094,9 @@ extern "C" int rv_warp3(const void* feat, const void* featUP, const float* conf,
   RV_REQUIRE(dtype == RV_F16 || dtype == RV_BF16, "rv_warp3: f16 / bf16 features only (use rv_warp for fp32)");
   RV_REQUIRE(C > 0 && C % 8 == 0, "rv_warp3: C=%d must be a multiple of 8", C);
   RV_REQUIRE((long long)4 * h * w * (C / 8) < (1ll << 31), "rv_warp3: map too large for 32-bit vector indices");
-  // tile shape (REFVSR_W3_TILE: 0 = 8 x 16 LR pixels / 256 threads, 1 = 4 x 16 / 256, 2 = 2 x 16 / 160).  Measured at 270x480x48 bf16:
-  // 32.3 / 35.0 / 38.1 us - every CTA pays the flow-tile load and two barriers before its first gather, so fewer, larger tiles win
-  // here (the opposite of aligned_sample2, whose single wave of 8 x 16 tiles ran its two phases in lock-step on every SM)
+  // tile shape (REFVSR_W3_TILE: 0 = 8 x 16 LR pixels / 256 threads, 1 = 4 x 16 / 256, 2 = 2 x 16 / 160).  Measured at 270x480x48 bf16
+  // on an H100 80GB HBM3 at a 400 W limit (tools/pointwise_bench.py): 52.7 / 52.7 / 57.3 us - every CTA pays the flow-tile load and
+  // two barriers before its first gather, so the smallest tiles lose
   static const int tile_env = getenv("REFVSR_W3_TILE") ? atoi(getenv("REFVSR_W3_TILE")) : RV_W3_TILE_DEFAULT;
   auto launch = [&](auto tag, auto cvtag, auto thtag) {
     using T = decltype(tag);

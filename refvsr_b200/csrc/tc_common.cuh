@@ -1,7 +1,6 @@
-// sm_100a primitives used by the tensor-core kernels: mbarrier, TMA (cp.async.bulk[.tensor]),
-// tcgen05.mma / commit / ld, TMEM allocation, and the UMMA shared-memory / instruction descriptors.
-// Bit layouts follow the PTX ISA "tcgen05 matrix descriptor" / "instruction descriptor" tables
-// (same fields as cute/arch/mma_sm100_desc.hpp in CUTLASS 4.x).
+// sm_90a primitives used by the tensor-core kernels: mbarrier, TMA (cp.async.bulk[.tensor]), warpgroup MMA
+// (wgmma.mma_async with both operands in shared memory, fp32 accumulators in registers) and its shared-memory matrix
+// descriptor.  Bit layouts follow the PTX ISA "wgmma matrix descriptor" table (same fields as cute/arch/mma_sm90_desc.hpp).
 #pragma once
 #include <cstdio>
 #include <cuda.h>
@@ -32,41 +31,8 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
 // The spin loop lives INSIDE the asm block: a C++ `while (!try_wait)` is a divergent loop to the compiler, after which
-// it no longer treats warp-uniform values (UMMA descriptors, barrier addresses) as uniform.
-#ifdef RV_WATCHDOG
-// diagnostics build (tools/conv_big_probe.py): a wait that never completes records who waited on what in a pinned HOST buffer
-// (device printf output does not survive the trap), then aborts the launch.  One copy of the pointer per translation unit.
-static __device__ unsigned long long* rv_wd_buf = nullptr;
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-  for (uint32_t spins = 0;; ++spins) {
-    if (mbar_try_wait(bar, parity)) return;
-    if (spins > (1u << 21)) {
-      if ((threadIdx.x & 31) == 0 && rv_wd_buf != nullptr) {
-        const unsigned long long i = atomicAdd(rv_wd_buf, 1ull);
-        if (i < 1000) {
-          rv_wd_buf[1 + i] = ((unsigned long long)blockIdx.x << 48) | ((unsigned long long)blockIdx.y << 40) |
-                             ((unsigned long long)(threadIdx.x >> 5) << 32) | ((unsigned long long)(smem_u32(bar) & 0xffffffu) << 8) | parity;
-        }
-        __threadfence_system();
-      }
-      __nanosleep(2000000);
-      __trap();
-    }
-  }
-}
-#else
+// it no longer treats warp-uniform values (descriptors, barrier addresses) as uniform.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
@@ -78,7 +44,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       "r"(parity)
       : "memory");
 }
-#endif
 
 // ---- TMA ---------------------------------------------------------------------------------------
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* m) {
@@ -109,107 +74,115 @@ __device__ __forceinline__ void bulk_load(const void* gmem, uint64_t* bar, void*
       : "memory");
 }
 
-// ---- tcgen05 -----------------------------------------------------------------------------------
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// whole warp must call
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]; single thread
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc,
-                                         uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// One elected lane of a fully converged warp.  tcgen05.mma / commit are issued as
-//   if (tc::elect_one()) { umma_f16(...); ... }
-// from WARP-UNIFORM control flow with warp-uniform operands: the compiler then keeps the descriptors in uniform
-// registers and emits back-to-back UTCHMMA.  Issued from an `if (lane == 0)` branch it cannot prove uniformity and
-// wraps every MMA in an ELECT / R2UR.BROADCAST / BRA.U.ANY waterfall (~27 SASS instructions, ~140 cycles per MMA
-// measured on B200 - profiles/r01_conv_timeline.md).
+// One elected lane of a fully converged warp (TMA issue from warp-uniform control flow).
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile("{\n\t.reg .pred P;\n\telect.sync _|P, 0xffffffff;\n\tselp.u32 %0, 1, 0, P;\n\t}" : "=r"(pred));
   return pred != 0;
 }
-// arrive on an mbarrier once all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 16 consecutive fp32 columns; warp w may only touch lanes [32*(w%4), +32)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t v[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t v[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]),
-        "=r"(v[7]), "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]),
-        "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]),
-        "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-        "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
 
-// K-major operand tile in shared memory written by TMA with SWIZZLE_128B: rows of 128 bytes
-// (64 x 16-bit), 8-row groups 1024 bytes apart.  `saddr` may be advanced by k*32 bytes inside the
-// first row of a 1024-byte-aligned atom to select a 16-element K slice.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr) {
+// ---- wgmma -------------------------------------------------------------------------------------
+// A warpgroup (4 consecutive warps, warp index % 4 == 0 first) issues every wgmma together.  fence: before the first MMA
+// that reads / writes accumulator registers the threads touched since; commit + wait<n>: at most n groups still in flight.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+
+// K-major operand tile written by TMA (or the host) with SWIZZLE_128B: rows of 128 bytes (64 x 16-bit), `sbo` bytes
+// between 8-row groups.  The start address may be advanced by k*32 bytes to select a 16-element K slice, and by whole
+// 128-byte rows: the swizzle is a function of the shared-memory address bits, so such a view reads what TMA wrote.
+__device__ __forceinline__ uint64_t desc_sw128(uint32_t saddr, uint32_t sbo = 1024) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);  // start address      bits [0,14)
-  d |= (uint64_t)1 << 16;                    // LBO = 16 B         bits [16,30) (unused, swizzled K-major)
-  d |= (uint64_t)(1024 >> 4) << 32;          // SBO = 1024 B       bits [32,46)
-  d |= (uint64_t)1 << 46;                    // descriptor version bits [46,48)
-  d |= (uint64_t)2 << 61;                    // SWIZZLE_128B       bits [61,64)
+  d |= (uint64_t)1 << 16;                    // LBO (unused for swizzled K-major)
+  d |= (uint64_t)(sbo >> 4) << 32;           // SBO                bits [32,46)
+  d |= (uint64_t)1 << 62;                    // SWIZZLE_128B       bits [62,64) = 1
   return d;
 }
-// K-major operand tile with SWIZZLE_32B: rows of 32 bytes (16 x 16-bit = one UMMA_K slice), 8-row groups 256 bytes
-// apart; 16-byte chunk j of row r sits at chunk j ^ ((r >> 2) & 1)  (Swizzle<1,4,3>: address bit 4 ^= bit 7).
-__device__ __forceinline__ uint64_t umma_desc_sw32(uint32_t saddr) {
+// K-major operand tile with SWIZZLE_32B: rows of 32 bytes (16 x 16-bit = one K slice), 8-row groups 256 bytes apart;
+// 16-byte chunk j of row r sits at chunk j ^ ((r >> 2) & 1)  (Swizzle<1,4,3>: address bit 4 ^= bit 7).
+__device__ __forceinline__ uint64_t desc_sw32(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)1 << 16;                    // LBO (unused)
-  d |= (uint64_t)(256 >> 4) << 32;           // SBO = 256 B
-  d |= (uint64_t)1 << 46;                    // descriptor version
-  d |= (uint64_t)6 << 61;                    // SWIZZLE_32B
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(256 >> 4) << 32;
+  d |= (uint64_t)3 << 62;                    // SWIZZLE_32B
   return d;
 }
-// kind::f16 instruction descriptor: fp32 accumulate, A/B both `fmt` (0 = f16, 1 = bf16), K-major
-__host__ __device__ __forceinline__ uint32_t umma_idesc(int fmt, int M, int N) {
-  return (1u << 4) | ((uint32_t)fmt << 7) | ((uint32_t)fmt << 10) | ((uint32_t)(N >> 3) << 17) |
-         ((uint32_t)(M >> 4) << 24);
+
+// D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, both K-major in shared memory, fp32 accumulators: thread t of the warpgroup
+// holds rows 16 * (t / 32) + (t % 32) / 4 (+ 8) and columns 8 j + 2 (t % 4) (+ 1) as d[4 j + {0, 1}] (+ 8 rows: {2, 3}).
+// acc == 0 overwrites D.  One wrapper per N; BF selects bf16 over f16 operands.
+#define RV_ACC4(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3])
+#define RV_ACC8(i) RV_ACC4(i), RV_ACC4(i + 4)
+#define RV_ACC16(i) RV_ACC8(i), RV_ACC8(i + 8)
+// T: operand type, N: columns, REGS: "%0, ..., %(N/2 - 1)", AB: "%(N/2), %(N/2 + 1)", P: "%(N/2 + 2)", then the N/2 accumulators
+#define RV_WGMMA(T, N, REGS, AB, P, ...)                                                                      \
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, " P ", 0;\n\twgmma.mma_async.sync.aligned.m64n" #N "k16.f32." T \
+               "." T " {" REGS "}, " AB ", p, 1, 1, 0, 0;\n\t}"                                                \
+               : __VA_ARGS__ : "l"(a), "l"(b), "r"(acc))
+template <bool BF>
+__device__ __forceinline__ void wgmma_m64n16k16(float (&d)[8], uint64_t a, uint64_t b, uint32_t acc) {
+#define RV_R "%0, %1, %2, %3, %4, %5, %6, %7"
+  if constexpr (BF) RV_WGMMA("bf16", 16, RV_R, "%8, %9", "%10", RV_ACC8(0));
+  else RV_WGMMA("f16", 16, RV_R, "%8, %9", "%10", RV_ACC8(0));
+#undef RV_R
+}
+template <bool BF>
+__device__ __forceinline__ void wgmma_m64n32k16(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
+#define RV_R "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+  if constexpr (BF) RV_WGMMA("bf16", 32, RV_R, "%16, %17", "%18", RV_ACC16(0));
+  else RV_WGMMA("f16", 32, RV_R, "%16, %17", "%18", RV_ACC16(0));
+#undef RV_R
+}
+template <bool BF>
+__device__ __forceinline__ void wgmma_m64n48k16(float (&d)[24], uint64_t a, uint64_t b, uint32_t acc) {
+#define RV_R "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23"
+  if constexpr (BF) RV_WGMMA("bf16", 48, RV_R, "%24, %25", "%26", RV_ACC16(0), RV_ACC8(16));
+  else RV_WGMMA("f16", 48, RV_R, "%24, %25", "%26", RV_ACC16(0), RV_ACC8(16));
+#undef RV_R
+}
+template <bool BF>
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
+#define RV_R "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+  if constexpr (BF) RV_WGMMA("bf16", 64, RV_R, "%32, %33", "%34", RV_ACC16(0), RV_ACC16(16));
+  else RV_WGMMA("f16", 64, RV_R, "%32, %33", "%34", RV_ACC16(0), RV_ACC16(16));
+#undef RV_R
+}
+template <bool BF>
+__device__ __forceinline__ void wgmma_m64n80k16(float (&d)[40], uint64_t a, uint64_t b, uint32_t acc) {
+#define RV_R "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39"
+  if constexpr (BF) RV_WGMMA("bf16", 80, RV_R, "%40, %41", "%42", RV_ACC16(0), RV_ACC16(16), RV_ACC8(32));
+  else RV_WGMMA("f16", 80, RV_R, "%40, %41", "%42", RV_ACC16(0), RV_ACC16(16), RV_ACC8(32));
+#undef RV_R
+}
+template <bool BF>
+__device__ __forceinline__ void wgmma_m64n96k16(float (&d)[48], uint64_t a, uint64_t b, uint32_t acc) {
+#define RV_R "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47"
+  if constexpr (BF) RV_WGMMA("bf16", 96, RV_R, "%48, %49", "%50", RV_ACC16(0), RV_ACC16(16), RV_ACC16(32));
+  else RV_WGMMA("f16", 96, RV_R, "%48, %49", "%50", RV_ACC16(0), RV_ACC16(16), RV_ACC16(32));
+#undef RV_R
+}
+template <bool BF>
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
+#define RV_R "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+  if constexpr (BF) RV_WGMMA("bf16", 128, RV_R, "%64, %65", "%66", RV_ACC16(0), RV_ACC16(16), RV_ACC16(32), RV_ACC16(48));
+  else RV_WGMMA("f16", 128, RV_R, "%64, %65", "%66", RV_ACC16(0), RV_ACC16(16), RV_ACC16(32), RV_ACC16(48));
+#undef RV_R
+}
+#undef RV_WGMMA
+#undef RV_ACC16
+#undef RV_ACC8
+#undef RV_ACC4
+
+template <int N, bool BF16>
+__device__ __forceinline__ void wgmma(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+  float (&r)[N / 2] = *reinterpret_cast<float (*)[N / 2]>(d);
+#define RV_WG(n) \
+  if constexpr (N == n) wgmma_m64n##n##k16<BF16>(r, a, b, acc);
+  RV_WG(16) RV_WG(32) RV_WG(48) RV_WG(64) RV_WG(80) RV_WG(96) RV_WG(128)
+#undef RV_WG
 }
 
 }  // namespace tc

@@ -1,5 +1,5 @@
 """`eval_qual_quan(config)` - drop-in for evaluation/eval_qual_quan.py:17-144 with the same inputs, printed lines, score file and
-image tree, re-organised so that the host loop no longer caps a ~90 frames/s network at ~1 frame/s:
+image tree, re-organised so that the host loop no longer caps a fast network at ~1 frame/s:
 
   reference (per frame)                                              here
   ------------------------------------------------------------------ ----------------------------------------------------

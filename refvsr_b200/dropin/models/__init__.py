@@ -1,5 +1,5 @@
 """Put `<repo>/refvsr_b200/dropin` in front of the reference checkout on sys.path and the reference's
-`from models.SRNet import SRNet` / `importlib.import_module('models.archs.RefVSR')` resolve to the B200
+`from models.SRNet import SRNet` / `importlib.import_module('models.archs.RefVSR')` resolve to the CUDA
 implementation; run.py / eval.py / trainers / ckpt_manager stay untouched (INTEGRATION.md).
 
 Only `models/SRNet.py` and `models/archs/RefVSR.py` are overridden.  The reference's `models/` directory (a namespace

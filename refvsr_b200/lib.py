@@ -1,7 +1,7 @@
 """ctypes binding of the C-ABI library (include/refvsr_b200.h) and the `CudaOps` operator set.
 
 `CudaOps` is the ONLY implementation of the operator interface that ships in the product: every
-method launches hand-written sm_100a kernels from `librefvsr_b200.so` on torch's current CUDA stream.
+method launches hand-written sm_90a kernels from `librefvsr_b200.so` on torch's current CUDA stream.
 There is no CPU / eager fallback - constructing `CudaOps` without the built library or without a
 CUDA device raises.  torch is used for device memory and streams only.
 """

@@ -1,9 +1,9 @@
-"""`Network` - the B200 implementation of models/archs/RefVSR.py::Network (reference lines cited inline).
+"""`Network` - the CUDA implementation of models/archs/RefVSR.py::Network (reference lines cited inline).
 
 The module keeps the reference's constructor signature (`Network(config)`), attribute names,
 `state_dict()` schema and the stateful `forward(lrs, refs, is_first_frame, is_log, is_train)` contract
 (RefVSR.py:151-325).  The forward pass is an explicit schedule of calls into the operator set
-(`lib.CudaOps`: hand-written sm_100a kernels behind the C ABI).  Differences to the reference are
+(`lib.CudaOps`: hand-written sm_90a kernels behind the C ABI).  Differences to the reference are
 confined to *how* results are obtained, never to what they are:
 
   * activations are NHWC f16/bf16/f32 buffers; concat / bias / activation / gating / residual /
@@ -87,8 +87,8 @@ class Network(nn.Module):
         self.act_dtype = _PREC[prec]
         # 'split' = fp32-grade matching GEMM ([hi|lo|hi] fp16 operands), 'single' = one fp16 pass
         # (what the reference does under autocast, trainers/trainer.py:237-239)
-        # measured (tools/match_mode_check.py, profiles/r01_match_mode.log): with bf16 activations the index-flip rate vs
-        # the reference is 1.1-1.7 % with either GEMM and PSNR is identical, so only the fp32 path pays for 'split'
+        # tools/match_mode_check.py compares the two against the reference; the fp32 path needs the fp32-grade
+        # argmax, the 16-bit paths already round their features
         self.match_mode = _cget(config, 'b200_match', 'split' if prec == 'fp32' else 'single')
         self.prefer_tc = bool(_cget(config, 'b200_tensor_cores', True))
         self.reuse = bool(_cget(config, 'b200_reuse', True))
@@ -104,24 +104,20 @@ class Network(nn.Module):
             raise ValueError("b200_reuse_check must be 'sync', 'async' or 'off'")
         self.reuse_fallbacks = 0      # calls that violated the sliding contract and were recomputed from scratch
         self.use_graphs = bool(_cget(config, 'b200_cuda_graphs', True))
-        # fused residual-block kernel: validated, but not faster than two conv launches yet (MMA-instruction bound,
-        # profiles/r01_conv_knockout.md) -> opt-in
+        # residual blocks through the fused rv_resblock kernel (one launch per block) -> opt-in
         self.fuse_resblocks = bool(_cget(config, 'b200_fuse_resblocks', False))
-        # cross-layer persistent chain kernel (rv_conv_chain): the 60-conv propagation trunks and the ResList decoders as ONE
-        # launch each, bit-identical to the per-layer path (csrc/conv_chain.cu).  Measured SLOWER than per-layer launches on
-        # B200 (20 vs 9.8 us per LR layer: per-tile GPU-scope synchronisation costs more than a launch boundary,
-        # profiles/r02_conv_chain.md) -> opt-in.
+        # rv_conv_chain: the 60-conv propagation trunks and the ResList decoders as one call each, the same results as the
+        # per-layer path (csrc/conv_chain.cu) -> opt-in.
         self.use_chain = bool(_cget(config, 'b200_conv_chain', False)) and not os.environ.get('REFVSR_NO_CHAIN')
         self.chain_max_ctas = int(_cget(config, 'b200_chain_max_ctas', 0))   # see rv_conv_chain_desc.max_ctas (dist.py sets it)
         # The forward-branch step of a steady window (RefVSR.py:248-277) needs only the previous call's state and per-frame products
         # of earlier calls; the products of the entering frame and the backward branch (RefVSR.py:211-238) do not depend on it.
         # With overlap on, the forward step is enqueued on a second stream (a fork / join inside the window's CUDA graph): the
-        # launches of the two branches fill each other's prologue / first-box latency / last-tile tail (~3.4 of the ~10 us of a
-        # trunk conv, profiles/r02_trunk_knockout.md).  Same kernels, same inputs, same order within each branch: bit-identical
-        # results (tests/test_gpu_model.py::test_branch_overlap_is_exact).  Measured 87.4 -> 89.1 frames/s.  Splitting the SMs
-        # statically between the two streams (rv_set_conv_cta_cap; 8.3 instead of 9.9 us per conv for two SYMMETRIC chains,
-        # profiles/r02_dual_chain.log) loses in the real window - 83.7 frames/s at 74 / 74, 86.3 with only the forward step capped -
-        # because the branches are not symmetric and a cap outlives the overlap; the caps therefore default to 0 (none).
+        # launches of the two branches fill each other's prologue / first-box latency / last-tile tail (part of every trunk
+        # conv).  Same kernels, same inputs, same order within each branch: bit-identical
+        # results (tests/test_gpu_model.py::test_branch_overlap_is_exact).  A static SM split between
+        # the two streams (rv_set_conv_cta_cap) is available; the branches are not symmetric and a cap outlives the overlap,
+        # so the caps default to 0 (none).
         self.overlap_branches = bool(_cget(config, 'b200_overlap_branches', True)) and not os.environ.get('REFVSR_NO_OVERLAP')
         # grid caps: forward step (second stream) / products and the first `overlap_bw_steps` backward steps (main stream); 0 = none
         self.overlap_cap = int(os.environ.get('REFVSR_OVERLAP_CAP', _cget(config, 'b200_overlap_cap', 0)))
@@ -221,7 +217,7 @@ class Network(nn.Module):
     # building blocks
     # ------------------------------------------------------------------------------------------
     def _resblock(self, conv1, conv2, x, out, tmp, act_mid, act_post=ACT_NONE):
-        """out = act_post(x + conv2(act_mid(conv1(x)))): one fused tcgen05 kernel when the block qualifies
+        """out = act_post(x + conv2(act_mid(conv1(x)))): rv_resblock when the block qualifies
         (16-bit activations, C <= 64), otherwise two convolutions through the scratch buffer `tmp`."""
         C = x.shape[2]
         m1, m2 = self.get_submodule(conv1), self.get_submodule(conv2)

@@ -6,7 +6,7 @@ Two layouts (see include/refvsr_b200.h):
   * TC   : 16-bit [nblk][S][kh][NB][64], S = kw * (chunks0 + chunks1), stage s = kx*nchunks + chunk;
            every [NB][64] slab is the byte image of a K-major SWIZZLE_128B UMMA operand tile
            (16-byte chunk j of row r stored at chunk j ^ (r % 8)), so the kernel fetches it with a plain
-           bulk copy and hands it to tcgen05.mma unchanged.
+           bulk copy and hands it to wgmma unchanged.
 """
 import hashlib
 import os
@@ -182,8 +182,7 @@ def layout1_fits(kh, kw, srcs, nb):
 def choose_layout(kh, kw, srcs, nb):
     """Default: layout 1 (ONE TMA box per tile and channel chunk; the kh x kw taps are shifted UMMA descriptor views
     of it) whenever all taps stay resident in shared memory, else layout 0 (one box per (kx, chunk) stage).  Layout 1
-    moves 1.7x fewer bytes from L2 and keeps >= 3 whole tiles in flight, which the multi-issuer MMA path needs
-    (profiles/r01_conv_timeline.md: 13.5 vs 16.2 ms / window).  REFVSR_TC_LAYOUT=0|1|2 forces a layout."""
+    moves 1.7x fewer bytes from L2 and keeps >= 3 whole tiles in flight, which the multi-issuer MMA path needs.  REFVSR_TC_LAYOUT=0|1|2 forces a layout."""
     import os
     forced = int(os.environ.get('REFVSR_TC_LAYOUT', str(DEFAULT_TC_LAYOUT)))
     if forced in (1, 3):     # 3 = layout-1 weight image with the kx-folded 3x3 mode disabled (A/B measurements)

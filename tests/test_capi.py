@@ -52,11 +52,11 @@ def test_invalid_arguments_return_error_codes_without_a_gpu():
     assert rc == -1
 
 
-def test_tensor_core_conv_plans_keep_issuers_exclusive():
-    """Regression test for the round-2 dead-lock (profiles/r02_8k.md): mbarrier parity waits are exact only if consecutive users of
-    a shared-memory slot / TMEM accumulator are the SAME issuing warp, i.e. tiles-in-flight and accumulators are multiples of the
-    issuer count.  rv_conv2d_tc_plan is host-only, so every conv shape of the path is checked here without a GPU, for the B200's
-    limits (232 448 B opt-in shared memory, 148 SMs) and for a smaller hypothetical budget."""
+def test_tensor_core_conv_plans_fit_and_keep_rings_per_consumer():
+    """rv_conv2d_tc_plan is host-only, so every conv shape of the path is planned here without a GPU, for the H100's limits
+    (232 448 B opt-in shared memory, 132 SMs) and for smaller hypothetical budgets: each of the two consumer warpgroups gets a
+    ring of >= 1 slot of its own, the plan fits the budget, and layout 1 (all taps as views of one box) only with resident
+    weights."""
     import ctypes as C
     from refvsr_b200.lib import load_library, rv_conv_desc
     lib = load_library()
@@ -71,7 +71,7 @@ def test_tensor_core_conv_plans_keep_issuers_exclusive():
                (8, 0, 64, 64, 3, 1, 0, 0), (64, 0, 64, 64, 3, 1, 0, 0), (64, 0, 128, 64, 3, 1, 0, 0), (128, 0, 16, 16, 1, 1, 0, 0),
                (8, 0, 32, 32, 5, 1, 0, 0), (32, 0, 32, 32, 3, 1, 0, 1), (128, 128, 32, 32, 3, 1, 0, 0), (192, 0, 48, 48, 3, 1, 0, 0), (48, 0, 3, 16, 3, 1, 0, 0)]
     seen = set()
-    for max_smem, sms in ((232448, 148), (166912, 132), (101376, 84)):
+    for max_smem, sms in ((232448, 132), (166912, 132), (101376, 84)):
         for (c0, c1, cout, nb, k, layout, ps, res) in shapes:
             for (H, W) in ((270, 480), (1080, 1920), (37, 53)):
                 d = rv_conv_desc()
@@ -86,11 +86,9 @@ def test_tensor_core_conv_plans_keep_issuers_exclusive():
                 if rc != 0:      # a shape this budget cannot hold is refused with a message, never mis-planned
                     assert lib.rv_last_error()
                     continue
-                mode, slots, grp, S, nmma, nacc, nb_, smem = list(out)
-                seen.add((mode, nmma))
-                assert 1 <= nmma <= 3 and nacc in (3, 6) and slots >= 1 and smem <= max_smem
-                unit = 1 if grp == S else S
-                if nmma > 1:
-                    assert nacc % nmma == 0, (c0, c1, cout, k, layout, list(out))
-                    assert slots % (unit * nmma) == 0 and slots // unit >= nmma, (c0, c1, cout, k, layout, list(out))
-    assert any(n == 3 for _, n in seen) and {m for m, _ in seen} >= {0, 1, 3}      # the sweep does reach the multi-issuer plans
+                mode, slots, resident, S, ncons, nacc, nb_, smem = list(out)
+                seen.add((mode, resident))
+                assert mode == (1 if layout in (1, 3) else layout) and nb_ == nb, (c0, c1, cout, k, layout, list(out))
+                assert ncons == nacc == 2 and slots >= 1 and smem <= max_smem, (c0, c1, cout, k, layout, list(out))
+                assert resident or mode != 1, (c0, c1, cout, k, layout, list(out))
+    assert {m for m, _ in seen} >= {0, 1, 2}      # the sweep reaches every mode

@@ -12,7 +12,7 @@ Bars (north_star: 1e-3 relative fp32, PSNR delta < 0.01 dB):
   fp32 path   PSNR vs reference >= 80 dB, 99.9 % of the pixels within 1e-3 (the hard argmax may flip near-ties: a handful of
               pixels can differ by more, which is why max-abs is reported, not bounded at 1e-3)
   16-bit path PSNR vs reference >= 60 dB (VERDICT r1: "raise the 42 dB bar"); index-map flip rate reported.
-Every run appends its numbers to gpurun_out/r02_parity_fullsize.jsonl (summarised in profiles/r02_parity_fullsize.md)."""
+With REFVSR_PARITY_LOG=<file> every run appends its numbers there as JSON lines."""
 import json
 import os
 
@@ -33,9 +33,10 @@ FULL = {
 
 
 def _report(rec):
-    os.makedirs(os.path.join(ROOT, 'gpurun_out'), exist_ok=True)
-    with open(os.path.join(ROOT, 'gpurun_out', 'r02_parity_fullsize.jsonl'), 'a') as f:
-        f.write(json.dumps(rec) + '\n')
+    path = os.environ.get('REFVSR_PARITY_LOG')
+    if path:
+        with open(path, 'a') as f:
+            f.write(json.dumps(rec) + '\n')
 
 
 def _load(name):

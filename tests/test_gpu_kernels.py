@@ -29,7 +29,7 @@ def close(a, b, tol, what=''):
 
 
 # ---------------------------------------------------------------------------------------------
-# convolution: SIMT and tcgen05 implementations against F.conv2d-based oracle
+# convolution: SIMT and wgmma implementations against F.conv2d-based oracle
 # ---------------------------------------------------------------------------------------------
 CONV_CASES = [
     # name, H, W, srcs[(real,alloc)], cout, k, stride, pad, act_pre, act_post, gate, res, shuffle, out_f32
@@ -103,7 +103,7 @@ def test_conv_tc(cuda_ops, oracle_ops, case, prec, layout):
         pytest.skip('weights of this conv are streamed (layout 0 only)')
     # layout 3 = the layout-1 weight image with the kx-folded 3x3 mode disabled (layout 1 folds when eligible)
     lc, out, exp = _run_conv(cuda_ops, oracle_ops, case, DT[prec], prefer_tc=True, tc_layout=layout)
-    assert lc.impl == IMPL_TC and lc.layout == layout, 'stride-1 16-bit convs must take the tcgen05 path'
+    assert lc.impl == IMPL_TC and lc.layout == layout, 'stride-1 16-bit convs must take the tensor-core path'
     close(out, exp, TOL[out.dtype] if out.dtype != torch.float32 else 2e-4, f'conv_tc[{case[0]},{prec}]')
 
 
@@ -160,7 +160,7 @@ def test_resblock_fused_full_size_matches_two_convs(cuda_ops):
 
 
 def test_conv_tc_large_matches_simt(cuda_ops):
-    """full-size property: tcgen05 path == CUDA-core path on a 270x480x48 map (fp16 storage ulp)."""
+    """full-size property: tensor-core path == CUDA-core path on a 270x480x48 map (fp16 storage ulp)."""
     H, W, C = 270, 480, 48
     w = rnd((C, C, 3, 3), 1, scale=0.07).half().float()
     b = rnd((C,), 2, scale=0.1)
@@ -293,7 +293,7 @@ def test_space_to_depth(cuda_ops, oracle_ops):
 
 
 def test_stride2_conv_via_space_to_depth_on_tensor_cores(cuda_ops, oracle_ops):
-    """ref_encoder2.0.0 (3x3 s2) and aa2.align.p_conv.0 (5x5 s2, two sources) through s2d + tcgen05"""
+    """ref_encoder2.0.0 (3x3 s2) and aa2.align.p_conv.0 (5x5 s2, two sources) through s2d + wgmma"""
     for k, srcs in ((3, [(48, 48)]), (5, [(32, 32), (32, 32)])):
         cin = sum(r for r, _ in srcs)
         w = rnd((32, cin, k, k), 1, scale=1.5 / (cin * k * k) ** 0.5).half().float()

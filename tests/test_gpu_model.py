@@ -1,4 +1,4 @@
-"""-m gpu: the whole hot path through SRNet.forward on the B200 against the golden vectors produced by the
+"""-m gpu: the whole hot path through SRNet.forward on the GPU against the golden vectors produced by the
 unmodified reference (tests/golden/make_golden.py) and against the oracle at a larger size.
 
 Bars (north_star): fp32 path <= 1e-3 relative; 16-bit paths are judged by PSNR against the reference output

@@ -1,6 +1,6 @@
 """Drop-in `data_loader` (decoded-frame cache): the reference's own Test_datasets returns bit-identical items with
-and without it, and decodes each file once per stream instead of T times.  Needs the reference checkout (build
-container only) - the GPU box has no /root/reference, where this test skips."""
+and without it, and decodes each file once per stream instead of T times.  Runs the reference checkout that build()
+stages under oracle/_ref/RefVSR (oracle/build_ref.py::ref_root); skips where none was staged."""
 import json
 import os
 import subprocess
@@ -14,8 +14,8 @@ CODE = r'''
 import sys, os, json, hashlib, time
 import numpy as np
 from PIL import Image
-root, tmp, use_dropin = sys.argv[1], sys.argv[2], sys.argv[3] == '1'
-sys.path[:0] = ([os.path.join(root, 'refvsr_b200', 'dropin')] if use_dropin else []) + [os.path.join(root, 'oracle', 'shims'), '/root/reference', root]
+root, tmp, use_dropin, ref_dir = sys.argv[1], sys.argv[2], sys.argv[3] == '1', sys.argv[4]
+sys.path[:0] = ([os.path.join(root, 'refvsr_b200', 'dropin')] if use_dropin else []) + [os.path.join(root, 'oracle', 'shims'), ref_dir, root]
 import importlib
 cfg = importlib.import_module('configs.config_RefVSR_small_MFID').get_config('p', 'm', 'config_RefVSR_small_MFID')
 cfg.dist = False
@@ -59,16 +59,23 @@ def _make_clip(tmp):
                 Image.fromarray(rng.integers(0, 256, (h, w, 3), dtype=np.uint8)).save(os.path.join(d, f'{k:04d}.png'))
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference/data_loader'), reason='reference checkout not present on this box')
+def _ref_root():
+    sys.path.insert(0, ROOT)
+    from oracle.build_ref import ref_root
+    return ref_root()
+
+
+@pytest.mark.skipif(_ref_root() is None, reason='no reference checkout staged (oracle/build_ref.py)')
 def test_cached_loader_returns_identical_items(tmp_path):
+    ref_dir = os.path.realpath(_ref_root())
     _make_clip(str(tmp_path))
     out = {}
     for flag in ('0', '1'):
-        r = subprocess.run([sys.executable, '-c', CODE, ROOT, str(tmp_path), flag], capture_output=True, text=True, timeout=600)
+        r = subprocess.run([sys.executable, '-c', CODE, ROOT, str(tmp_path), flag, ref_dir], capture_output=True, text=True, timeout=600)
         assert r.returncode == 0, r.stderr[-3000:]
         out[flag] = json.loads(r.stdout.strip().splitlines()[-1])
     ref, ours = out['0'], out['1']
-    assert '/root/reference' in ref['utils_file'] and 'dropin' in ours['utils_file']
+    assert os.path.realpath(ref['utils_file']).startswith(ref_dir) and 'dropin' in ours['utils_file']
     assert ours['items'] == ref['items'] == 10
     assert ours['meta'] == ref['meta']
     assert ours['sha'] == ref['sha'], 'every tensor of every item must be bit-identical'

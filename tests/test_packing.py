@@ -1,4 +1,4 @@
-"""Weight repacking (refvsr_b200/packing.py): the SIMT matrix and the swizzled tcgen05 image decode back to
+"""Weight repacking (refvsr_b200/packing.py): the SIMT matrix and the swizzled tensor-core image decode back to
 the original convolution weights under the layouts documented in include/refvsr_b200.h / conv_tc.cu."""
 import pytest
 import torch

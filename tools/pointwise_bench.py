@@ -9,7 +9,7 @@ from refvsr_b200.lib import CudaOps   # noqa: E402
 H, W, C = 270, 480, int(os.environ.get('PW_C', 48))
 dt = torch.bfloat16
 e = 2
-PEAK = 6575.0
+PEAK = 3350.0                     # H100 SXM data-sheet HBM3 bandwidth, GB/s
 
 
 def timeit(fn, iters=30, warm=5):

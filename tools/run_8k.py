@@ -1,4 +1,4 @@
-"""BASELINE configs[4]: config_RefVSR_MFID_8K at its real size - LR (and Ref) 1080x1920 -> 4320x7680, T = 7, bf16 - on ONE B200.
+"""BASELINE configs[4]: config_RefVSR_MFID_8K at its real size - LR (and Ref) 1080x1920 -> 4320x7680, T = 7, bf16 - on ONE GPU.
 Reports ms / window (first, steady, CUDA-graph replays), peak device memory against DESIGN.md's plan, and - at 540x960 LR, where
 the fp32 CUDA-core yardstick path is still affordable - PSNR of the bf16 tensor-core path against the fp32 path (which is pinned
 to the reference by the flag_HD_in goldens at fixture size).  Writes gpurun_out/r02_8k.json."""

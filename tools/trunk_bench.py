@@ -1,17 +1,12 @@
 """Where the time of the trunk convs goes, measured the way the window runs them: a chain of 60 conv launches (30 residual blocks,
-ping-pong maps that stay L2-resident) inside one CUDA graph, against the isolated launch with L2-cold / L2-warm buffers, plus the
-knock-outs of the experiments build (REFVSR_CONV_DBG: 1 no MMA, 8 no TMA loads, 64 no output stores, 128 no residual loads) and an
-L2-resident copy for scale.  Usage: python tools/trunk_bench.py [exp]"""
+ping-pong maps that stay L2-resident) inside one CUDA graph, against the isolated launch with L2-cold / L2-warm buffers, plus an
+L2-resident copy for scale.  Usage: python tools/trunk_bench.py"""
 import os
 import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import torch                                    # noqa: E402
 import refvsr_b200.lib as L                     # noqa: E402
-EXP = len(sys.argv) > 1 and sys.argv[1] == 'exp'
-if EXP:
-    L._lib = None
-    L.load_library(os.path.join(ROOT, 'refvsr_b200', 'librefvsr_b200_exp.so'))
 ops = L.CudaOps()
 from refvsr_b200 import packing                 # noqa: E402
 from refvsr_b200.lib import ACT_RELU, ACT_NONE  # noqa: E402
@@ -67,16 +62,6 @@ def report(tag):
 
 
 report('baseline')
-for k, v in (('REFVSR_NMMA', '1'), ('REFVSR_NMMA', '2')):
-    os.environ[k] = v
-    report(f'{k}={v}')
-    del os.environ[k]
-if EXP:
-    for bits, name in ((64, 'no output stores'), (128, 'no residual loads'), (192, 'no stores, no residual'), (1, 'no MMA'), (8, 'no TMA loads'),
-                       (9, 'no TMA, no MMA'), (201, 'barriers + TMEM reads only')):
-        os.environ['REFVSR_CONV_DBG'] = str(bits)
-        report(f'DBG {bits}: {name}')
-    del os.environ['REFVSR_CONV_DBG']
 # L2-resident copy for scale (12.4 MB maps): read + write bytes per second through L2
 for n in (1, 2, 4):
     src = [torch.randn((n * H, W, C), device=dev).to(dt) for _ in range(2)]
