@@ -65,6 +65,8 @@ uint64_t rv_launch_count(void);
  *   v       = act_pre(acc);  if (gate) v *= gate[pix][n];  if (res) v += res[pix][n];
  *   v       = act_post(v);
  *   out     = pixel_shuffle ? out[(2y+a, 2x+b)][n/4] (n = 4c+2a+b) : out[pix][n]
+ * `out` must not overlap src0, src1, gate or res: a tile reads the src0 / src1 halo that neighbouring tiles store,
+ * and the TC path fetches the gate / residual of later tiles while earlier tiles store.
  * ------------------------------------------------------------------------------------------------ */
 typedef struct rv_conv_desc {
   const void* src0;   /* [H][W][c0]                                                       */

@@ -16,6 +16,10 @@
 // Warp roles (384 threads): warp 0 = TMA producer (warps 1-3 idle), warpgroups 1 and 2 = consumers.  Consumer c owns the
 // CTA's local tiles c, c + 2, ... and its own ring of shared-memory slots, so one consumer's MMAs overlap the other's
 // epilogue (bias / act / gate / residual / act / NHWC or pixel-shuffled store straight from the accumulator registers).
+// Up to NB = 48 the epilogue never waits on a global load of the gate / residual: with 16-bit, 16-byte aligned operands
+// they arrive as TMA boxes in a per-consumer shared-memory buffer (plan_tc counts it, shrinking the ring), issued one
+// tile ahead by the consumer itself; otherwise each thread loads them into registers before issuing the tile's MMAs.
+// NB >= 64 loads each channel pair where it is used.  Stores stay plain global stores from registers.
 #include <algorithm>
 #include <cstdlib>
 
@@ -48,6 +52,8 @@ struct TcP {
   int res_cs;
   void* out;
   int out_cs, pixel_shuffle, pair_ok, fmt;
+  int epi_tma;                   // gate / residual tiles arrive by TMA in per-consumer shared-memory buffers
+  uint32_t epi_bytes, epi_tx;    // bytes of one such buffer ([128 pixels][NB] 16-bit) / of all buffers of one tile
 };
 
 // All MMAs of one pipeline stage into both 64-row halves.  Descriptor start addresses are in 16-byte units: +2 per
@@ -94,17 +100,28 @@ __device__ __forceinline__ void issue_stage(const TcP& p, float (&acc)[2][NB / 2
   }
 }
 
+// Gate / residual values of the channel pair (n, n + 1) as loaded, before conversion: 16-bit types packed into one
+// register (half the registers of a float2 while the loads are in flight), fp32 as float2.  `second`: n + 1 < cout.
+template <typename T> struct RawPair { using type = uint32_t; };
+template <> struct RawPair<float> { using type = float2; };
+
 template <typename T>
-__device__ __forceinline__ float2 ld2(const T* q, bool pair) {
+__device__ __forceinline__ typename RawPair<T>::type ld_raw2(const T* q, bool pair, bool second) {
   if constexpr (sizeof(T) == 2) {
-    if (pair) {
-      if constexpr (std::is_same<T, __half>::value) return __half22float2(*reinterpret_cast<const __half2*>(q));
-      else return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(q));
-    }
+    const uint16_t* u = reinterpret_cast<const uint16_t*>(q);
+    if (pair) return *reinterpret_cast<const uint32_t*>(q);
+    return (uint32_t)u[0] | (second ? (uint32_t)u[1] << 16 : 0u);
   } else {
     if (pair) return *reinterpret_cast<const float2*>(q);
+    return make_float2(q[0], second ? q[1] : 0.f);
   }
-  return make_float2(to_f(q[0]), 0.f);
+}
+
+template <typename T>
+__device__ __forceinline__ float2 raw2_to_f2(typename RawPair<T>::type r) {
+  if constexpr (std::is_same<T, __half>::value) return __half22float2(*reinterpret_cast<const __half2*>(&r));
+  else if constexpr (std::is_same<T, __nv_bfloat16>::value) return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&r));
+  else return r;
 }
 
 template <typename T>
@@ -123,10 +140,11 @@ __device__ __forceinline__ void st2(T* q, float a, float b, bool pair) {
 
 template <typename TI, typename TR, typename TO, int MODE, int NB>   // NB: output channels per CTA (= p.NB)
 __global__ void __launch_bounds__(128 * (1 + NCONS), 1)
-conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1, const TcP p) {
+conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1,
+               const __grid_constant__ CUtensorMap tmg, const __grid_constant__ CUtensorMap tmr, const TcP p) {
   constexpr bool BF = std::is_same<TI, __nv_bfloat16>::value;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ uint64_t bar_full[NCONS][MAX_SLOTS], bar_empty[NCONS][MAX_SLOTS], bar_w;
+  __shared__ uint64_t bar_full[NCONS][MAX_SLOTS], bar_empty[NCONS][MAX_SLOTS], bar_w, bar_epi[NCONS];
   __shared__ __align__(16) float bias_s[MAX_NB];
 
   const uint32_t raw = tc::smem_u32(smem_raw);
@@ -150,6 +168,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
         tc::mbar_init(&bar_empty[c][i], 4);   // one arrival per consumer warp
       }
     tc::mbar_init(&bar_w, 1);
+    for (int c = 0; c < NCONS; ++c) tc::mbar_init(&bar_epi[c], 1);
     tc::fence_barrier_init();
     tc::prefetch_tmap(&tm0);
     if (p.nch1 || p.nq1) tc::prefetch_tmap(&tm1);
@@ -217,7 +236,55 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
     int slot = 0;
     uint32_t ph = 0;
     float acc[2][NB / 2];
+    // Up to NB = 48 the epilogue takes a tile's gate and residual values from registers filled before it starts (loaded
+    // where they are used, each pair's load would cost the epilogue a full global-memory latency):
+    //  * p.epi_tma (16-bit, 16-byte aligned operands): the tile's [128 pixels][NB] gate / residual boxes arrive by TMA in
+    //    this consumer's buffers while an earlier tile's epilogue and this tile's MMAs run; the epilogue copies them to
+    //    registers and then, the buffers being free, issues the boxes of the consumer's next tile;
+    //  * otherwise each thread loads its values from global memory before issuing the tile's MMAs.
+    // Wider tiles keep per-pair loads: their accumulators leave no room for the whole tile's operands in 168 registers.
+    constexpr int NJ = NB / 8;
+    constexpr bool EARLY = NB <= 48;
+    constexpr bool TMA_OK = EARLY && sizeof(TR) == 2;
+    const bool epi_tma = TMA_OK && p.epi_tma;
+    uint8_t* epi_g = ring + (size_t)NCONS * p.slots * p.slot_bytes + (size_t)cons * p.epi_tx;   // gate box, then residual box
+    uint8_t* epi_r = epi_g + (gate != nullptr ? p.epi_bytes : 0u);
+    auto epi_load = [&](int tl) {     // one thread; the caller knows the consumer's buffers are free
+      if (tl >= ntiles) return;
+      const int ty = tl / p.tiles_x, tx = tl - ty * p.tiles_x;
+      tc::mbar_expect_tx(&bar_epi[cons], p.epi_tx);
+      if (gate != nullptr) tc::tma_load_3d(&tmg, &bar_epi[cons], epi_g, nblk * NB, tx * p.tw, ty * p.th);
+      if (res != nullptr) tc::tma_load_3d(&tmr, &bar_epi[cons], epi_r, nblk * NB, tx * p.tw, ty * p.th);
+    };
+    uint32_t eph = 0;
+    if (epi_tma && t == 0) {
+      tc::prefetch_tmap(&tmg);
+      tc::prefetch_tmap(&tmr);
+      epi_load(blockIdx.x + cons * gridDim.x);
+    }
     for (int tile = blockIdx.x + cons * gridDim.x; tile < ntiles; tile += NCONS * gridDim.x) {
+      const int ty0 = tile / p.tiles_x, tx0 = tile - ty0 * p.tiles_x;
+      typename RawPair<TI>::type gv[2][2][NJ];   // [h][r2][j], as the epilogue below indexes the accumulators
+      typename RawPair<TR>::type rv[2][2][NJ];
+      if (EARLY && !epi_tma) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int r2 = 0; r2 < 2; ++r2) {
+            const int m = 64 * h + 16 * wq + (lane >> 2) + 8 * r2;
+            const int oy = ty0 * p.th + (m >> p.tw_shift), ox = tx0 * p.tw + (m & (p.tw - 1));
+            if (oy >= p.Ho || ox >= p.Wo) continue;
+            const size_t pix = (size_t)oy * p.Wo + ox;
+#pragma unroll
+            for (int j = 0; j < NJ; ++j) {
+              const int n = nblk * NB + 8 * j + 2 * (lane & 3);
+              if (n >= p.cout) continue;
+              const bool second = n + 1 < p.cout, pair = p.pair_ok && second;
+              if (gate != nullptr) gv[h][r2][j] = ld_raw2<TI>(gate + pix * p.gate_cs + n, pair, second);
+              if (res != nullptr) rv[h][r2][j] = ld_raw2<TR>(res + pix * p.res_cs + n, pair, second);
+            }
+          }
+      }
       int ch = 0, prev = -1;
       for (int s = 0; s < p.S; ++s) {
         int ksteps = 4;
@@ -246,9 +313,31 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
       }
       tc::wgmma_wait<0>();
       if (prev >= 0 && lane == 0) tc::mbar_arrive(&bar_empty[cons][prev]);
+      if constexpr (TMA_OK) {
+        if (epi_tma) {
+          tc::mbar_wait(&bar_epi[cons], eph);
+          eph ^= 1u;
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int r2 = 0; r2 < 2; ++r2)
+#pragma unroll
+              for (int j = 0; j < NJ; ++j) {
+                const int m = 64 * h + 16 * wq + (lane >> 2) + 8 * r2;
+                const uint32_t off = (uint32_t)(m * NB + 8 * j + 2 * (lane & 3)) * 2u;
+                if (gate != nullptr) gv[h][r2][j] = *reinterpret_cast<const uint32_t*>(epi_g + off);
+                if (res != nullptr) rv[h][r2][j] = *reinterpret_cast<const uint32_t*>(epi_r + off);
+              }
+          // all 128 threads have read the buffers: order those reads before the async proxy's writes of the next tile
+          asm volatile("bar.sync %0, 128;" ::"r"(1 + cons) : "memory");
+          if (t == 0) {
+            tc::fence_proxy_async();
+            epi_load(tile + NCONS * gridDim.x);
+          }
+        }
+      }
 
       // ---- epilogue: thread t holds rows 64 h + 16 wq + lane / 4 (+ 8) and column pairs 8 j + 2 (lane % 4) ----
-      const int ty0 = tile / p.tiles_x, tx0 = tile - ty0 * p.tiles_x;
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
 #pragma unroll
@@ -258,7 +347,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
           if (oy >= p.Ho || ox >= p.Wo) continue;
           const size_t pix = (size_t)oy * p.Wo + ox;
 #pragma unroll
-          for (int j = 0; j < NB / 8; ++j) {
+          for (int j = 0; j < NJ; ++j) {
             const int nl = 8 * j + 2 * (lane & 3);
             const int n = nblk * NB + nl;
             if (n >= p.cout) continue;
@@ -270,13 +359,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
               v[e] = fmaxf(x, x * p.pre_slope);     // slope in [0,1]: identity / ReLU / LeakyReLU without a select
             }
             if (gate != nullptr) {
-              float2 g = ld2<TI>(gate + pix * p.gate_cs + n, pair);
-              if (!pair && n + 1 < p.cout) g.y = to_f(gate[pix * p.gate_cs + n + 1]);
+              const float2 g = raw2_to_f2<TI>(EARLY ? gv[h][r2][j] : ld_raw2<TI>(gate + pix * p.gate_cs + n, pair, n + 1 < p.cout));
               v[0] *= g.x; v[1] *= g.y;
             }
             if (res != nullptr) {
-              float2 r = ld2<TR>(res + pix * p.res_cs + n, pair);
-              if (!pair && n + 1 < p.cout) r.y = to_f(res[pix * p.res_cs + n + 1]);
+              const float2 r = raw2_to_f2<TR>(EARLY ? rv[h][r2][j] : ld_raw2<TR>(res + pix * p.res_cs + n, pair, n + 1 < p.cout));
               v[0] += r.x; v[1] += r.y;
             }
 #pragma unroll
@@ -316,19 +403,24 @@ PFN_tmapEncodeTiled get_tmap_encoder() {
   return fn;
 }
 
-static int make_act_tmap(CUtensorMap* m, const void* ptr, int C, int W, int H, int box_w, int box_rows, int fmt, int sw32 = 0) {
+// 16-bit NHWC map [H][W][C], boxes of box_c x box_w x box_rows; out-of-bounds elements read as zero
+static int make_tmap_3d(CUtensorMap* m, const void* ptr, int C, int W, int H, int box_c, int box_w, int box_rows, int fmt,
+                        CUtensorMapSwizzle swz) {
   PFN_tmapEncodeTiled enc = get_tmap_encoder();
   if (!enc) return fail(RV_E_CUDA, "cuTensorMapEncodeTiled entry point not available");
   cuuint64_t gdim[3] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H};
   cuuint64_t gstr[2] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2};
-  cuuint32_t box[3] = {sw32 ? 16u : 64u, (cuuint32_t)box_w, (cuuint32_t)box_rows};
+  cuuint32_t box[3] = {(cuuint32_t)box_c, (cuuint32_t)box_w, (cuuint32_t)box_rows};
   cuuint32_t estr[3] = {1, 1, 1};
   CUresult r = enc(m, fmt ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3,
                    const_cast<void*>(ptr), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   sw32 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                   swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(RV_E_CUDA, "cuTensorMapEncodeTiled failed (%d) C=%d W=%d H=%d", (int)r, C, W, H);
   return RV_OK;
+}
+
+static int make_act_tmap(CUtensorMap* m, const void* ptr, int C, int W, int H, int box_w, int box_rows, int fmt, int sw32 = 0) {
+  return make_tmap_3d(m, ptr, C, W, H, sw32 ? 16 : 64, box_w, box_rows, fmt, sw32 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 static int g_num_sms = 0;
@@ -337,8 +429,7 @@ static int g_cta_cap = 0;          // rv_set_conv_cta_cap: upper bound of the pe
 int set_conv_cta_cap(int cap) { const int old = g_cta_cap; g_cta_cap = cap > 0 ? cap : 0; return old; }
 
 template <typename TI, typename TR, typename TO, int MODE, int NB>
-static int launch_tc_mode(const CUtensorMap& tm0, const CUtensorMap& tm1, const TcP& p, dim3 grid, size_t smem,
-                          cudaStream_t st) {
+static int launch_tc_mode(const CUtensorMap* tm, const TcP& p, dim3 grid, size_t smem, cudaStream_t st) {
   auto kern = conv_tc_kernel<TI, TR, TO, MODE, NB>;
   static size_t configured = 0;   // per template instantiation
   if (smem > configured) {
@@ -356,29 +447,29 @@ static int launch_tc_mode(const CUtensorMap& tm0, const CUtensorMap& tm1, const 
   static const bool use_pdl = getenv("REFVSR_NO_PDL") == nullptr;
   cfg.attrs = attr;
   cfg.numAttrs = use_pdl ? 1 : 0;
-  RV_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tm0, tm1, p));
+  RV_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tm[0], tm[1], tm[2], tm[3], p));
   RV_LAUNCH_CHECK("conv_tc");
   return RV_OK;
 }
 
 template <typename TI, typename TR, typename TO, int NB>
-static int launch_tc_nb(const CUtensorMap& tm0, const CUtensorMap& tm1, const TcP& p, dim3 grid, size_t smem, cudaStream_t st) {
+static int launch_tc_nb(const CUtensorMap* tm, const TcP& p, dim3 grid, size_t smem, cudaStream_t st) {
   switch (p.mode) {
-    case 2: return launch_tc_mode<TI, TR, TO, 2, NB>(tm0, tm1, p, grid, smem, st);
-    case 1: return launch_tc_mode<TI, TR, TO, 1, NB>(tm0, tm1, p, grid, smem, st);
-    default: return launch_tc_mode<TI, TR, TO, 0, NB>(tm0, tm1, p, grid, smem, st);
+    case 2: return launch_tc_mode<TI, TR, TO, 2, NB>(tm, p, grid, smem, st);
+    case 1: return launch_tc_mode<TI, TR, TO, 1, NB>(tm, p, grid, smem, st);
+    default: return launch_tc_mode<TI, TR, TO, 0, NB>(tm, p, grid, smem, st);
   }
 }
 
 template <typename TI, typename TR, typename TO>
-static int launch_tc(const CUtensorMap& tm0, const CUtensorMap& tm1, const TcP& p, dim3 grid, size_t smem, cudaStream_t st) {
+static int launch_tc(const CUtensorMap* tm, const TcP& p, dim3 grid, size_t smem, cudaStream_t st) {
   switch (p.NB) {
-    case 16: return launch_tc_nb<TI, TR, TO, 16>(tm0, tm1, p, grid, smem, st);
-    case 32: return launch_tc_nb<TI, TR, TO, 32>(tm0, tm1, p, grid, smem, st);
-    case 48: return launch_tc_nb<TI, TR, TO, 48>(tm0, tm1, p, grid, smem, st);
-    case 64: return launch_tc_nb<TI, TR, TO, 64>(tm0, tm1, p, grid, smem, st);
-    case 80: return launch_tc_nb<TI, TR, TO, 80>(tm0, tm1, p, grid, smem, st);
-    default: return launch_tc_nb<TI, TR, TO, 96>(tm0, tm1, p, grid, smem, st);
+    case 16: return launch_tc_nb<TI, TR, TO, 16>(tm, p, grid, smem, st);
+    case 32: return launch_tc_nb<TI, TR, TO, 32>(tm, p, grid, smem, st);
+    case 48: return launch_tc_nb<TI, TR, TO, 48>(tm, p, grid, smem, st);
+    case 64: return launch_tc_nb<TI, TR, TO, 64>(tm, p, grid, smem, st);
+    case 80: return launch_tc_nb<TI, TR, TO, 80>(tm, p, grid, smem, st);
+    default: return launch_tc_nb<TI, TR, TO, 96>(tm, p, grid, smem, st);
   }
 }
 
@@ -433,10 +524,20 @@ static int plan_tc(const rv_conv_desc* d, TcP& p, size_t& smem_out, int& nblk_ou
   // shared-memory plan: weights resident when they leave room for two slots per consumer (layout 1: one), else streamed with
   // A; a consumer with a single slot still overlaps with the other consumer's ring
   const size_t w_all = (size_t)p.S * p.w_bytes;
-  if (w_all + (size_t)NCONS * (p.mode == 1 ? 1 : 2) * p.a_bytes <= budget) {
+  const size_t ring_min = (size_t)NCONS * (p.mode == 1 ? 1 : 2) * p.a_bytes;
+  // TMA epilogue: 16-bit gate / residual whose boxes TMA can address (16-byte aligned base and pixel stride), tiles the
+  // register epilogue keeps whole (NB <= 48), and room for the buffers next to resident weights and the minimal ring
+  const int rdt0 = d->res ? d->res_dtype : d->in_dtype;
+  auto tma_ok = [](const void* q, int cs) { return q == nullptr || ((uintptr_t)q % 16 == 0 && cs > 0 && cs % 8 == 0); };
+  p.epi_bytes = (uint32_t)p.th * p.tw * p.NB * 2;
+  p.epi_tx = (uint32_t)((d->gate ? 1 : 0) + (d->res ? 1 : 0)) * p.epi_bytes;
+  p.epi_tma = (d->gate || d->res) && p.NB <= 48 && rdt0 == d->in_dtype && tma_ok(d->gate, d->gate_cs) &&
+              tma_ok(d->res, d->res_cs) && w_all + ring_min + (size_t)NCONS * p.epi_tx <= budget;
+  const size_t epi_all = p.epi_tma ? (size_t)NCONS * p.epi_tx : 0;
+  if (w_all + ring_min + epi_all <= budget) {
     p.resident = 1;
     p.slot_bytes = p.a_bytes;
-    p.slots = (int)std::min<size_t>(MAX_SLOTS, (budget - w_all) / ((size_t)NCONS * p.a_bytes));
+    p.slots = (int)std::min<size_t>(MAX_SLOTS, (budget - w_all - epi_all) / ((size_t)NCONS * p.a_bytes));
   } else {
     RV_REQUIRE(p.mode != 1, "rv_conv2d(tc): layout 1 weights do not fit in shared memory");
     p.resident = 0;
@@ -444,7 +545,7 @@ static int plan_tc(const rv_conv_desc* d, TcP& p, size_t& smem_out, int& nblk_ou
     p.slots = (int)std::min<size_t>(MAX_SLOTS, budget / ((size_t)NCONS * p.slot_bytes));
     RV_REQUIRE(p.slots >= 1, "rv_conv2d(tc): stage of %u bytes does not fit once per consumer in shared memory", p.slot_bytes);
   }
-  const size_t smem = 1024 + (p.resident ? w_all : 0) + (size_t)NCONS * p.slots * p.slot_bytes;
+  const size_t smem = 1024 + (p.resident ? w_all : 0) + (size_t)NCONS * p.slots * p.slot_bytes + epi_all;
   p.wpack = (const uint8_t*)d->wpack; p.bias = d->bias;
   auto slope = [](int act) { return act == RV_ACT_RELU ? 0.f : act == RV_ACT_LRELU01 ? 0.1f : act == RV_ACT_LRELU02 ? 0.2f : 1.f; };
   RV_REQUIRE(d->act_pre != RV_ACT_CLAMP3, "rv_conv2d(tc): clamp3 is only supported as act_post");
@@ -478,23 +579,27 @@ int conv2d_tc(const rv_conv_desc* d, cudaStream_t st) {
   }
   const int rdt = d->res ? d->res_dtype : d->out_dtype;
   const int sw32 = p.mode == 2;
-  CUtensorMap tm0, tm1;
-  int rc = make_act_tmap(&tm0, d->src0, p.c0, d->W, d->H, p.mode == 1 ? p.tw + d->kw - 1 : p.tw, p.th + d->kh - 1, p.fmt, sw32);
+  CUtensorMap tm[4];    // src0, src1, gate, res (unused ones: copies of src0)
+  int rc = make_act_tmap(&tm[0], d->src0, p.c0, d->W, d->H, p.mode == 1 ? p.tw + d->kw - 1 : p.tw, p.th + d->kh - 1, p.fmt, sw32);
   if (rc) return rc;
+  tm[1] = tm[2] = tm[3] = tm[0];
   if (p.c1) {
-    rc = make_act_tmap(&tm1, d->src1, p.c1, d->W, d->H, p.mode == 1 ? p.tw + d->kw - 1 : p.tw, p.th + d->kh - 1, p.fmt, sw32);
+    rc = make_act_tmap(&tm[1], d->src1, p.c1, d->W, d->H, p.mode == 1 ? p.tw + d->kw - 1 : p.tw, p.th + d->kh - 1, p.fmt, sw32);
     if (rc) return rc;
-  } else {
-    tm1 = tm0;
   }
+  // gate / residual boxes for the TMA epilogue: [th][tw][NB], unswizzled, so box pixel m sits at m * NB channels
+  if (p.epi_tma && d->gate && (rc = make_tmap_3d(&tm[2], d->gate, d->gate_cs, p.Wo, p.Ho, p.NB, p.tw, p.th, p.fmt, CU_TENSOR_MAP_SWIZZLE_NONE)))
+    return rc;
+  if (p.epi_tma && d->res && (rc = make_tmap_3d(&tm[3], d->res, d->res_cs, p.Wo, p.Ho, p.NB, p.tw, p.th, p.fmt, CU_TENSOR_MAP_SWIZZLE_NONE)))
+    return rc;
   const int ntiles = p.tiles_x * p.tiles_y;
   int gx = std::min(ntiles, std::max(1, g_num_sms / nblk));
   if (g_cta_cap > 0) gx = std::min(gx, std::max(1, g_cta_cap / nblk));     // two capped launches on different streams share the SMs
   dim3 grid(gx, nblk);
-  if (d->in_dtype == RV_F16 && rdt == RV_F16 && d->out_dtype == RV_F16) return launch_tc<__half, __half, __half>(tm0, tm1, p, grid, smem, st);
-  if (d->in_dtype == RV_F16 && rdt == RV_F32 && d->out_dtype == RV_F32) return launch_tc<__half, float, float>(tm0, tm1, p, grid, smem, st);
-  if (d->in_dtype == RV_BF16 && rdt == RV_BF16 && d->out_dtype == RV_BF16) return launch_tc<__nv_bfloat16, __nv_bfloat16, __nv_bfloat16>(tm0, tm1, p, grid, smem, st);
-  if (d->in_dtype == RV_BF16 && rdt == RV_F32 && d->out_dtype == RV_F32) return launch_tc<__nv_bfloat16, float, float>(tm0, tm1, p, grid, smem, st);
+  if (d->in_dtype == RV_F16 && rdt == RV_F16 && d->out_dtype == RV_F16) return launch_tc<__half, __half, __half>(tm, p, grid, smem, st);
+  if (d->in_dtype == RV_F16 && rdt == RV_F32 && d->out_dtype == RV_F32) return launch_tc<__half, float, float>(tm, p, grid, smem, st);
+  if (d->in_dtype == RV_BF16 && rdt == RV_BF16 && d->out_dtype == RV_BF16) return launch_tc<__nv_bfloat16, __nv_bfloat16, __nv_bfloat16>(tm, p, grid, smem, st);
+  if (d->in_dtype == RV_BF16 && rdt == RV_F32 && d->out_dtype == RV_F32) return launch_tc<__nv_bfloat16, float, float>(tm, p, grid, smem, st);
   return fail(RV_E_UNSUPPORTED, "rv_conv2d(tc): unsupported dtype combination in=%d res=%d out=%d", d->in_dtype, rdt, d->out_dtype);
 }
 
