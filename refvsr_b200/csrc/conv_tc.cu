@@ -13,13 +13,20 @@
 //   * B operand: weights pre-packed on the host in exactly the swizzled shared-memory image, fetched with plain bulk
 //     copies; resident for the whole CTA lifetime when they fit, otherwise streamed through the ring with A.
 //   * D: fp32 accumulators in the registers of the consumer warpgroup (two m64nNk16 halves of the 128-pixel tile).
+// MODE 1 3 x 3 convolutions whose every channel chunk takes 3 K-steps (48 channels: the trunk, fusions, pixel shuffles and
+// the HR tail) at NB 16 / 48 / 96 run a kernel whose tap and K-step loops are unrolled at compile time (p.fixed): a stage
+// is then one fence, 54 wgmmas with no branch between them and one commit, where the runtime loop makes ptxas fence and
+// wait on every wgmma.  Other shapes (8 + 48 channels, 7 x 7) keep the runtime loop; both issue the same MMAs in the same order.
 // Warp roles (384 threads): warp 0 = TMA producer (warps 1-3 idle), warpgroups 1 and 2 = consumers.  Consumer c owns the
 // CTA's local tiles c, c + 2, ... and its own ring of shared-memory slots, so one consumer's MMAs overlap the other's
 // epilogue (bias / act / gate / residual / act / NHWC or pixel-shuffled store straight from the accumulator registers).
 // Up to NB = 48 the epilogue never waits on a global load of the gate / residual: with 16-bit, 16-byte aligned operands
 // they arrive as TMA boxes in a per-consumer shared-memory buffer (plan_tc counts it, shrinking the ring), issued one
 // tile ahead by the consumer itself; otherwise each thread loads them into registers before issuing the tile's MMAs.
-// NB >= 64 loads each channel pair where it is used.  Stores stay plain global stores from registers.
+// NB >= 64 loads each channel pair where it is used.  Stores stay plain global stores from registers.  The upsampling
+// convs (3 x 3, NB = 96, pixel shuffle into a 16-bit map, no gate / residual; p.ps_vec) run a twin of the compile-time
+// kernel (PSV) whose epilogue exchanges column pairs between lanes q and q ^ 2, so that each thread holds the 24
+// consecutive channels of one output pixel and writes them as three 16-byte vectors instead of 24 2-byte stores.
 #include <algorithm>
 #include <cstdlib>
 
@@ -54,14 +61,39 @@ struct TcP {
   int out_cs, pixel_shuffle, pair_ok, fmt;
   int epi_tma;                   // gate / residual tiles arrive by TMA in per-consumer shared-memory buffers
   uint32_t epi_bytes, epi_tx;    // bytes of one such buffer ([128 pixels][NB] 16-bit) / of all buffers of one tile
+  int fixed;                     // MODE 1 with FIX_KS x FIX_KS taps and FIX_KST K-steps in every chunk (compile-time loop)
+  int ps_vec;                    // pixel shuffle: each output pixel's NB / 4 channels as 16-byte stores (PSV kernel)
 };
 
+// MODE 1 shapes whose tap / K-step loops are unrolled at compile time: KS x KS taps and KST K = 16 steps in every channel
+// chunk (3 x 3 over 48-channel chunks: the trunk, fusions, pixel shuffles and the HR tail), at the NB the window uses.
+static constexpr int FIX_KS = 3, FIX_KST = 3;
+__host__ __device__ constexpr bool fixed_nb(int nb) { return nb == 16 || nb == 48 || nb == 96; }
+
 // All MMAs of one pipeline stage into both 64-row halves.  Descriptor start addresses are in 16-byte units: +2 per
-// K = 16 slice of a 128-byte row, whole rows per tap.
-template <int MODE, bool BF, int NB>
+// K = 16 slice of a 128-byte row, whole rows per tap.  KS > 0 (MODE 1 only): kh = kw = KS and KST K-steps per chunk known
+// at compile time, so the stage is one unbranched run of wgmmas that ptxas issues behind a single warpgroup.arrive; the
+// MMA order per accumulator half (ky, kx, k) is the runtime loop's, so the results are the same bits.
+template <int MODE, bool BF, int NB, int KS = 0, int KST = 0>
 __device__ __forceinline__ void issue_stage(const TcP& p, float (&acc)[2][NB / 2], uint32_t a_addr, uint32_t b_addr,
                                             int s, int ksteps) {
-  if constexpr (MODE == 2) {
+  if constexpr (MODE == 1 && KS > 0) {
+    constexpr uint32_t sbo = (uint32_t)(8 + KS - 1) * 128;   // box width bw = tw + KS - 1 pixels of 128 bytes
+#pragma unroll
+    for (int ky = 0; ky < KS; ++ky)
+#pragma unroll
+      for (int kx = 0; kx < KS; ++kx) {
+        const uint64_t bd = tc::desc_sw128(b_addr + (uint32_t)((ky * KS + kx) * NB * 128));
+        const uint32_t at = a_addr + (uint32_t)((ky * (8 + KS - 1) + kx) * 128);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint64_t ad = tc::desc_sw128(at + (uint32_t)h * 8 * sbo, sbo);
+#pragma unroll
+          for (int k = 0; k < KST; ++k)
+            tc::wgmma<NB, BF>(acc[h], ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (s | ky | kx | k) ? 1u : 0u);
+        }
+      }
+  } else if constexpr (MODE == 2) {
     const int nq = p.nq0 + p.nq1;
     for (int ky = 0; ky < p.kh; ++ky)
       for (int qd = 0; qd < nq; ++qd) {
@@ -138,7 +170,16 @@ __device__ __forceinline__ void st2(T* q, float a, float b, bool pair) {
   q[0] = from_f<T>(a);
 }
 
-template <typename TI, typename TR, typename TO, int MODE, int NB>   // NB: output channels per CTA (= p.NB)
+// two 16-bit values, a in the low half (the lower address of a little-endian store)
+template <typename T>
+__device__ __forceinline__ uint32_t pack2(float a, float b) {
+  const T lo = from_f<T>(a), hi = from_f<T>(b);
+  return (uint32_t)*reinterpret_cast<const uint16_t*>(&lo) | (uint32_t)*reinterpret_cast<const uint16_t*>(&hi) << 16;
+}
+
+// NB: output channels per CTA (= p.NB); KS, KST: compile-time taps and K-steps of MODE 1 (0: the runtime loop, p.fixed = 0);
+// PSV: the 16-byte pixel-shuffle epilogue (p.ps_vec), which has no gate / residual
+template <typename TI, typename TR, typename TO, int MODE, int NB, int KS, int KST, bool PSV>
 __global__ void __launch_bounds__(128 * (1 + NCONS), 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1,
                const __grid_constant__ CUtensorMap tmg, const __grid_constant__ CUtensorMap tmr, const TcP p) {
@@ -297,7 +338,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
         const uint32_t a_addr = ring_addr + (uint32_t)slot * p.slot_bytes;
         const uint32_t b_addr = p.resident ? w_addr + (uint32_t)s * p.w_bytes : a_addr + p.a_bytes;
         tc::wgmma_fence();
-        issue_stage<MODE, BF, NB>(p, acc, a_addr, b_addr, s, ksteps);
+        issue_stage<MODE, BF, NB, KS, KST>(p, acc, a_addr, b_addr, s, ksteps);
         tc::wgmma_commit();
         if (p.slots == 1) {
           // a single slot is refilled only after these MMAs have read it
@@ -338,6 +379,49 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
       }
 
       // ---- epilogue: thread t holds rows 64 h + 16 wq + lane / 4 (+ 8) and column pairs 8 j + 2 (lane % 4) ----
+      if constexpr (PSV) {
+        // Pixel shuffle into a 16-bit map without gate / residual.  n = 4c + 2a + b  ->  out[(2oy+a, 2ox+b)][c].  Lane
+        // q = lane % 4 holds (c, a) = (2j + q / 2, q % 2) for b = 0, 1; one exchange with lane q ^ 2 (same row, same a)
+        // leaves it pixel (a, b) = (q % 2, q / 2) for c = 2j, 2j + 1 of every j: the block's NB / 4 consecutive channels
+        // of one output pixel, stored as 16-byte vectors.  The general epilogue below is not compiled into this kernel.
+        static_assert(sizeof(TO) == 2 && (NB / 4) % 8 == 0, "16-byte pixel-shuffle rows need 16-bit outputs, NB % 32 == 0");
+        const int a = lane & 1, b = (lane >> 1) & 1;
+        // own (b = 0 | b = 1) word and the partner's: b = 0 keeps both low halves, b = 1 both high halves (c = 2j first)
+        const uint32_t sel = b ? 0x3276u : 0x5410u;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+          for (int r2 = 0; r2 < 2; ++r2) {
+            const int m = 64 * h + 16 * wq + (lane >> 2) + 8 * r2;
+            const int oy = ty0 * p.th + (m >> p.tw_shift), ox = tx0 * p.tw + (m & (p.tw - 1));
+            const bool in = oy < p.Ho && ox < p.Wo;     // the same for both partners of the exchange
+#pragma unroll
+            for (int i = 0; i < NJ / 4; ++i) {          // channels 8 i .. 8 i + 7 of the pixel: column pairs j = 4 i .. 4 i + 3
+              uint32_t pk[4];
+#pragma unroll
+              for (int jj = 0; jj < 4; ++jj) {
+                const int j = 4 * i + jj;
+                float v[2];
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  const float x = acc[h][4 * j + 2 * r2 + e] + bias_s[8 * j + 2 * (lane & 3) + e];
+                  v[e] = fmaxf(x, x * p.pre_slope);
+                  v[e] = fmaxf(v[e], v[e] * p.post_slope);
+                  if (p.post_clamp3) v[e] = fminf(fmaxf(v[e], -3.f), 3.f);
+                }
+                const uint32_t own = pack2<TO>(v[0], v[1]);
+                const uint32_t got = __shfl_xor_sync(0xffffffffu, own, 2);
+                pk[jj] = __byte_perm(own, got, sel);
+              }
+              if (in) {
+                TO* o = out + ((size_t)(2 * oy + a) * (2 * p.Wo) + 2 * ox + b) * p.out_cs + nblk * (NB / 4) + 8 * i;
+                *reinterpret_cast<uint4*>(o) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+              }
+            }
+          }
+        }
+        continue;
+      }
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
 #pragma unroll
@@ -428,9 +512,9 @@ static int g_max_smem = 0;
 static int g_cta_cap = 0;          // rv_set_conv_cta_cap: upper bound of the persistent grid (0 = one CTA per SM)
 int set_conv_cta_cap(int cap) { const int old = g_cta_cap; g_cta_cap = cap > 0 ? cap : 0; return old; }
 
-template <typename TI, typename TR, typename TO, int MODE, int NB>
+template <typename TI, typename TR, typename TO, int MODE, int NB, int KS = 0, int KST = 0, bool PSV = false>
 static int launch_tc_mode(const CUtensorMap* tm, const TcP& p, dim3 grid, size_t smem, cudaStream_t st) {
-  auto kern = conv_tc_kernel<TI, TR, TO, MODE, NB>;
+  auto kern = conv_tc_kernel<TI, TR, TO, MODE, NB, KS, KST, PSV>;
   static size_t configured = 0;   // per template instantiation
   if (smem > configured) {
     RV_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -456,7 +540,13 @@ template <typename TI, typename TR, typename TO, int NB>
 static int launch_tc_nb(const CUtensorMap* tm, const TcP& p, dim3 grid, size_t smem, cudaStream_t st) {
   switch (p.mode) {
     case 2: return launch_tc_mode<TI, TR, TO, 2, NB>(tm, p, grid, smem, st);
-    case 1: return launch_tc_mode<TI, TR, TO, 1, NB>(tm, p, grid, smem, st);
+    case 1:
+      if constexpr (fixed_nb(NB)) {
+        if constexpr (NB == 96 && sizeof(TO) == 2)
+          if (p.ps_vec) return launch_tc_mode<TI, TR, TO, 1, NB, FIX_KS, FIX_KST, true>(tm, p, grid, smem, st);
+        if (p.fixed) return launch_tc_mode<TI, TR, TO, 1, NB, FIX_KS, FIX_KST>(tm, p, grid, smem, st);
+      }
+      return launch_tc_mode<TI, TR, TO, 1, NB>(tm, p, grid, smem, st);
     default: return launch_tc_mode<TI, TR, TO, 0, NB>(tm, p, grid, smem, st);
   }
 }
@@ -558,6 +648,18 @@ static int plan_tc(const rv_conv_desc* d, TcP& p, size_t& smem_out, int& nblk_ou
   auto al = [](const void* q, int cs, int dt) { return q == nullptr || (((uintptr_t)q % (2 * dtype_size(dt)) == 0) && cs % 2 == 0); };
   p.pair_ok = al(d->out, d->out_cs, d->out_dtype) && al(d->gate, d->gate_cs, d->in_dtype) && al(d->res, d->res_cs, rdt);
   p.fmt = d->in_dtype == RV_BF16 ? 1 : 0;
+  // the compile-time tap loop: a square FIX_KS kernel whose every channel chunk takes FIX_KST K-steps (e.g. 48 + 48
+  // channels, not 8 + 48); other shapes keep the runtime loop
+  p.fixed = p.mode == 1 && d->kh == FIX_KS && d->kw == FIX_KS && fixed_nb(p.NB);
+  for (int ch = 0; ch < p.nch0 + p.nch1 && p.fixed; ++ch) {
+    const int crem = (ch < p.nch0) ? (p.c0 - ch * 64) : (p.c1 - (ch - p.nch0) * 64);
+    p.fixed = (std::min(crem, 64) + 15) / 16 == FIX_KST;
+  }
+  // the upsampling convs (compile-time 3 x 3 loop, NB = 96, pixel shuffle into a 16-bit map, no gate / residual): a thread
+  // gathers one output pixel's 24 channels and stores them as three 16-byte vectors, when every channel of the block
+  // exists and the pixel rows stay 16-byte aligned; other pixel shuffles keep the 2-byte stores
+  p.ps_vec = p.fixed && p.pixel_shuffle && p.NB == 96 && dtype_size(d->out_dtype) == 2 && d->cout % p.NB == 0 &&
+             !d->gate && !d->res && (uintptr_t)d->out % 16 == 0 && (d->out_cs * 2) % 16 == 0;
   smem_out = smem;
   nblk_out = nblk;
   return RV_OK;
