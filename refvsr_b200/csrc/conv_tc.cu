@@ -23,7 +23,11 @@
 // Up to NB = 48 the epilogue never waits on a global load of the gate / residual: with 16-bit, 16-byte aligned operands
 // they arrive as TMA boxes in a per-consumer shared-memory buffer (plan_tc counts it, shrinking the ring), issued one
 // tile ahead by the consumer itself; otherwise each thread loads them into registers before issuing the tile's MMAs.
-// NB >= 64 loads each channel pair where it is used.  Stores stay plain global stores from registers.  The upsampling
+// NB >= 64 loads each channel pair where it is used.  The compile-time kernels up to NB = 48 with a plain 16-bit output
+// write the tile into a per-consumer shared-memory buffer and store it with one TMA box store (p.out_tma): a tile's 24
+// channel-pair stores per thread, each behind its own bounds branches, made the epilogue the longest phase of a tile.
+// In every compile-time kernel the two consumers also take turns issuing their MMA batches, so that each epilogue
+// overlaps the other consumer's MMAs.  Other epilogues store from registers.  The upsampling
 // convs (3 x 3, NB = 96, pixel shuffle into a 16-bit map, no gate / residual; p.ps_vec) run a twin of the compile-time
 // kernel (PSV) whose epilogue exchanges column pairs between lanes q and q ^ 2, so that each thread holds the 24
 // consecutive channels of one output pixel and writes them as three 16-byte vectors instead of 24 2-byte stores.
@@ -63,6 +67,8 @@ struct TcP {
   uint32_t epi_bytes, epi_tx;    // bytes of one such buffer ([128 pixels][NB] 16-bit) / of all buffers of one tile
   int fixed;                     // MODE 1 with FIX_KS x FIX_KS taps and FIX_KST K-steps in every chunk (compile-time loop)
   int ps_vec;                    // pixel shuffle: each output pixel's NB / 4 channels as 16-byte stores (PSV kernel)
+  int out_tma;                   // the output tile is staged in a per-consumer shared-memory buffer and written by TMA
+  uint32_t out_off;              // byte offset of those buffers from the ring ([128 pixels][NB] 16-bit each)
 };
 
 // MODE 1 shapes whose tap / K-step loops are unrolled at compile time: KS x KS taps and KST K = 16 steps in every channel
@@ -70,21 +76,54 @@ struct TcP {
 static constexpr int FIX_KS = 3, FIX_KST = 3;
 __host__ __device__ constexpr bool fixed_nb(int nb) { return nb == 16 || nb == 48 || nb == 96; }
 
+// Timeline instrumentation, compiled only with -DRV_CONV_TIMELINE into a separate library (tools/conv_timeline.py); the
+// product library has none of it.  One thread per role (0 = producer, 1 + c = consumer c) writes clock64 stamps of its
+// i-th local tile: tl[cta][role][i][event], cta = blockIdx.y * gridDim.x + blockIdx.x.
+//   producer: 0 empty-slot wait start, 1 wait end, 2 TMA issued
+//   consumer: 0 full-slot wait start, 1 wait end, 2 first wgmma issued, 3 wgmma.wait_group 0 returned,
+//             4 epilogue-buffer wait end, 5 epilogue end
+// tl_diag splits the cost (S = 1 convs only): 1 = MMA-only (every tile re-issues its batch on the consumer's first,
+// resident slot: no full-slot waits after the first, no slot release, no epilogue), 2 = the same with every A view on a
+// 1024-byte swizzle atom (wrong values, same wgmma count), 3 = epilogue-only (no A loads, no MMAs).
+#ifdef RV_CONV_TIMELINE
+static constexpr int TL_TILES = 128, TL_EV = 8, TL_ROLES = 1 + NCONS;
+__device__ long long* g_tl;
+__device__ int g_tl_diag;
+static int g_tl_max_slots = 0;   // host: ring slots per consumer at most (0: the plan's)
+__device__ __forceinline__ void tl_stamp(long long* tl, int role, int it, int ev) {
+  if (tl != nullptr && it < TL_TILES) {
+    long long c;
+    asm volatile("mov.u64 %0, %%clock64;" : "=l"(c) :: "memory");
+    tl[(((size_t)(blockIdx.y * gridDim.x + blockIdx.x) * TL_ROLES + role) * TL_TILES + it) * TL_EV + ev] = c;
+  }
+}
+// the buffer pointer and the variant are read once per thread (RV_TL_INIT), so that a stamp costs a clock read and a
+// store, and a variant test no global load
+#define RV_TL_INIT long long* const tl_buf = g_tl; const int tl_diag = g_tl_diag
+#define RV_TL(on, role, it, ev) do { if (on) tl_stamp(tl_buf, role, it, ev); } while (0)
+#define RV_TL_DIAG tl_diag
+#else
+#define RV_TL_INIT do { } while (0)
+#define RV_TL(on, role, it, ev) do { } while (0)
+#define RV_TL_DIAG 0
+#endif
+
 // All MMAs of one pipeline stage into both 64-row halves.  Descriptor start addresses are in 16-byte units: +2 per
 // K = 16 slice of a 128-byte row, whole rows per tap.  KS > 0 (MODE 1 only): kh = kw = KS and KST K-steps per chunk known
 // at compile time, so the stage is one unbranched run of wgmmas that ptxas issues behind a single warpgroup.arrive; the
 // MMA order per accumulator half (ky, kx, k) is the runtime loop's, so the results are the same bits.
-template <int MODE, bool BF, int NB, int KS = 0, int KST = 0>
+// ALIGNED (timeline diagnostic only): every A view at the slot's first swizzle atom, 8-row groups 1024 bytes apart.
+template <int MODE, bool BF, int NB, int KS = 0, int KST = 0, bool ALIGNED = false>
 __device__ __forceinline__ void issue_stage(const TcP& p, float (&acc)[2][NB / 2], uint32_t a_addr, uint32_t b_addr,
                                             int s, int ksteps) {
   if constexpr (MODE == 1 && KS > 0) {
-    constexpr uint32_t sbo = (uint32_t)(8 + KS - 1) * 128;   // box width bw = tw + KS - 1 pixels of 128 bytes
+    constexpr uint32_t sbo = ALIGNED ? 1024u : (uint32_t)(8 + KS - 1) * 128;   // box width bw = tw + KS - 1 pixels of 128 bytes
 #pragma unroll
     for (int ky = 0; ky < KS; ++ky)
 #pragma unroll
       for (int kx = 0; kx < KS; ++kx) {
         const uint64_t bd = tc::desc_sw128(b_addr + (uint32_t)((ky * KS + kx) * NB * 128));
-        const uint32_t at = a_addr + (uint32_t)((ky * (8 + KS - 1) + kx) * 128);
+        const uint32_t at = a_addr + (ALIGNED ? 0u : (uint32_t)((ky * (8 + KS - 1) + kx) * 128));
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const uint64_t ad = tc::desc_sw128(at + (uint32_t)h * 8 * sbo, sbo);
@@ -182,10 +221,11 @@ __device__ __forceinline__ uint32_t pack2(float a, float b) {
 template <typename TI, typename TR, typename TO, int MODE, int NB, int KS, int KST, bool PSV>
 __global__ void __launch_bounds__(128 * (1 + NCONS), 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1,
-               const __grid_constant__ CUtensorMap tmg, const __grid_constant__ CUtensorMap tmr, const TcP p) {
+               const __grid_constant__ CUtensorMap tmg, const __grid_constant__ CUtensorMap tmr,
+               const __grid_constant__ CUtensorMap tmo, const TcP p) {
   constexpr bool BF = std::is_same<TI, __nv_bfloat16>::value;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ uint64_t bar_full[NCONS][MAX_SLOTS], bar_empty[NCONS][MAX_SLOTS], bar_w, bar_epi[NCONS];
+  __shared__ uint64_t bar_full[NCONS][MAX_SLOTS], bar_empty[NCONS][MAX_SLOTS], bar_w, bar_epi[NCONS], bar_turn[NCONS];
   __shared__ __align__(16) float bias_s[MAX_NB];
 
   const uint32_t raw = tc::smem_u32(smem_raw);
@@ -197,6 +237,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
   const int nblk = blockIdx.y;
   const int ntiles = p.tiles_x * p.tiles_y;
   const int nchunks = p.nch0 + p.nch1;
+  RV_TL_INIT;
 
   // Programmatic dependent launch: the next kernel of the stream may start its prologue now; activations are read and
   // written only after griddepcontrol.wait, while barrier init, bias and the (constant) weight fetch overlap the tail
@@ -210,6 +251,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
       }
     tc::mbar_init(&bar_w, 1);
     for (int c = 0; c < NCONS; ++c) tc::mbar_init(&bar_epi[c], 1);
+    for (int c = 0; c < NCONS; ++c) tc::mbar_init(&bar_turn[c], 4);   // one arrival per warp of the other consumer
     tc::fence_barrier_init();
     tc::prefetch_tmap(&tm0);
     if (p.nch1 || p.nq1) tc::prefetch_tmap(&tm1);
@@ -232,14 +274,19 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
     const uint32_t tx_bytes = p.a_tx + (p.resident ? 0u : p.w_bytes);
     int slot[NCONS] = {0, 0};
     uint32_t ph[NCONS] = {0u, 0u};
-    int cons = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    int cons = 0, it = 0;
+    const bool tl0 = threadIdx.x == 0;
+    (void)tl0;
+    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
+      if (RV_TL_DIAG == 3 || (RV_TL_DIAG != 0 && it >= NCONS)) break;   // diagnostics: only the resident slots / nothing
       const int ty0 = tile / p.tiles_x, tx0 = tile - ty0 * p.tiles_x;
       const int yc = ty0 * p.th - p.pad, xc = tx0 * p.tw - p.pad;
       int kx = 0, ch = 0;
       for (int s = 0; s < p.S; ++s) {
         const int sl = slot[cons];
+        RV_TL(tl0 && s == 0, 0, it, 0);
         tc::mbar_wait(&bar_empty[cons][sl], ph[cons] ^ 1u);
+        RV_TL(tl0 && s == 0, 0, it, 1);
         if (tc::elect_one()) {
           uint64_t* bar = &bar_full[cons][sl];
           uint8_t* dst = ring + ((size_t)cons * p.slots + sl) * p.slot_bytes;
@@ -256,6 +303,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
           if (!p.resident) tc::bulk_load(wsrc + (size_t)s * p.w_bytes, bar, dst + p.a_bytes, p.w_bytes);
         }
         __syncwarp();
+        RV_TL(tl0 && s == p.S - 1, 0, it, 2);
         // stage order: mode 0 = (kx, chunk), mode 1 = (chunk), mode 2 = (kx)
         if (MODE == 2) ++kx;
         else if (++ch == nchunks) { ch = 0; kx += (MODE == 1) ? 0 : 1; }
@@ -276,6 +324,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
     asm volatile("griddepcontrol.wait;" ::: "memory");     // gate / residual reads and all stores come after this
     int slot = 0;
     uint32_t ph = 0;
+    // Compile-time kernels: the consumers take turns on the tensor cores.  A consumer issues a tile's MMAs only after the
+    // other consumer has issued its previous tile's MMAs (consumer 0 starts), so the batches queue back to back and one
+    // consumer's epilogue runs under the other's MMAs; left alone, both consumers tend to issue at once, share the tensor
+    // cores, and then both run their epilogues with the tensor cores idle.
+    constexpr bool TURNS = KS > 0;
+    uint32_t tph = 0;
     float acc[2][NB / 2];
     // Up to NB = 48 the epilogue takes a tile's gate and residual values from registers filled before it starts (loaded
     // where they are used, each pair's load would cost the epilogue a full global-memory latency):
@@ -303,8 +357,24 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
       tc::prefetch_tmap(&tmr);
       epi_load(blockIdx.x + cons * gridDim.x);
     }
-    for (int tile = blockIdx.x + cons * gridDim.x; tile < ntiles; tile += NCONS * gridDim.x) {
+    // p.out_tma (compile-time 3 x 3 kernels up to NB = 48 with a 16-bit output TMA can address): the epilogue writes the
+    // tile's values into this consumer's [128 pixels][NB] buffer with no bounds branches, and one thread stores the buffer
+    // with TMA, which clips edge tiles and channels >= cout.  Otherwise each thread stores its channel pairs itself.
+    constexpr bool OUT_TMA_OK = KS > 0 && !PSV && EARLY && sizeof(TO) == 2;
+    const bool out_tma = OUT_TMA_OK && p.out_tma;
+    uint8_t* out_s = ring + p.out_off + (size_t)cons * p.epi_bytes;
+    if (out_tma && t == 0) tc::prefetch_tmap(&tmo);
+    int it = 0;
+    const bool tl0 = t == 0;
+    (void)tl0;
+    for (int tile = blockIdx.x + cons * gridDim.x; tile < ntiles; tile += NCONS * gridDim.x, ++it) {
       const int ty0 = tile / p.tiles_x, tx0 = tile - ty0 * p.tiles_x;
+      if (RV_TL_DIAG == 3) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int i = 0; i < NB / 2; ++i) acc[h][i] = 0.f;
+      }
       typename RawPair<TI>::type gv[2][2][NJ];   // [h][r2][j], as the epilogue below indexes the accumulators
       typename RawPair<TR>::type rv[2][2][NJ];
       if (EARLY && !epi_tma) {
@@ -334,12 +404,23 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
           ksteps = (min(crem, 64) + 15) >> 4;
           if (++ch == nchunks) ch = 0;
         }
-        tc::mbar_wait(&bar_full[cons][slot], ph);
+        if (RV_TL_DIAG == 3) break;
+        RV_TL(tl0 && s == 0, 1 + cons, it, 0);
+        if (RV_TL_DIAG == 0 || it == 0) tc::mbar_wait(&bar_full[cons][slot], ph);
+        if (TURNS && s == 0 && (cons != 0 || it != 0)) {
+          tc::mbar_wait(&bar_turn[cons], tph);
+          tph ^= 1u;
+        }
+        RV_TL(tl0 && s == 0, 1 + cons, it, 1);
         const uint32_t a_addr = ring_addr + (uint32_t)slot * p.slot_bytes;
         const uint32_t b_addr = p.resident ? w_addr + (uint32_t)s * p.w_bytes : a_addr + p.a_bytes;
         tc::wgmma_fence();
-        issue_stage<MODE, BF, NB, KS, KST>(p, acc, a_addr, b_addr, s, ksteps);
+        RV_TL(tl0 && s == 0, 1 + cons, it, 2);
+        if (RV_TL_DIAG == 2) issue_stage<MODE, BF, NB, KS, KST, true>(p, acc, a_addr, b_addr, s, ksteps);
+        else issue_stage<MODE, BF, NB, KS, KST>(p, acc, a_addr, b_addr, s, ksteps);
         tc::wgmma_commit();
+        if (TURNS && s == p.S - 1 && lane == 0) tc::mbar_arrive(&bar_turn[cons ^ 1]);   // the other consumer's turn
+        if (RV_TL_DIAG != 0) continue;    // MMA-only: the slot stays resident (S = 1)
         if (p.slots == 1) {
           // a single slot is refilled only after these MMAs have read it
           tc::wgmma_wait<0>();
@@ -353,6 +434,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
         if (++slot == p.slots) { slot = 0; ph ^= 1u; }
       }
       tc::wgmma_wait<0>();
+      RV_TL(tl0, 1 + cons, it, 3);
+      if (RV_TL_DIAG == 1 || RV_TL_DIAG == 2) continue;
       if (prev >= 0 && lane == 0) tc::mbar_arrive(&bar_empty[cons][prev]);
       if constexpr (TMA_OK) {
         if (epi_tma) {
@@ -377,6 +460,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
           }
         }
       }
+      RV_TL(tl0, 1 + cons, it, 4);
 
       // ---- epilogue: thread t holds rows 64 h + 16 wq + lane / 4 (+ 8) and column pairs 8 j + 2 (lane % 4) ----
       if constexpr (PSV) {
@@ -420,7 +504,52 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
             }
           }
         }
+        RV_TL(tl0, 1 + cons, it, 5);
         continue;
+      }
+      if constexpr (OUT_TMA_OK) {
+        if (out_tma) {
+          if (t == 0) tc::bulk_wait_read<0>();      // this consumer's previous store has read the buffer
+          asm volatile("bar.sync %0, 128;" ::"r"(1 + cons) : "memory");
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int r2 = 0; r2 < 2; ++r2) {
+              const int m = 64 * h + 16 * wq + (lane >> 2) + 8 * r2;
+#pragma unroll
+              for (int j = 0; j < NJ; ++j) {
+                const int nl = 8 * j + 2 * (lane & 3);
+                float v[2];
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  const float x = acc[h][4 * j + 2 * r2 + e] + bias_s[nl + e];
+                  v[e] = fmaxf(x, x * p.pre_slope);
+                }
+                if (gate != nullptr) {
+                  const float2 g = raw2_to_f2<TI>(gv[h][r2][j]);
+                  v[0] *= g.x; v[1] *= g.y;
+                }
+                if (res != nullptr) {
+                  const float2 r = raw2_to_f2<TR>(rv[h][r2][j]);
+                  v[0] += r.x; v[1] += r.y;
+                }
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  v[e] = fmaxf(v[e], v[e] * p.post_slope);
+                  if (p.post_clamp3) v[e] = fminf(fmaxf(v[e], -3.f), 3.f);
+                }
+                *reinterpret_cast<uint32_t*>(out_s + (uint32_t)(m * NB + nl) * 2u) = pack2<TO>(v[0], v[1]);
+              }
+            }
+          tc::fence_proxy_async();                  // the buffer's writes, before the async proxy reads them
+          asm volatile("bar.sync %0, 128;" ::"r"(1 + cons) : "memory");
+          if (t == 0) {
+            tc::tma_store_3d(&tmo, out_s, nblk * NB, tx0 * p.tw, ty0 * p.th);
+            tc::bulk_commit();
+          }
+          RV_TL(tl0, 1 + cons, it, 5);
+          continue;
+        }
       }
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
@@ -469,7 +598,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
           }
         }
       }
+      RV_TL(tl0, 1 + cons, it, 5);
     }
+    if (out_tma && t == 0) tc::bulk_wait<0>();     // the last stores are complete before the CTA exits
   }
 }
 
@@ -487,13 +618,15 @@ PFN_tmapEncodeTiled get_tmap_encoder() {
   return fn;
 }
 
-// 16-bit NHWC map [H][W][C], boxes of box_c x box_w x box_rows; out-of-bounds elements read as zero
+// 16-bit NHWC map [H][W][C] with `cs` (default C) channels between pixels, boxes of box_c x box_w x box_rows;
+// out-of-bounds elements read as zero and are not written
 static int make_tmap_3d(CUtensorMap* m, const void* ptr, int C, int W, int H, int box_c, int box_w, int box_rows, int fmt,
-                        CUtensorMapSwizzle swz) {
+                        CUtensorMapSwizzle swz, int cs = 0) {
   PFN_tmapEncodeTiled enc = get_tmap_encoder();
   if (!enc) return fail(RV_E_CUDA, "cuTensorMapEncodeTiled entry point not available");
+  if (cs == 0) cs = C;
   cuuint64_t gdim[3] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H};
-  cuuint64_t gstr[2] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2};
+  cuuint64_t gstr[2] = {(cuuint64_t)cs * 2, (cuuint64_t)W * cs * 2};
   cuuint32_t box[3] = {(cuuint32_t)box_c, (cuuint32_t)box_w, (cuuint32_t)box_rows};
   cuuint32_t estr[3] = {1, 1, 1};
   CUresult r = enc(m, fmt ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3,
@@ -531,7 +664,7 @@ static int launch_tc_mode(const CUtensorMap* tm, const TcP& p, dim3 grid, size_t
   static const bool use_pdl = getenv("REFVSR_NO_PDL") == nullptr;
   cfg.attrs = attr;
   cfg.numAttrs = use_pdl ? 1 : 0;
-  RV_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tm[0], tm[1], tm[2], tm[3], p));
+  RV_CUDA_OK(cudaLaunchKernelEx(&cfg, kern, tm[0], tm[1], tm[2], tm[3], tm[4], p));
   RV_LAUNCH_CHECK("conv_tc");
   return RV_OK;
 }
@@ -624,10 +757,26 @@ static int plan_tc(const rv_conv_desc* d, TcP& p, size_t& smem_out, int& nblk_ou
   p.epi_tma = (d->gate || d->res) && p.NB <= 48 && rdt0 == d->in_dtype && tma_ok(d->gate, d->gate_cs) &&
               tma_ok(d->res, d->res_cs) && w_all + ring_min + (size_t)NCONS * p.epi_tx <= budget;
   const size_t epi_all = p.epi_tma ? (size_t)NCONS * p.epi_tx : 0;
-  if (w_all + ring_min + epi_all <= budget) {
+  // the compile-time tap loop: a square FIX_KS kernel whose every channel chunk takes FIX_KST K-steps (e.g. 48 + 48
+  // channels, not 8 + 48); other shapes keep the runtime loop
+  p.fixed = p.mode == 1 && d->kh == FIX_KS && d->kw == FIX_KS && fixed_nb(p.NB);
+  for (int ch = 0; ch < p.nch0 + p.nch1 && p.fixed; ++ch) {
+    const int crem = (ch < p.nch0) ? (p.c0 - ch * 64) : (p.c1 - (ch - p.nch0) * 64);
+    p.fixed = (std::min(crem, 64) + 15) / 16 == FIX_KST;
+  }
+  // TMA-store epilogue: compile-time kernels up to NB = 48 writing a plain (not pixel-shuffled) map of the input's 16-bit
+  // type whose base and pixel stride TMA can address, when a [128 pixels][NB] buffer per consumer fits next to the
+  // resident weights, the gate / residual buffers and the minimal ring
+  p.out_tma = p.fixed && p.NB <= 48 && !d->pixel_shuffle && d->out_dtype == d->in_dtype && d->out != nullptr &&
+              tma_ok(d->out, d->out_cs) && w_all + ring_min + epi_all + (size_t)NCONS * p.epi_bytes <= budget;
+  const size_t out_all = p.out_tma ? (size_t)NCONS * p.epi_bytes : 0;
+  if (w_all + ring_min + epi_all + out_all <= budget) {
     p.resident = 1;
     p.slot_bytes = p.a_bytes;
-    p.slots = (int)std::min<size_t>(MAX_SLOTS, (budget - w_all - epi_all) / ((size_t)NCONS * p.a_bytes));
+    p.slots = (int)std::min<size_t>(MAX_SLOTS, (budget - w_all - epi_all - out_all) / ((size_t)NCONS * p.a_bytes));
+#ifdef RV_CONV_TIMELINE
+    if (g_tl_max_slots > 0) p.slots = std::min(p.slots, g_tl_max_slots);
+#endif
   } else {
     RV_REQUIRE(p.mode != 1, "rv_conv2d(tc): layout 1 weights do not fit in shared memory");
     p.resident = 0;
@@ -635,7 +784,8 @@ static int plan_tc(const rv_conv_desc* d, TcP& p, size_t& smem_out, int& nblk_ou
     p.slots = (int)std::min<size_t>(MAX_SLOTS, budget / ((size_t)NCONS * p.slot_bytes));
     RV_REQUIRE(p.slots >= 1, "rv_conv2d(tc): stage of %u bytes does not fit once per consumer in shared memory", p.slot_bytes);
   }
-  const size_t smem = 1024 + (p.resident ? w_all : 0) + (size_t)NCONS * p.slots * p.slot_bytes + epi_all;
+  p.out_off = (uint32_t)((size_t)NCONS * p.slots * p.slot_bytes + epi_all);
+  const size_t smem = 1024 + (p.resident ? w_all : 0) + (size_t)NCONS * p.slots * p.slot_bytes + epi_all + out_all;
   p.wpack = (const uint8_t*)d->wpack; p.bias = d->bias;
   auto slope = [](int act) { return act == RV_ACT_RELU ? 0.f : act == RV_ACT_LRELU01 ? 0.1f : act == RV_ACT_LRELU02 ? 0.2f : 1.f; };
   RV_REQUIRE(d->act_pre != RV_ACT_CLAMP3, "rv_conv2d(tc): clamp3 is only supported as act_post");
@@ -648,13 +798,6 @@ static int plan_tc(const rv_conv_desc* d, TcP& p, size_t& smem_out, int& nblk_ou
   auto al = [](const void* q, int cs, int dt) { return q == nullptr || (((uintptr_t)q % (2 * dtype_size(dt)) == 0) && cs % 2 == 0); };
   p.pair_ok = al(d->out, d->out_cs, d->out_dtype) && al(d->gate, d->gate_cs, d->in_dtype) && al(d->res, d->res_cs, rdt);
   p.fmt = d->in_dtype == RV_BF16 ? 1 : 0;
-  // the compile-time tap loop: a square FIX_KS kernel whose every channel chunk takes FIX_KST K-steps (e.g. 48 + 48
-  // channels, not 8 + 48); other shapes keep the runtime loop
-  p.fixed = p.mode == 1 && d->kh == FIX_KS && d->kw == FIX_KS && fixed_nb(p.NB);
-  for (int ch = 0; ch < p.nch0 + p.nch1 && p.fixed; ++ch) {
-    const int crem = (ch < p.nch0) ? (p.c0 - ch * 64) : (p.c1 - (ch - p.nch0) * 64);
-    p.fixed = (std::min(crem, 64) + 15) / 16 == FIX_KST;
-  }
   // the upsampling convs (compile-time 3 x 3 loop, NB = 96, pixel shuffle into a 16-bit map, no gate / residual): a thread
   // gathers one output pixel's 24 channels and stores them as three 16-byte vectors, when every channel of the block
   // exists and the pixel rows stay 16-byte aligned; other pixel shuffles keep the 2-byte stores
@@ -681,10 +824,10 @@ int conv2d_tc(const rv_conv_desc* d, cudaStream_t st) {
   }
   const int rdt = d->res ? d->res_dtype : d->out_dtype;
   const int sw32 = p.mode == 2;
-  CUtensorMap tm[4];    // src0, src1, gate, res (unused ones: copies of src0)
+  CUtensorMap tm[5];    // src0, src1, gate, res, out (unused ones: copies of src0)
   int rc = make_act_tmap(&tm[0], d->src0, p.c0, d->W, d->H, p.mode == 1 ? p.tw + d->kw - 1 : p.tw, p.th + d->kh - 1, p.fmt, sw32);
   if (rc) return rc;
-  tm[1] = tm[2] = tm[3] = tm[0];
+  tm[1] = tm[2] = tm[3] = tm[4] = tm[0];
   if (p.c1) {
     rc = make_act_tmap(&tm[1], d->src1, p.c1, d->W, d->H, p.mode == 1 ? p.tw + d->kw - 1 : p.tw, p.th + d->kh - 1, p.fmt, sw32);
     if (rc) return rc;
@@ -693,6 +836,9 @@ int conv2d_tc(const rv_conv_desc* d, cudaStream_t st) {
   if (p.epi_tma && d->gate && (rc = make_tmap_3d(&tm[2], d->gate, d->gate_cs, p.Wo, p.Ho, p.NB, p.tw, p.th, p.fmt, CU_TENSOR_MAP_SWIZZLE_NONE)))
     return rc;
   if (p.epi_tma && d->res && (rc = make_tmap_3d(&tm[3], d->res, d->res_cs, p.Wo, p.Ho, p.NB, p.tw, p.th, p.fmt, CU_TENSOR_MAP_SWIZZLE_NONE)))
+    return rc;
+  // output tiles [th][tw][NB] of the TMA-store epilogue; channels >= cout (and pixels outside the map) are not written
+  if (p.out_tma && (rc = make_tmap_3d(&tm[4], d->out, d->cout, p.Wo, p.Ho, p.NB, p.tw, p.th, p.fmt, CU_TENSOR_MAP_SWIZZLE_NONE, d->out_cs)))
     return rc;
   const int ntiles = p.tiles_x * p.tiles_y;
   int gx = std::min(ntiles, std::max(1, g_num_sms / nblk));
@@ -723,3 +869,23 @@ int conv2d_tc_plan(const rv_conv_desc* d, int max_smem, int num_sms, int* out) {
 }
 
 }  // namespace rv
+
+#ifdef RV_CONV_TIMELINE
+// instrumented library only: stamp buffer (nullptr: off) of TL_ROLES x TL_TILES x TL_EV int64 per CTA, and the diagnostic
+// variant (0 = the product kernel) for the following launches
+extern "C" int rv_conv_timeline_set(void* buf, int diag) {
+  long long* b = static_cast<long long*>(buf);
+  if (cudaMemcpyToSymbol(rv::g_tl, &b, sizeof(b)) != cudaSuccess) return 1;
+  if (cudaMemcpyToSymbol(rv::g_tl_diag, &diag, sizeof(diag)) != cudaSuccess) return 1;
+  return 0;
+}
+extern "C" int rv_conv_timeline_max_slots(int n) {
+  const int old = rv::g_tl_max_slots;
+  rv::g_tl_max_slots = n;
+  return old;
+}
+extern "C" int rv_conv_timeline_dims(int* out3) {
+  out3[0] = rv::TL_ROLES; out3[1] = rv::TL_TILES; out3[2] = rv::TL_EV;
+  return 0;
+}
+#endif

@@ -65,6 +65,20 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* m, uint64_t* bar,
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
+// shared -> global tensor store of one box (out-of-bounds elements are not written), tracked by the issuing thread's
+// bulk async-groups: commit after the stores of a buffer, wait_read<0> before that buffer is written again, wait<0> before
+// the thread exits
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, const void* smem, int c0, int c1, int c2) {
+  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(m)),
+               "r"(smem_u32(smem)), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 // plain (non-tensor) bulk copy global -> shared; bytes % 16 == 0, both addresses 16-byte aligned
 __device__ __forceinline__ void bulk_load(const void* gmem, uint64_t* bar, void* smem, uint32_t bytes) {
   asm volatile(
