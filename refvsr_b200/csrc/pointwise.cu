@@ -109,6 +109,25 @@ __device__ __forceinline__ Vec<T, V> blend4(const Vec<T, V>& a, const Vec<T, V>&
   return r;
 }
 
+// The same blend in the order the compiler contracts aligned_sample_kernel's `lt * a + rb * b + lb * c + rt * d`:
+// fma(d, w.w, fma(c, w.z, fma(a, w.x, b * w.y))) - for the fast paths that must reproduce that kernel bit for bit.
+template <typename T, int V>
+__device__ __forceinline__ Vec<T, V> blend4_as_generic(const Vec<T, V>& a, const Vec<T, V>& b, const Vec<T, V>& c, const Vec<T, V>& d,
+                                                       float4 w) {
+  static_assert(V % 2 == 0, "blend4 works on pairs");
+  const float2 wx = make_float2(w.x, w.x), wy = make_float2(w.y, w.y), wz = make_float2(w.z, w.z), ww = make_float2(w.w, w.w);
+  Vec<T, V> r;
+#pragma unroll
+  for (int k = 0; k < V; k += 2) {
+    float2 acc = fmul2(unpack2<T>(&b.v[k]), wy);
+    acc = ffma2(unpack2<T>(&a.v[k]), wx, acc);
+    acc = ffma2(unpack2<T>(&c.v[k]), wz, acc);
+    acc = ffma2(unpack2<T>(&d.v[k]), ww, acc);
+    pack2<T>(&r.v[k], acc);
+  }
+  return r;
+}
+
 // torch.linspace(-1, 1, n)[i]  (symmetric evaluation, aten RangeFactories)
 __device__ __forceinline__ float linspace_m1_1(int i, int n) {
   if (n == 1) return -1.f;
@@ -630,7 +649,7 @@ __global__ void gather_blocks_kernel(const uint8_t* __restrict__ value, int Hv, 
   else *reinterpret_cast<uint16_t*>(d) = *reinterpret_cast<const uint16_t*>(s);
 }
 
-// 16-byte rows, ks = 1 / 2: one thread = one (cell, 16-byte vector) - the index lookup and its division are done once per
+// 16-byte rows, ks = 1 / 2 / 4: one thread = one (cell, 16-byte vector) - the index lookup and its division are done once per
 // cell and the thread then moves the ks * ks pixels of the cell (the per-output-vector version above spends ~190 instructions,
 // six integer divisions among them, on every 16 bytes).  blockIdx.y = cell row.  Pure copies: bit-identical.
 template <int KS, int NVC>
@@ -776,6 +795,68 @@ __global__ void __launch_bounds__(256) aligned_sample2_kernel(const T* __restric
     const Vec<T, V> t_lt = ldvi<T, V>(x, o.x * cv + vc), t_rb = ldvi<T, V>(x, o.y * cv + vc),
                     t_lb = ldvi<T, V>(x, o.z * cv + vc), t_rt = ldvi<T, V>(x, o.w * cv + vc);
     stvi<T, V>(out, (Y * W + X) * cv + vc, blend4<T, V>(t_lt, t_rb, t_lb, t_rt, g));
+  }
+}
+
+// ks = 4 (aa2 of the x2 models, aa1 of the flag_HD_in models): the sibling of aligned_sample2_kernel on tiles of 8 x 8 cells =
+// 32 x 32 output pixels.  Phase 1 evaluates the 16 sampling positions of a cell once (sin / cos once per cell instead of once per
+// channel vector of every pixel), phase 2 is the same 4-tap gather.  Bit-identical to aligned_sample_kernel: the rotation and
+// the blend are written out in the order the compiler contracts that kernel's expressions.
+template <typename T, int CV>
+__global__ void __launch_bounds__(256) aligned_sample4_kernel(const T* __restrict__ x, int h, int w, int C,
+                                                              const float* __restrict__ affine, T* __restrict__ out) {
+  constexpr int V = 16 / (int)sizeof(T);
+  constexpr int ks = 4, AS_TH = 8, AS_TW = 8, NC = AS_TH * AS_TW, NP = ks * ks * NC, PW = ks * AS_TW;
+  __shared__ float4 s_w[NP];
+  __shared__ int4 s_o[NP];
+  const int H = ks * h, W = ks * w, Hp = H + 2, Wp = W + 2;
+  const int tiles_x = (w + AS_TW - 1) / AS_TW;
+  const int ci0 = (blockIdx.x / tiles_x) * AS_TH, cj0 = (blockIdx.x % tiles_x) * AS_TW;
+  const int Y0 = ks * ci0, X0 = ks * cj0;
+  for (int c = threadIdx.x; c < NC; c += blockDim.x) {
+    const int li = c / AS_TW, lj = c % AS_TW;
+    const int ci = ci0 + li, cj = cj0 + lj;
+    if (ci >= h || cj >= w) continue;                       // (entries of cells outside the image are never read)
+    const float* af = affine + ((size_t)ci * w + cj) * 3;
+    const float s_x = af[0], s_y = af[1], th = (af[2] - 1.0f) * 1.0472f;
+    const float half = (float)((ks - 1) / 2) + 0.5f;
+    const float cs = cosf(th), sn = sinf(th);
+    const float Hm = (float)(Hp - 1), Wm = (float)(Wp - 1);
+#pragma unroll
+    for (int a = 0; a < ks; ++a)
+#pragma unroll
+      for (int b = 0; b < ks; ++b) {
+        const float u = ((float)a - half) * s_x, v = ((float)b - half) * s_y;
+        // the contraction aligned_sample_kernel gets from the compiler, spelled out: with a, b known here the compiler would
+        // otherwise fuse the other product of each pair (its products of v are shared across rows)
+        const float rr = __fmaf_rn(u, cs, -__fmul_rn(v, sn)), cc = __fmaf_rn(v, cs, __fmul_rn(u, sn));
+        float pr = rr + half + (float)(1 + ci * ks);
+        float pc = cc + half + (float)(1 + cj * ks);
+        float ltr = floorf(pr), ltc = floorf(pc);
+        float rbr = ltr + 1.f, rbc = ltc + 1.f;
+        ltr = fminf(fmaxf(ltr, 0.f), Hm); rbr = fminf(fmaxf(rbr, 0.f), Hm);
+        ltc = fminf(fmaxf(ltc, 0.f), Wm); rbc = fminf(fmaxf(rbc, 0.f), Wm);
+        pr = fminf(fmaxf(pr, 0.f), Hm); pc = fminf(fmaxf(pc, 0.f), Wm);
+        const int r0 = reflect1((int)ltr - 1, H), r1 = reflect1((int)rbr - 1, H);
+        const int c0 = reflect1((int)ltc - 1, W), c1 = reflect1((int)rbc - 1, W);
+        const int e = (ks * li + a) * PW + ks * lj + b;
+        // order (lt, rb, lb, rt) as in aligned_sample_kernel
+        s_w[e] = make_float4((1.f + (ltr - pr)) * (1.f + (ltc - pc)), (1.f - (rbr - pr)) * (1.f - (rbc - pc)),
+                             (1.f + (ltr - pr)) * (1.f - (rbc - pc)), (1.f - (rbr - pr)) * (1.f + (ltc - pc)));
+        s_o[e] = make_int4(r0 * W + c0, r1 * W + c1, r0 * W + c1, r1 * W + c0);
+      }
+  }
+  __syncthreads();
+  const int cv = CV > 0 ? CV : C / V;
+  for (int it = threadIdx.x; it < NP * cv; it += blockDim.x) {
+    const int pl = it / cv, vc = it - pl * cv;
+    const int Y = Y0 + pl / PW, X = X0 + pl % PW;
+    if (Y >= H || X >= W) continue;
+    const float4 g = s_w[pl];
+    const int4 o = s_o[pl];
+    const Vec<T, V> t_lt = ldvi<T, V>(x, o.x * cv + vc), t_rb = ldvi<T, V>(x, o.y * cv + vc),
+                    t_lb = ldvi<T, V>(x, o.z * cv + vc), t_rt = ldvi<T, V>(x, o.w * cv + vc);
+    stvi<T, V>(out, (Y * W + X) * cv + vc, blend4_as_generic<T, V>(t_lt, t_rb, t_lb, t_rt, g));
   }
 }
 
@@ -986,6 +1067,68 @@ __global__ void __launch_bounds__(128) reconstruct4_kernel(const float4* __restr
   }
 }
 
+// one horizontal tap row of bicubic_planar as reconstruct_kernel evaluates it: fma(w3, v3, fma(w2, v2, fma(w0, v0, w1 * v1)))
+__device__ __forceinline__ float row4(const float* wt, float v0, float v1, float v2, float v3) {
+  return __fmaf_rn(wt[3], v3, __fmaf_rn(wt[2], v2, __fmaf_rn(wt[0], v0, __fmul_rn(wt[1], v1))));
+}
+
+// x2 fast path, the counterpart of reconstruct4_kernel: one thread per LR pixel produces its 2 x 2 output pixels from one shared
+// 5 x 5 LR neighbourhood (phase 0 looks left / up: taps l-2 .. l+1, phase 1 right / down: l-1 .. l+2).  conv_last's output is read
+// as 16-byte vectors, the planar result written as 8-byte pairs.  Weights, taps and summation are those of bicubic_planar, with
+// the products fused the way the compiler contracts it (bit-identical to reconstruct_kernel at scale 2; the weights here are
+// compile-time constants, which would otherwise let the compiler fuse the other product of a row).
+__global__ void __launch_bounds__(128) reconstruct2_kernel(const float4* __restrict__ x, const float* __restrict__ lr, int h, int w,
+                                                           int clamp01, float* __restrict__ out) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= h * w) return;
+  const int ly = p / w, lx = p - ly * w;
+  const int Ho = 2 * h, Wo = 2 * w;
+  float wt[2][4];
+#pragma unroll
+  for (int a = 0; a < 2; ++a) {
+    const float r = 0.5f * ((float)a + 0.5f) - 0.5f;           // fractional part of the source coordinate of phase a
+    cubic_weights(r - floorf(r), wt[a]);
+  }
+  int ry[5], rx[5];
+#pragma unroll
+  for (int i = 0; i < 5; ++i) { ry[i] = clampi(ly - 2 + i, 0, h - 1); rx[i] = clampi(lx - 2 + i, 0, w - 1); }
+  float res[3][2][2];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const float* s = lr + (size_t)c * h * w;
+    float hrow[2][5];                                          // [phase b][neighbourhood row]
+#pragma unroll
+    for (int i = 0; i < 5; ++i) {
+      const float* r = s + (size_t)ry[i] * w;
+      const float v0 = __ldg(r + rx[0]), v1 = __ldg(r + rx[1]), v2 = __ldg(r + rx[2]), v3 = __ldg(r + rx[3]), v4 = __ldg(r + rx[4]);
+      hrow[0][i] = row4(wt[0], v0, v1, v2, v3);
+      hrow[1][i] = row4(wt[1], v1, v2, v3, v4);
+    }
+#pragma unroll
+    for (int a = 0; a < 2; ++a) {
+#pragma unroll
+      for (int b = 0; b < 2; ++b) {
+        float acc = 0.f;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc = __fmaf_rn(wt[a][j], hrow[b][a + j], acc);
+        res[c][a][b] = fminf(fmaxf(acc, 0.f), 1.f);
+      }
+    }
+  }
+#pragma unroll
+  for (int a = 0; a < 2; ++a) {
+    const size_t row = (size_t)(2 * ly + a) * Wo + 2 * lx;
+    const float4 x0 = __ldg(x + row), x1 = __ldg(x + row + 1);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      float v0 = ((c == 0) ? x0.x : (c == 1 ? x0.y : x0.z)) + res[c][a][0];
+      float v1 = ((c == 0) ? x1.x : (c == 1 ? x1.y : x1.z)) + res[c][a][1];
+      if (clamp01) { v0 = fminf(fmaxf(v0, 0.f), 1.f); v1 = fminf(fmaxf(v1, 0.f), 1.f); }
+      *reinterpret_cast<float2*>(out + (size_t)c * Ho * Wo + row) = make_float2(v0, v1);
+    }
+  }
+}
+
 }  // namespace rv
 
 // =================================================================================================
@@ -1147,12 +1290,15 @@ extern "C" int rv_gather_blocks(const void* value, int Hv, int Wv, int C, int dt
   uint8_t* o = (uint8_t*)out;
   bool a16 = ((uintptr_t)value % 16 == 0) && ((uintptr_t)out % 16 == 0);
   static const bool fast_ok = getenv("REFVSR_NO_FAST_POINTWISE") == nullptr;
-  if (fast_ok && rowbytes % 16 == 0 && a16 && (ks == 1 || ks == 2) && hq <= 65535) {
+  if (fast_ok && rowbytes % 16 == 0 && a16 && (ks == 1 || ks == 2 || ks == 4) && hq <= 65535) {
     const int nv = rowbytes / 16;
     const dim3 grid((unsigned)cdiv((long long)wq * nv, 256), (unsigned)hq);
     const uint4* v4 = (const uint4*)value;
     uint4* o4 = (uint4*)out;
-    if (ks == 2 && nv == 6) gather_cells_kernel<2, 6><<<grid, 256, 0, st>>>(v4, Wv, nv, idx, wq, o4);
+    if (ks == 4 && nv == 6) gather_cells_kernel<4, 6><<<grid, 256, 0, st>>>(v4, Wv, nv, idx, wq, o4);
+    else if (ks == 4 && nv == 3) gather_cells_kernel<4, 3><<<grid, 256, 0, st>>>(v4, Wv, nv, idx, wq, o4);
+    else if (ks == 4) gather_cells_kernel<4, 0><<<grid, 256, 0, st>>>(v4, Wv, nv, idx, wq, o4);
+    else if (ks == 2 && nv == 6) gather_cells_kernel<2, 6><<<grid, 256, 0, st>>>(v4, Wv, nv, idx, wq, o4);
     else if (ks == 2 && nv == 3) gather_cells_kernel<2, 3><<<grid, 256, 0, st>>>(v4, Wv, nv, idx, wq, o4);
     else if (ks == 2) gather_cells_kernel<2, 0><<<grid, 256, 0, st>>>(v4, Wv, nv, idx, wq, o4);
     else if (nv == 6) gather_cells_kernel<1, 6><<<grid, 256, 0, st>>>(v4, Wv, nv, idx, wq, o4);
@@ -1193,6 +1339,13 @@ static int aligned_sample_launch(const void* x, int h, int w, int ks, int C, con
     else if (cv == 3) by_tile(std::integral_constant<int, 3>{});
     else if (cv == 12) by_tile(std::integral_constant<int, 12>{});
     else by_tile(std::integral_constant<int, 0>{});
+  }
+  else if (fast_ok && ks == 4 && C % VMAX == 0 && a16 && px * (C / VMAX) < (1ll << 31)) {
+    const int cv = C / VMAX, tiles = ((h + 7) / 8) * ((w + 7) / 8);
+    if (cv == 6) aligned_sample4_kernel<T, 6><<<tiles, 256, 0, st>>>((const T*)x, h, w, C, affine, (T*)out);
+    else if (cv == 3) aligned_sample4_kernel<T, 3><<<tiles, 256, 0, st>>>((const T*)x, h, w, C, affine, (T*)out);
+    else if (cv == 12) aligned_sample4_kernel<T, 12><<<tiles, 256, 0, st>>>((const T*)x, h, w, C, affine, (T*)out);
+    else aligned_sample4_kernel<T, 0><<<tiles, 256, 0, st>>>((const T*)x, h, w, C, affine, (T*)out);
   }
   else if (C % VMAX == 0 && a16)
     aligned_sample_kernel<T, VMAX><<<cdiv(px * (C / VMAX), 256), 256, 0, st>>>((const T*)x, h, w, ks, C, affine, (T*)out);
@@ -1274,6 +1427,8 @@ extern "C" int rv_reconstruct(const void* x, int xc, int x_dtype, const float* l
   static const bool fast_ok = getenv("REFVSR_NO_FAST_POINTWISE") == nullptr;
   if (fast_ok && scale == 4 && x_dtype == RV_F32 && xc == 4 && (uintptr_t)x % 16 == 0 && (uintptr_t)out % 16 == 0) {
     reconstruct4_kernel<<<cdiv((long long)h * w, 128), 128, 0, (cudaStream_t)stream>>>((const float4*)x, lr, h, w, clamp01, out);
+  } else if (fast_ok && scale == 2 && x_dtype == RV_F32 && xc == 4 && (uintptr_t)x % 16 == 0 && (uintptr_t)out % 8 == 0) {
+    reconstruct2_kernel<<<cdiv((long long)h * w, 128), 128, 0, (cudaStream_t)stream>>>((const float4*)x, lr, h, w, clamp01, out);
   } else {
     RV_DISPATCH_DTYPE(x_dtype, T, (reconstruct_kernel<T><<<cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(
                                       (const T*)x, xc, lr, h, w, scale, clamp01, out)));

@@ -72,7 +72,7 @@ def exchange_halo(local, plan, rank, halo, group=None):
 
 def run_sharded(net, frames_lr, frames_ref, first_index, own, num_frames, T):
     """Process the owned output frames `own = (f0, f1)`.  `frames_*` hold clip frames
-    [first_index, first_index + len) (own + halo).  Yields (k, result (3, 4h, 4w)).  The first owned frame
+    [first_index, first_index + len) (own + halo).  Yields (k, result (3, scale*h, scale*w)).  The first owned frame
     starts a new stream (is_first_frame=True) - it sits on a reset boundary by construction."""
     f0, f1 = own
     for k in range(f0, f1):
@@ -141,7 +141,7 @@ def _unpack_state(buf, state):
 
 
 def run_clip_frame_sharded(net, frames_lr, frames_ref, g0, plan, rank, groups=None, pre_windows=None, timing=None):
-    """Process this rank's frames of ONE clip; returns [(k, (3, 4h, 4w) tensor)] in frame order.
+    """Process this rank's frames of ONE clip; returns [(k, (3, scale*h, scale*w) tensor)] in frame order.
 
     `frames_*`: clip frames [g0, g0 + m) = own range + T//2 input halo on each side (exchange_halo), on the compute device.
     Work split (DESIGN.md section 6):

@@ -64,12 +64,21 @@ class Network(nn.Module):
         self.scale = config.scale
         self.flag_HD_in = config.flag_HD_in
         self.mid_channels = config.mid_channels
-        if self.scale != 4:
-            # the x2 models are a further row of the scope table; fail loudly instead of silently computing
-            # something else.  flag_HD_in (the "8K" configs: VGG[0:7] matching at 1/4 resolution, matching_ksize 8,
-            # AlignedConv2d on both alignment levels) is handled by the same schedule.
-            raise NotImplementedError('refvsr_b200 implements the x4 models (config_RefVSR_{small_,}{L1,MFID}{,_8K}); '
-                                      'got scale=%s' % (self.scale,))
+        if self.scale == 2:
+            # the x2 models (config_RefVSR_*.py:30-34: scale 2 with matching_ksize 4): VGG[0:7] matching at 1/2 resolution,
+            # AlignedConv2d on both alignment levels (aa1 blocks of 2, aa2 blocks of 4), no upsample2.  The other x2
+            # combinations fail inside the reference itself, so there is nothing to reproduce.
+            if self.flag_HD_in:
+                raise NotImplementedError('scale=2 with flag_HD_in is not supported: the reference cannot compute it '
+                                          '(its block gather indexes past the unfolded reference, attention.py:143)')
+            if config.matching_ksize != 4:
+                raise NotImplementedError('scale=2 needs matching_ksize=4 (got %s): with any other block size the reference '
+                                          'cannot compute it (F.fold size mismatch, attention.py:144)' % (config.matching_ksize,))
+        elif self.scale != 4:
+            # fail loudly instead of silently computing something else.  flag_HD_in (the "8K" configs: VGG[0:7] matching at
+            # 1/4 resolution, matching_ksize 8, AlignedConv2d on both alignment levels) is handled by the same schedule.
+            raise NotImplementedError('refvsr_b200 implements the x4 models (config_RefVSR_{small_,}{L1,MFID}{,_8K}) and '
+                                      'the x2 models (scale=2, matching_ksize=4); got scale=%s' % (self.scale,))
         build_parameter_tree(self, config)
 
         # cross-call recurrent state (RefVSR.py:96-101), one entry per batch element
@@ -365,7 +374,7 @@ class Network(nn.Module):
                         [(3, 8)], act_pre=ACT_RELU)
         f2 = self._conv('feature_match.feature_extract.2', f1, None, self._buf(tag + '.f2', (H, W, 64), dt),
                         [(64, 64)], act_pre=ACT_RELU)
-        if self.flag_HD_in:                                   # vgg_range = 7 (attention.py:31-40): maxpool, conv 64->128, ReLU
+        if self.feature_match.vgg_range == 7:                 # flag_HD_in or x2 (attention.py:31-40): maxpool, conv 64->128, ReLU
             Hm, Wm = H // 2, W // 2
             mp = self._buf(tag + '.mp', (Hm, Wm, 64), dt)
             self.ops.maxpool2(f2, mp)
@@ -378,8 +387,8 @@ class Network(nn.Module):
         return f3
 
     def _feature_match(self, lr, ref, conf, idx):
-        """conf (h,w) fp32, idx (hm*wm,) int32 indexing the reference feature grid; (hm, wm) = (h, w), or
-        (h/4, w/4) with flag_HD_in, where the relevance map is then bicubic-upsampled x4 (attention.py:93-98)."""
+        """conf (h,w) fp32, idx (hm*wm,) int32 indexing the reference feature grid; (hm, wm) = (h, w), (h/2, w/2) at x2 or
+        (h/4, w/4) with flag_HD_in, where the relevance map is then bicubic-upsampled to (h, w) (attention.py:93-98)."""
         h, w = lr.shape[1], lr.shape[2]
         split = self.match_mode == 'split'
         kpad = 448 if split else 192
@@ -430,7 +439,7 @@ class Network(nn.Module):
     def _aligned_attention(self, aa, query_img, ref8, idx, value, out):
         """AlignedAttention + AlignedConv2d (attention.py:131-159, alignment.py:39-100) -> out (2hq', 2wq', C) where
         `query_img` (3, hq', wq') fp32 is the LR-side image (lr for aa2, lr_down for aa1), blocks are ks x ks pixels,
-        ks = module scale (aa2: 2, or 8 with flag_HD_in; aa1: 4 with flag_HD_in).  `ref8` is gathered on ITS OWN
+        ks = module scale (aa2: 2, 4 at x2, or 8 with flag_HD_in; aa1: 2 at x2, 4 with flag_HD_in).  `ref8` is gathered on ITS OWN
         block grid, as the reference does (RefVSR.py:127 passes the full-resolution reference image to aa1)."""
         C, dt = self.mid_channels, self.act_dtype
         ks = self.get_submodule(aa).scale
@@ -454,12 +463,18 @@ class Network(nn.Module):
         self.ops.aligned_sample(warped, affine, ks, out)
         return out
 
+    def _match_step(self):
+        """LR pixels per matching-grid cell along each axis: the nearest x0.5 of flag_HD_in (attention.py:65-67) times the
+        max-pool of VGG[0:7] (attention.py:31-40)"""
+        return (2 if self.flag_HD_in else 1) * (2 if self.feature_match.vgg_range == 7 else 1)
+
     def _frame_slot(self, slot, h, w):
         """ring buffers of one frame"""
         C, dt = self.mid_channels, self.act_dtype
         r = f'ring{self._b}'
+        f = self._match_step()
         return {'conf': self._buf(f'{r}.conf.{slot}', (h, w), torch.float32),
-                'idx': self._buf(f'{r}.idx.{slot}', ((h // 4) * (w // 4) if self.flag_HD_in else h * w,), torch.int32),
+                'idx': self._buf(f'{r}.idx.{slot}', ((h // f) * (w // f),), torch.int32),
                 'aligned': self._buf(f'{r}.al.{slot}', (h, w, C), dt),
                 'aligned_up': self._buf(f'{r}.alup.{slot}', (2 * h, 2 * w, C), dt),
                 'lr8': self._buf(f'{r}.lr8.{slot}', (h, w, 8), dt)}
@@ -473,7 +488,7 @@ class Network(nn.Module):
         fp = self._frame_slot(slot, h, w)
         self._feature_match(lr, ref, fp['conf'], fp['idx'])
         ref8, ref_feat, ref_feat_down = self._ref_features(ref)
-        if self.aa1.has_align:                                   # flag_HD_in: aa1 scale 4 with AlignedConv2d (RefVSR.py:37,125-127)
+        if self.aa1.has_align:                   # x2 / flag_HD_in: aa1 scale 2 / 4 with AlignedConv2d (RefVSR.py:39,125-127)
             lr_down = self._buf('aa1.lrd', (3, h // 2, w // 2), torch.float32)
             self.ops.resize_planes(lr, lr_down, 2.0, mode='bicubic', clamp01=True)
             self._aligned_attention('aa1', lr_down, ref8, fp['idx'], ref_feat_down, fp['aligned'])
@@ -538,13 +553,17 @@ class Network(nn.Module):
         fused = self._conv('feat_fusion_BWFW.1.0', f0, None, self._buf('up.fused', (H2, W2, C), dt), [(C, C)],
                            act_pre=ACT_LRELU02, gate=alpha, res=base)
         dec = self._reslist('feat_decoder_BWFW', 4, fused, self._buf('up.dec', (H2, W2, C), dt), 'up.decs')
-        # lrelu(pixel_shuffle(conv)) == pixel_shuffle(lrelu(conv))  (RefVSR.py:114-115)
-        hr = self._conv('upsample2.upsample_conv', dec, None, self._buf('up.hr', (4 * h, 4 * w, C), dt), [(C, C)],
-                        act_pre=ACT_LRELU01, pixel_shuffle=True)
-        hr2 = self._conv('conv_hr', hr, None, self._buf('up.hr2', (4 * h, 4 * w, C), dt), [(C, C)], act_pre=ACT_LRELU01)
-        last = self._conv('conv_last', hr2, None, self._buf('up.last', (4 * h, 4 * w, 4), torch.float32), [(C, C)])
-        out = self._buf('up.out', (3, 4 * h, 4 * w), torch.float32)
-        self.ops.reconstruct(last, lr_center, self.scale, clamp01, out)
+        s = self.scale
+        if s == 4:
+            # lrelu(pixel_shuffle(conv)) == pixel_shuffle(lrelu(conv))  (RefVSR.py:114-115)
+            hr = self._conv('upsample2.upsample_conv', dec, None, self._buf('up.hr', (4 * h, 4 * w, C), dt), [(C, C)],
+                            act_pre=ACT_LRELU01, pixel_shuffle=True)
+        else:
+            hr = dec                                             # x2: no upsample2 (RefVSR.py:89-90,114-115)
+        hr2 = self._conv('conv_hr', hr, None, self._buf('up.hr2', (s * h, s * w, C), dt), [(C, C)], act_pre=ACT_LRELU01)
+        last = self._conv('conv_last', hr2, None, self._buf('up.last', (s * h, s * w, 4), torch.float32), [(C, C)])
+        out = self._buf('up.out', (3, s * h, s * w), torch.float32)
+        self.ops.reconstruct(last, lr_center, s, clamp01, out)      # + bicubic x scale of the centre frame (RefVSR.py:288)
         return out
 
     # ------------------------------------------------------------------------------------------
@@ -658,6 +677,10 @@ class Network(nn.Module):
             raise ValueError('flag_HD_in: LR height/width must be multiples of 4 and Ref height/width multiples of 8 '
                              '(4x4 / 8x8 alignment blocks on the 1/4-resolution matching grid, attention.py:142-154); '
                              f'got LR {h}x{w}, Ref {refs.size(3)}x{refs.size(4)}')
+        if self.scale == 2 and (h % 2 or w % 2 or refs.size(3) % 4 or refs.size(4) % 4):
+            raise ValueError('scale=2: LR height/width must be even and Ref height/width multiples of 4 '
+                             '(2x2 / 4x4 alignment blocks on the 1/2-resolution matching grid, attention.py:142-154); '
+                             f'got LR {h}x{w}, Ref {refs.size(3)}x{refs.size(4)}')
         self._device = lrs.device
         if is_train and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             # trainers/trainer.py:159-172 would call loss.backward() on the result: fail here, with a clear message
@@ -694,7 +717,7 @@ class Network(nn.Module):
         and ONLY the entering frame is handed over - lr (3, h, w), ref (3, hr, wr) in [0, 1], the frame that would have been
         lrs[b, t-1] / refs[b, t-1] of the next forward() call.  The other t-1 frames are the engine's own staged ring slots, so there
         is nothing to verify (no reuse-guard launch, no host sync) and the caller moves 1/t of the window's bytes.  Returns the
-        same tensor forward()['result'][b] would: (3, 4h, 4w).  Needs a previous forward() call on this batch slot (the clip's first
+        same tensor forward()['result'][b] would: (3, scale*h, scale*w).  Needs a previous forward() call on this batch slot (the clip's first
         window, is_first_frame=True); forced resets (reset_branch) follow the same counter as forward()."""
         if lr.dim() != 3 or ref.dim() != 3 or lr.size(0) != 3 or ref.size(0) != 3:
             raise ValueError('push_frame takes one LR frame (3, h, w) and one Ref frame (3, hr, wr)')
@@ -1099,7 +1122,7 @@ class Network(nn.Module):
 
     def shard_finish_window(self, k):
         """backward branch (window-local) + upsampling tail of output frame k; its forward step must be done.
-        -> (3, 4h, 4w) fp32 (a fresh tensor)"""
+        -> (3, scale*h, scale*w) fp32 (a fresh tensor)"""
         st = self._shard
         t, h, w, hr, wr = st['geom']
         mid = t // 2

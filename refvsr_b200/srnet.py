@@ -55,5 +55,5 @@ class SRNet(nn.Module):
 
     def push_frame(self, lr, ref):
         """streaming twin of forward() for callers that keep their own decoded-frame ring: after the clip's first window, hand
-        over only the entering (LR, Ref) frame -> (3, 4h, 4w); see Network.push_frame (no counterpart in the reference)"""
+        over only the entering (LR, Ref) frame -> (3, scale*h, scale*w); see Network.push_frame (no counterpart in the reference)"""
         return self.Network.push_frame(lr, ref)
