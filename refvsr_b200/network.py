@@ -391,7 +391,7 @@ class Network(nn.Module):
         (h/4, w/4) with flag_HD_in, where the relevance map is then bicubic-upsampled to (h, w) (attention.py:93-98)."""
         h, w = lr.shape[1], lr.shape[2]
         split = self.match_mode == 'split'
-        kpad = 448 if split else 192
+        kpad = 432 if split else 144          # 3 x 144 / 144 patch values: no zero columns for the GEMM to multiply
         lr_f = self._match_features(lr, False, 'fm.lr')
         hm, wm = lr_f.shape[0], lr_f.shape[1]
         conf_out = conf
