@@ -110,6 +110,9 @@ int rv_set_conv_cta_cap(int cap);
  * warpgroups, accumulator sets, nb, dynamic smem bytes}.  No CUDA call is made (pointers in `d` are only tested for null / alignment).  Lets the
  * ring invariants (every issuing warp owns its slots and accumulators) be checked without a GPU. */
 int rv_conv2d_tc_plan(const rv_conv_desc* d, int max_smem_optin, int num_sms, int32_t* out8);
+/* Host-only, same plan: *depth = gate / residual tiles a consumer's shared-memory buffers hold ahead of its epilogue (1 or 2), 0 when
+ * the epilogue loads those operands itself (no gate / residual, NB > 48, or operands TMA cannot address). */
+int rv_conv2d_tc_epi_depth(const rv_conv_desc* d, int max_smem_optin, int num_sms, int32_t* depth);
 
 /* ------------------------------------------------------------------------------------------------
  * rv_resblock - residual block  out = act_post( x + conv2( act_mid( conv1(x) ) ) ), 3x3 / stride 1 / pad 1,

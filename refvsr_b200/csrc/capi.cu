@@ -21,6 +21,7 @@ int fail(int code, const char* fmt, ...) {
 int conv2d_simt(const rv_conv_desc* d, cudaStream_t st);
 int conv2d_tc(const rv_conv_desc* d, cudaStream_t st);
 int conv2d_tc_plan(const rv_conv_desc* d, int max_smem, int num_sms, int* out);
+int conv2d_tc_epi_depth(const rv_conv_desc* d, int max_smem, int num_sms, int* depth);
 int set_conv_cta_cap(int cap);
 
 }  // namespace rv
@@ -45,4 +46,9 @@ extern "C" int rv_set_conv_cta_cap(int cap) { return rv::set_conv_cta_cap(cap); 
 extern "C" int rv_conv2d_tc_plan(const rv_conv_desc* d, int max_smem_optin, int num_sms, int32_t* out8) {
   RV_REQUIRE(d != nullptr && out8 != nullptr && max_smem_optin > 0 && num_sms > 0, "rv_conv2d_tc_plan: bad arguments");
   return rv::conv2d_tc_plan(d, max_smem_optin, num_sms, out8);
+}
+
+extern "C" int rv_conv2d_tc_epi_depth(const rv_conv_desc* d, int max_smem_optin, int num_sms, int32_t* depth) {
+  RV_REQUIRE(d != nullptr && depth != nullptr && max_smem_optin > 0 && num_sms > 0, "rv_conv2d_tc_epi_depth: bad arguments");
+  return rv::conv2d_tc_epi_depth(d, max_smem_optin, num_sms, depth);
 }

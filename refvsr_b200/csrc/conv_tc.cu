@@ -17,12 +17,15 @@
 // the HR tail) at NB 16 / 48 / 96 run a kernel whose tap and K-step loops are unrolled at compile time (p.fixed): a stage
 // is then one fence, 54 wgmmas with no branch between them and one commit, where the runtime loop makes ptxas fence and
 // wait on every wgmma.  Other shapes (8 + 48 channels, 7 x 7) keep the runtime loop; both issue the same MMAs in the same order.
-// Warp roles (384 threads): warp 0 = TMA producer (warps 1-3 idle), warpgroups 1 and 2 = consumers.  Consumer c owns the
-// CTA's local tiles c, c + 2, ... and its own ring of shared-memory slots, so one consumer's MMAs overlap the other's
-// epilogue (bias / act / gate / residual / act / NHWC or pixel-shuffled store straight from the accumulator registers).
+// Warp roles (384 threads): warpgroup 0 = TMA producers, warpgroups 1 and 2 = consumers.  Consumer c owns the CTA's local
+// tiles c, c + 2, ... and its own ring of shared-memory slots, so one consumer's MMAs overlap the other's epilogue
+// (bias / act / gate / residual / act / NHWC or pixel-shuffled store straight from the accumulator registers).  Producer
+// warp c fills consumer c's ring only and warp 2 + c its gate / residual buffers only, each with its own slot and phase
+// state, so a consumer that is slow to free a slot never holds back the other consumer's fills.
 // Up to NB = 48 the epilogue never waits on a global load of the gate / residual: with 16-bit, 16-byte aligned operands
-// they arrive as TMA boxes in a per-consumer shared-memory buffer (plan_tc counts it, shrinking the ring), issued one
-// tile ahead by the consumer itself; otherwise each thread loads them into registers before issuing the tile's MMAs.
+// they arrive as TMA boxes in a ring of epi_depth per-consumer shared-memory buffers (plan_tc counts them, shrinking the
+// A ring), issued by warp 2 + c as soon as a buffer is free; otherwise each thread loads them into registers before
+// issuing the tile's MMAs.
 // NB >= 64 loads each channel pair where it is used.  The compile-time kernels up to NB = 48 with a plain 16-bit output
 // write the tile into a per-consumer shared-memory buffer and store it with one TMA box store (p.out_tma): a tile's 24
 // channel-pair stores per thread, each behind its own bounds branches, made the epilogue the longest phase of a tile.
@@ -42,6 +45,7 @@ namespace rv {
 static constexpr int TH = 8, TW = 16;
 static constexpr int NCONS = 2;      // consumer warpgroups
 static constexpr int MAX_SLOTS = 6;  // ring slots per consumer
+static constexpr int MAX_EPI = 2;    // gate / residual buffers per consumer
 static constexpr int MAX_NB = 96;
 
 struct TcP {
@@ -64,6 +68,7 @@ struct TcP {
   void* out;
   int out_cs, pixel_shuffle, pair_ok, fmt;
   int epi_tma;                   // gate / residual tiles arrive by TMA in per-consumer shared-memory buffers
+  int epi_depth;                 // tiles of those buffers per consumer (1 or 2)
   uint32_t epi_bytes, epi_tx;    // bytes of one such buffer ([128 pixels][NB] 16-bit) / of all buffers of one tile
   int fixed;                     // MODE 1 with FIX_KS x FIX_KS taps and FIX_KST K-steps in every chunk (compile-time loop)
   int ps_vec;                    // pixel shuffle: each output pixel's NB / 4 channels as 16-byte stores (PSV kernel)
@@ -77,16 +82,19 @@ static constexpr int FIX_KS = 3, FIX_KST = 3;
 __host__ __device__ constexpr bool fixed_nb(int nb) { return nb == 16 || nb == 48 || nb == 96; }
 
 // Timeline instrumentation, compiled only with -DRV_CONV_TIMELINE into a separate library (tools/conv_timeline.py); the
-// product library has none of it.  One thread per role (0 = producer, 1 + c = consumer c) writes clock64 stamps of its
-// i-th local tile: tl[cta][role][i][event], cta = blockIdx.y * gridDim.x + blockIdx.x.
-//   producer: 0 empty-slot wait start, 1 wait end, 2 TMA issued
-//   consumer: 0 full-slot wait start, 1 wait end, 2 first wgmma issued, 3 wgmma.wait_group 0 returned,
-//             4 epilogue-buffer wait end, 5 epilogue end
+// product library has none of it.  Lane 0 of each role writes clock64 stamps of consumer c's i-th local tile:
+// tl[cta][role][i][event], cta = blockIdx.y * gridDim.x + blockIdx.x, role c = the producer warps of consumer c (A warp
+// events 0-2, gate / residual warp events 3-5), role NCONS + c = consumer c.
+//   producer: 0 empty-slot wait start, 1 wait end, 2 A box (all stages of the tile) issued,
+//             3 empty epilogue-buffer wait start, 4 wait end, 5 gate / residual boxes issued
+//   consumer: 0 full-slot wait start, 1 full-slot wait end, 2 turn wait end, 3 first wgmma issued,
+//             4 wgmma.wait_group 0 returned, 5 epilogue-buffer wait end, 6 store-drain wait start, 7 store-drain wait end,
+//             8 epilogue end
 // tl_diag splits the cost (S = 1 convs only): 1 = MMA-only (every tile re-issues its batch on the consumer's first,
 // resident slot: no full-slot waits after the first, no slot release, no epilogue), 2 = the same with every A view on a
 // 1024-byte swizzle atom (wrong values, same wgmma count), 3 = epilogue-only (no A loads, no MMAs).
 #ifdef RV_CONV_TIMELINE
-static constexpr int TL_TILES = 128, TL_EV = 8, TL_ROLES = 1 + NCONS;
+static constexpr int TL_TILES = 128, TL_EV = 10, TL_ROLES = 2 * NCONS;
 __device__ long long* g_tl;
 __device__ int g_tl_diag;
 static int g_tl_max_slots = 0;   // host: ring slots per consumer at most (0: the plan's)
@@ -225,7 +233,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
                const __grid_constant__ CUtensorMap tmo, const TcP p) {
   constexpr bool BF = std::is_same<TI, __nv_bfloat16>::value;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ uint64_t bar_full[NCONS][MAX_SLOTS], bar_empty[NCONS][MAX_SLOTS], bar_w, bar_epi[NCONS], bar_turn[NCONS];
+  __shared__ uint64_t bar_full[NCONS][MAX_SLOTS], bar_empty[NCONS][MAX_SLOTS], bar_w, bar_turn[NCONS];
+  __shared__ uint64_t bar_efull[NCONS][MAX_EPI], bar_eempty[NCONS][MAX_EPI];
   __shared__ __align__(16) float bias_s[MAX_NB];
 
   const uint32_t raw = tc::smem_u32(smem_raw);
@@ -250,7 +259,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
         tc::mbar_init(&bar_empty[c][i], 4);   // one arrival per consumer warp
       }
     tc::mbar_init(&bar_w, 1);
-    for (int c = 0; c < NCONS; ++c) tc::mbar_init(&bar_epi[c], 1);
+    for (int c = 0; c < NCONS; ++c)
+      for (int i = 0; i < p.epi_depth; ++i) {
+        tc::mbar_init(&bar_efull[c][i], 1);
+        tc::mbar_init(&bar_eempty[c][i], 1);   // released by one consumer thread after a named barrier
+      }
     for (int c = 0; c < NCONS; ++c) tc::mbar_init(&bar_turn[c], 4);   // one arrival per warp of the other consumer
     tc::fence_barrier_init();
     tc::prefetch_tmap(&tm0);
@@ -262,34 +275,79 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
   }
   __syncthreads();
 
-  if (warp_u == 0) {
-    // ============================ TMA producer ============================
+  // Up to NB = 48 the epilogue takes a tile's gate and residual values from registers filled before it starts (loaded
+  // where they are used, each pair's load would cost the epilogue a full global-memory latency):
+  //  * p.epi_tma (16-bit, 16-byte aligned operands): producer warp 2 + c loads consumer c's [128 pixels][NB] gate /
+  //    residual boxes by TMA into a ring of p.epi_depth buffers, up to p.epi_depth tiles ahead of the epilogue, which
+  //    copies a buffer to registers and releases it;
+  //  * otherwise each thread loads its values from global memory before issuing the tile's MMAs.
+  // Wider tiles keep per-pair loads: their accumulators leave no room for the whole tile's operands in 168 registers.
+  constexpr int NJ = NB / 8;
+  constexpr bool EARLY = NB <= 48;
+  constexpr bool TMA_OK = EARLY && sizeof(TR) == 2;
+  const bool epi_tma = TMA_OK && p.epi_tma;
+  const void* const gate_p = p.gate;
+  // consumer c's gate / residual buffer b: the gate box, then the residual box
+  auto epi_buf = [&](int c, int b) {
+    return ring + (size_t)NCONS * p.slots * p.slot_bytes + (size_t)(c * p.epi_depth + b) * p.epi_tx;
+  };
+  auto epi_res = [&](uint8_t* g) { return g + (gate_p != nullptr ? p.epi_bytes : 0u); };
+
+  if (warp_u < 4) {
+    // ============================ TMA producers ============================
+    // warp c < NCONS: consumer c's A boxes (and streamed weights); warp NCONS + c: consumer c's gate / residual boxes
+    const int pc = warp_u % NCONS;
     const uint8_t* wsrc = p.wpack + (size_t)nblk * p.S * p.w_bytes;
-    if (p.resident && tc::elect_one()) {
+    if (warp_u == 0 && p.resident && tc::elect_one()) {
       tc::mbar_expect_tx(&bar_w, (uint32_t)p.S * p.w_bytes);
       for (int s = 0; s < p.S; ++s) tc::bulk_load(wsrc + (size_t)s * p.w_bytes, &bar_w, smemW + (size_t)s * p.w_bytes, p.w_bytes);
     }
     __syncwarp();
     asm volatile("griddepcontrol.wait;" ::: "memory");
-    const uint32_t tx_bytes = p.a_tx + (p.resident ? 0u : p.w_bytes);
-    int slot[NCONS] = {0, 0};
-    uint32_t ph[NCONS] = {0u, 0u};
-    int cons = 0, it = 0;
-    const bool tl0 = threadIdx.x == 0;
+    const bool tl0 = (threadIdx.x & 31) == 0;
     (void)tl0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      if (RV_TL_DIAG == 3 || (RV_TL_DIAG != 0 && it >= NCONS)) break;   // diagnostics: only the resident slots / nothing
+    if (warp_u >= NCONS) {
+      // MMA-only diagnostics run no epilogue, so nothing would free the buffers
+      if (!epi_tma || RV_TL_DIAG == 1 || RV_TL_DIAG == 2) return;
+      if (tc::elect_one()) {
+        tc::prefetch_tmap(&tmg);
+        tc::prefetch_tmap(&tmr);
+      }
+      int buf = 0, it = 0;
+      uint32_t eph = 0;
+      for (int tile = blockIdx.x + pc * gridDim.x; tile < ntiles; tile += NCONS * gridDim.x, ++it) {
+        const int ty = tile / p.tiles_x, tx = tile - ty * p.tiles_x;
+        RV_TL(tl0, pc, it, 3);
+        tc::mbar_wait(&bar_eempty[pc][buf], eph ^ 1u);
+        RV_TL(tl0, pc, it, 4);
+        if (tc::elect_one()) {
+          uint64_t* bar = &bar_efull[pc][buf];
+          uint8_t* g = epi_buf(pc, buf);
+          tc::mbar_expect_tx(bar, p.epi_tx);
+          if (gate_p != nullptr) tc::tma_load_3d(&tmg, bar, g, nblk * NB, tx * p.tw, ty * p.th);
+          if (p.res != nullptr) tc::tma_load_3d(&tmr, bar, epi_res(g), nblk * NB, tx * p.tw, ty * p.th);
+        }
+        __syncwarp();
+        RV_TL(tl0, pc, it, 5);
+        if (++buf == p.epi_depth) { buf = 0; eph ^= 1u; }
+      }
+      return;
+    }
+    const uint32_t tx_bytes = p.a_tx + (p.resident ? 0u : p.w_bytes);
+    int slot = 0, it = 0;
+    uint32_t ph = 0;
+    for (int tile = blockIdx.x + pc * gridDim.x; tile < ntiles; tile += NCONS * gridDim.x, ++it) {
+      if (RV_TL_DIAG == 3 || (RV_TL_DIAG != 0 && it >= 1)) break;   // diagnostics: only the resident slot / nothing
       const int ty0 = tile / p.tiles_x, tx0 = tile - ty0 * p.tiles_x;
       const int yc = ty0 * p.th - p.pad, xc = tx0 * p.tw - p.pad;
       int kx = 0, ch = 0;
       for (int s = 0; s < p.S; ++s) {
-        const int sl = slot[cons];
-        RV_TL(tl0 && s == 0, 0, it, 0);
-        tc::mbar_wait(&bar_empty[cons][sl], ph[cons] ^ 1u);
-        RV_TL(tl0 && s == 0, 0, it, 1);
+        RV_TL(tl0 && s == 0, pc, it, 0);
+        tc::mbar_wait(&bar_empty[pc][slot], ph ^ 1u);
+        RV_TL(tl0 && s == 0, pc, it, 1);
         if (tc::elect_one()) {
-          uint64_t* bar = &bar_full[cons][sl];
-          uint8_t* dst = ring + ((size_t)cons * p.slots + sl) * p.slot_bytes;
+          uint64_t* bar = &bar_full[pc][slot];
+          uint8_t* dst = ring + ((size_t)pc * p.slots + slot) * p.slot_bytes;
           tc::mbar_expect_tx(bar, tx_bytes);
           if constexpr (MODE == 2) {
             for (int qd = 0; qd < p.nq0 + p.nq1; ++qd) {
@@ -303,15 +361,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
           if (!p.resident) tc::bulk_load(wsrc + (size_t)s * p.w_bytes, bar, dst + p.a_bytes, p.w_bytes);
         }
         __syncwarp();
-        RV_TL(tl0 && s == p.S - 1, 0, it, 2);
+        RV_TL(tl0 && s == p.S - 1, pc, it, 2);
         // stage order: mode 0 = (kx, chunk), mode 1 = (chunk), mode 2 = (kx)
         if (MODE == 2) ++kx;
         else if (++ch == nchunks) { ch = 0; kx += (MODE == 1) ? 0 : 1; }
-        if (++slot[cons] == p.slots) { slot[cons] = 0; ph[cons] ^= 1u; }
+        if (++slot == p.slots) { slot = 0; ph ^= 1u; }
       }
-      if (++cons == NCONS) cons = 0;
     }
-  } else if (warp_u >= 4) {
+  } else {
     // ============================ consumers ================================
     const int cons = (warp_u >> 2) - 1;
     const int t = threadIdx.x & 127, wq = t >> 5, lane = t & 31;
@@ -331,32 +388,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
     constexpr bool TURNS = KS > 0;
     uint32_t tph = 0;
     float acc[2][NB / 2];
-    // Up to NB = 48 the epilogue takes a tile's gate and residual values from registers filled before it starts (loaded
-    // where they are used, each pair's load would cost the epilogue a full global-memory latency):
-    //  * p.epi_tma (16-bit, 16-byte aligned operands): the tile's [128 pixels][NB] gate / residual boxes arrive by TMA in
-    //    this consumer's buffers while an earlier tile's epilogue and this tile's MMAs run; the epilogue copies them to
-    //    registers and then, the buffers being free, issues the boxes of the consumer's next tile;
-    //  * otherwise each thread loads its values from global memory before issuing the tile's MMAs.
-    // Wider tiles keep per-pair loads: their accumulators leave no room for the whole tile's operands in 168 registers.
-    constexpr int NJ = NB / 8;
-    constexpr bool EARLY = NB <= 48;
-    constexpr bool TMA_OK = EARLY && sizeof(TR) == 2;
-    const bool epi_tma = TMA_OK && p.epi_tma;
-    uint8_t* epi_g = ring + (size_t)NCONS * p.slots * p.slot_bytes + (size_t)cons * p.epi_tx;   // gate box, then residual box
-    uint8_t* epi_r = epi_g + (gate != nullptr ? p.epi_bytes : 0u);
-    auto epi_load = [&](int tl) {     // one thread; the caller knows the consumer's buffers are free
-      if (tl >= ntiles) return;
-      const int ty = tl / p.tiles_x, tx = tl - ty * p.tiles_x;
-      tc::mbar_expect_tx(&bar_epi[cons], p.epi_tx);
-      if (gate != nullptr) tc::tma_load_3d(&tmg, &bar_epi[cons], epi_g, nblk * NB, tx * p.tw, ty * p.th);
-      if (res != nullptr) tc::tma_load_3d(&tmr, &bar_epi[cons], epi_r, nblk * NB, tx * p.tw, ty * p.th);
-    };
+    int ebuf = 0;
     uint32_t eph = 0;
-    if (epi_tma && t == 0) {
-      tc::prefetch_tmap(&tmg);
-      tc::prefetch_tmap(&tmr);
-      epi_load(blockIdx.x + cons * gridDim.x);
-    }
     // p.out_tma (compile-time 3 x 3 kernels up to NB = 48 with a 16-bit output TMA can address): the epilogue writes the
     // tile's values into this consumer's [128 pixels][NB] buffer with no bounds branches, and one thread stores the buffer
     // with TMA, which clips edge tiles and channels >= cout.  Otherwise each thread stores its channel pairs itself.
@@ -377,7 +410,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
       }
       typename RawPair<TI>::type gv[2][2][NJ];   // [h][r2][j], as the epilogue below indexes the accumulators
       typename RawPair<TR>::type rv[2][2][NJ];
-      if (EARLY && !epi_tma) {
+      // skipped whole when there is nothing to load: its unrolled, branchy code is several KB of instructions that every
+      // tile of a plain conv would otherwise fetch and step through between its epilogue and its next MMA batch
+      if (EARLY && !epi_tma && (gate != nullptr || res != nullptr)) {
 #pragma unroll
         for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -405,17 +440,18 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
           if (++ch == nchunks) ch = 0;
         }
         if (RV_TL_DIAG == 3) break;
-        RV_TL(tl0 && s == 0, 1 + cons, it, 0);
+        RV_TL(tl0 && s == 0, NCONS + cons, it, 0);
         if (RV_TL_DIAG == 0 || it == 0) tc::mbar_wait(&bar_full[cons][slot], ph);
+        RV_TL(tl0 && s == 0, NCONS + cons, it, 1);
         if (TURNS && s == 0 && (cons != 0 || it != 0)) {
           tc::mbar_wait(&bar_turn[cons], tph);
           tph ^= 1u;
         }
-        RV_TL(tl0 && s == 0, 1 + cons, it, 1);
+        RV_TL(tl0 && s == 0, NCONS + cons, it, 2);
         const uint32_t a_addr = ring_addr + (uint32_t)slot * p.slot_bytes;
         const uint32_t b_addr = p.resident ? w_addr + (uint32_t)s * p.w_bytes : a_addr + p.a_bytes;
         tc::wgmma_fence();
-        RV_TL(tl0 && s == 0, 1 + cons, it, 2);
+        RV_TL(tl0 && s == 0, NCONS + cons, it, 3);
         if (RV_TL_DIAG == 2) issue_stage<MODE, BF, NB, KS, KST, true>(p, acc, a_addr, b_addr, s, ksteps);
         else issue_stage<MODE, BF, NB, KS, KST>(p, acc, a_addr, b_addr, s, ksteps);
         tc::wgmma_commit();
@@ -434,13 +470,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
         if (++slot == p.slots) { slot = 0; ph ^= 1u; }
       }
       tc::wgmma_wait<0>();
-      RV_TL(tl0, 1 + cons, it, 3);
+      RV_TL(tl0, NCONS + cons, it, 4);
       if (RV_TL_DIAG == 1 || RV_TL_DIAG == 2) continue;
       if (prev >= 0 && lane == 0) tc::mbar_arrive(&bar_empty[cons][prev]);
       if constexpr (TMA_OK) {
         if (epi_tma) {
-          tc::mbar_wait(&bar_epi[cons], eph);
-          eph ^= 1u;
+          tc::mbar_wait(&bar_efull[cons][ebuf], eph);
+          RV_TL(tl0, NCONS + cons, it, 5);
+          uint8_t* epi_g = epi_buf(cons, ebuf);
+          const uint8_t* epi_r = epi_res(epi_g);
 #pragma unroll
           for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -452,15 +490,17 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
                 if (gate != nullptr) gv[h][r2][j] = *reinterpret_cast<const uint32_t*>(epi_g + off);
                 if (res != nullptr) rv[h][r2][j] = *reinterpret_cast<const uint32_t*>(epi_r + off);
               }
-          // all 128 threads have read the buffers: order those reads before the async proxy's writes of the next tile
+          // all 128 threads have read the buffer: order those reads before the async proxy's writes of a later tile, then
+          // hand the buffer back to producer warp NCONS + cons
           asm volatile("bar.sync %0, 128;" ::"r"(1 + cons) : "memory");
           if (t == 0) {
             tc::fence_proxy_async();
-            epi_load(tile + NCONS * gridDim.x);
+            tc::mbar_arrive(&bar_eempty[cons][ebuf]);
           }
+          if (++ebuf == p.epi_depth) { ebuf = 0; eph ^= 1u; }
         }
       }
-      RV_TL(tl0, 1 + cons, it, 4);
+      RV_TL(tl0 && !epi_tma, NCONS + cons, it, 5);
 
       // ---- epilogue: thread t holds rows 64 h + 16 wq + lane / 4 (+ 8) and column pairs 8 j + 2 (lane % 4) ----
       if constexpr (PSV) {
@@ -504,13 +544,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
             }
           }
         }
-        RV_TL(tl0, 1 + cons, it, 5);
+        RV_TL(tl0, NCONS + cons, it, 8);
         continue;
       }
       if constexpr (OUT_TMA_OK) {
         if (out_tma) {
+          RV_TL(tl0, NCONS + cons, it, 6);
           if (t == 0) tc::bulk_wait_read<0>();      // this consumer's previous store has read the buffer
           asm volatile("bar.sync %0, 128;" ::"r"(1 + cons) : "memory");
+          RV_TL(tl0, NCONS + cons, it, 7);
 #pragma unroll
           for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -547,7 +589,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
             tc::tma_store_3d(&tmo, out_s, nblk * NB, tx0 * p.tw, ty0 * p.th);
             tc::bulk_commit();
           }
-          RV_TL(tl0, 1 + cons, it, 5);
+          RV_TL(tl0, NCONS + cons, it, 8);
           continue;
         }
       }
@@ -598,7 +640,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
           }
         }
       }
-      RV_TL(tl0, 1 + cons, it, 5);
+      RV_TL(tl0, NCONS + cons, it, 8);
     }
     if (out_tma && t == 0) tc::bulk_wait<0>();     // the last stores are complete before the CTA exits
   }
@@ -756,7 +798,10 @@ static int plan_tc(const rv_conv_desc* d, TcP& p, size_t& smem_out, int& nblk_ou
   p.epi_tx = (uint32_t)((d->gate ? 1 : 0) + (d->res ? 1 : 0)) * p.epi_bytes;
   p.epi_tma = (d->gate || d->res) && p.NB <= 48 && rdt0 == d->in_dtype && tma_ok(d->gate, d->gate_cs) &&
               tma_ok(d->res, d->res_cs) && w_all + ring_min + (size_t)NCONS * p.epi_tx <= budget;
-  const size_t epi_all = p.epi_tma ? (size_t)NCONS * p.epi_tx : 0;
+  // a second buffer lets the boxes arrive up to two tiles ahead of the epilogue; it is taken only while two A slots and the
+  // output buffer per consumer still fit (gate + residual at NB = 48 keeps two A slots and one buffer)
+  p.epi_depth = p.epi_tma && w_all + (size_t)NCONS * (2 * p.a_bytes + MAX_EPI * p.epi_tx + p.epi_bytes) <= budget ? MAX_EPI : 1;
+  const size_t epi_all = p.epi_tma ? (size_t)NCONS * p.epi_depth * p.epi_tx : 0;
   // the compile-time tap loop: a square FIX_KS kernel whose every channel chunk takes FIX_KST K-steps (e.g. 48 + 48
   // channels, not 8 + 48); other shapes keep the runtime loop
   p.fixed = p.mode == 1 && d->kh == FIX_KS && d->kw == FIX_KS && fixed_nb(p.NB);
@@ -854,17 +899,32 @@ int conv2d_tc(const rv_conv_desc* d, cudaStream_t st) {
 // host-only: the launch plan of rv_conv2d (tensor-core path) for given device limits -> out[8] = {mode, slots per consumer,
 // weights resident, S, consumer warpgroups, accumulator sets, nb, smem bytes}.  mode: 0 boxes per (kx, chunk), 1 single box,
 // 2 32B-swizzled quads.
-int conv2d_tc_plan(const rv_conv_desc* d, int max_smem, int num_sms, int* out) {
+static int plan_for(const rv_conv_desc* d, int max_smem, int num_sms, TcP& p, size_t& smem) {
   const int s0 = g_num_sms, s1 = g_max_smem;
   g_num_sms = num_sms; g_max_smem = max_smem;
-  TcP p;
-  size_t smem = 0;
   int nblk = 1;
   const int rc = plan_tc(d, p, smem, nblk);
   g_num_sms = s0; g_max_smem = s1;
+  return rc;
+}
+
+int conv2d_tc_plan(const rv_conv_desc* d, int max_smem, int num_sms, int* out) {
+  TcP p;
+  size_t smem = 0;
+  const int rc = plan_for(d, max_smem, num_sms, p, smem);
   if (rc) return rc;
   out[0] = p.mode;
   out[1] = p.slots; out[2] = p.resident; out[3] = p.S; out[4] = NCONS; out[5] = NCONS; out[6] = p.NB; out[7] = (int)smem;
+  return RV_OK;
+}
+
+// host-only: gate / residual buffers per consumer of that plan (0: the epilogue loads them itself)
+int conv2d_tc_epi_depth(const rv_conv_desc* d, int max_smem, int num_sms, int* depth) {
+  TcP p;
+  size_t smem = 0;
+  const int rc = plan_for(d, max_smem, num_sms, p, smem);
+  if (rc) return rc;
+  *depth = p.epi_tma ? p.epi_depth : 0;
   return RV_OK;
 }
 

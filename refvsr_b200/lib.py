@@ -66,6 +66,7 @@ SIGNATURES = {
     'rv_conv2d': (_I, [C.POINTER(rv_conv_desc), _P]),
     'rv_set_conv_cta_cap': (_I, [_I]),
     'rv_conv2d_tc_plan': (_I, [C.POINTER(rv_conv_desc), _I, _I, C.POINTER(C.c_int32)]),
+    'rv_conv2d_tc_epi_depth': (_I, [C.POINTER(rv_conv_desc), _I, _I, C.POINTER(C.c_int32)]),
     'rv_resblock': (_I, [C.POINTER(rv_resblock_desc), _P]),
     'rv_conv_chain': (_I, [C.POINTER(rv_conv_chain_desc), _P]),
     'rv_space_to_depth2': (_I, [_P, _I, _I, _I, _I, _P, _P]),
