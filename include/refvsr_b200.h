@@ -95,6 +95,10 @@ typedef struct rv_conv_desc {
                          /*         N = 3*NB per MMA),                                     */
                          /*     2 = 32B-swizzled 16-channel quads,                         */
                          /*     3 = weight image of 1, kx-folding disabled (test / A-B)    */
+  int32_t ps_order;      /* TC pixel shuffle: 0 = columns n = 4c+2a+b; 1 = HR-row order   */
+                         /*   (packing.ps_rows_order: cout = 2*nb, block a = HR sub-row a, */
+                         /*   both sub-pixels x all cout/4 channels; weights and bias      */
+                         /*   permuted to match).  Other descs must leave it 0.            */
 } rv_conv_desc;
 
 int rv_conv2d(const rv_conv_desc* d, void* stream);
@@ -104,6 +108,10 @@ int rv_conv2d(const rv_conv_desc* d, void* stream);
  * different streams with half the SMs each - two capped launches overlap each other's prologue / first-box latency / last-tile tail,
  * which a single dependent chain of launches exposes once per layer. */
 int rv_set_conv_cta_cap(int cap);
+/* Upper bound of the shared memory per CTA that the following rv_conv2d (tensor-core) launches plan with; 0 restores the device's
+ * opt-in limit.  Returns the previous value.  A smaller bound takes the plan branches of a device with less shared memory (fewer
+ * ring slots, no TMA output buffer), so that each can be run and compared on one device. */
+int rv_set_conv_smem_cap(int bytes);
 
 /* Host-only: the launch plan rv_conv2d's tensor-core path would use on a device with `max_smem_optin` bytes of opt-in shared memory
  * per block and `num_sms` SMs -> out8 = {mode, smem slots per consumer, weights resident, stages per tile, consumer
@@ -113,6 +121,10 @@ int rv_conv2d_tc_plan(const rv_conv_desc* d, int max_smem_optin, int num_sms, in
 /* Host-only, same plan: *depth = gate / residual tiles a consumer's shared-memory buffers hold ahead of its epilogue (1 or 2), 0 when
  * the epilogue loads those operands itself (no gate / residual, NB > 48, or operands TMA cannot address). */
 int rv_conv2d_tc_epi_depth(const rv_conv_desc* d, int max_smem_optin, int num_sms, int32_t* depth);
+/* Host-only, same plan: how the output is stored.  *kind = 0 per-thread stores from registers, 1 TMA boxes of NHWC tiles staged
+ * in shared memory, 2 TMA boxes of pixel-shuffled HR rows staged in shared memory (ps_order 1), 3 pixel-shuffled HR rows as
+ * 16-byte stores from registers (ps_order 1, when the staging buffers do not fit). */
+int rv_conv2d_tc_out_store(const rv_conv_desc* d, int max_smem_optin, int num_sms, int32_t* kind);
 
 /* ------------------------------------------------------------------------------------------------
  * rv_resblock - residual block  out = act_post( x + conv2( act_mid( conv1(x) ) ) ), 3x3 / stride 1 / pad 1,

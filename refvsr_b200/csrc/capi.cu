@@ -22,7 +22,9 @@ int conv2d_simt(const rv_conv_desc* d, cudaStream_t st);
 int conv2d_tc(const rv_conv_desc* d, cudaStream_t st);
 int conv2d_tc_plan(const rv_conv_desc* d, int max_smem, int num_sms, int* out);
 int conv2d_tc_epi_depth(const rv_conv_desc* d, int max_smem, int num_sms, int* depth);
+int conv2d_tc_out_store(const rv_conv_desc* d, int max_smem, int num_sms, int* kind);
 int set_conv_cta_cap(int cap);
+int set_conv_smem_cap(int bytes);
 
 }  // namespace rv
 
@@ -37,11 +39,13 @@ extern "C" int rv_conv2d(const rv_conv_desc* d, void* stream) {
              "rv_conv2d: bad geometry H=%d W=%d c0=%d cout=%d k=%dx%d stride=%d", d->H, d->W, d->c0,
              d->cout, d->kh, d->kw, d->stride);
   if (d->impl == RV_CONV_IMPL_TC) return rv::conv2d_tc(d, (cudaStream_t)stream);
+  RV_REQUIRE(d->ps_order == 0 || d->impl == RV_CONV_IMPL_TC, "rv_conv2d: ps_order=%d is a tensor-core weight order", d->ps_order);
   if (d->impl == RV_CONV_IMPL_SIMT) return rv::conv2d_simt(d, (cudaStream_t)stream);
   return rv::fail(RV_E_INVALID, "rv_conv2d: unknown impl %d", d->impl);
 }
 
 extern "C" int rv_set_conv_cta_cap(int cap) { return rv::set_conv_cta_cap(cap); }
+extern "C" int rv_set_conv_smem_cap(int bytes) { return rv::set_conv_smem_cap(bytes); }
 
 extern "C" int rv_conv2d_tc_plan(const rv_conv_desc* d, int max_smem_optin, int num_sms, int32_t* out8) {
   RV_REQUIRE(d != nullptr && out8 != nullptr && max_smem_optin > 0 && num_sms > 0, "rv_conv2d_tc_plan: bad arguments");
@@ -51,4 +55,9 @@ extern "C" int rv_conv2d_tc_plan(const rv_conv_desc* d, int max_smem_optin, int 
 extern "C" int rv_conv2d_tc_epi_depth(const rv_conv_desc* d, int max_smem_optin, int num_sms, int32_t* depth) {
   RV_REQUIRE(d != nullptr && depth != nullptr && max_smem_optin > 0 && num_sms > 0, "rv_conv2d_tc_epi_depth: bad arguments");
   return rv::conv2d_tc_epi_depth(d, max_smem_optin, num_sms, depth);
+}
+
+extern "C" int rv_conv2d_tc_out_store(const rv_conv_desc* d, int max_smem_optin, int num_sms, int32_t* kind) {
+  RV_REQUIRE(d != nullptr && kind != nullptr && max_smem_optin > 0 && num_sms > 0, "rv_conv2d_tc_out_store: bad arguments");
+  return rv::conv2d_tc_out_store(d, max_smem_optin, num_sms, kind);
 }

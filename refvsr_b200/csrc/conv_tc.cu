@@ -21,19 +21,26 @@
 // tiles c, c + 2, ... and its own ring of shared-memory slots, so one consumer's MMAs overlap the other's epilogue
 // (bias / act / gate / residual / act / NHWC or pixel-shuffled store straight from the accumulator registers).  Producer
 // warp c fills consumer c's ring only and warp 2 + c its gate / residual buffers only, each with its own slot and phase
-// state, so a consumer that is slow to free a slot never holds back the other consumer's fills.
+// state, so a consumer that is slow to free a slot never holds back the other consumer's fills.  In the compile-time
+// kernels the two A warps still issue their first ring fills alternately (a start-up hand-off through bar_fill), as the
+// single producer before them did, so that consumer 1's first box does not queue behind all of consumer 0's.
 // Up to NB = 48 the epilogue never waits on a global load of the gate / residual: with 16-bit, 16-byte aligned operands
 // they arrive as TMA boxes in a ring of epi_depth per-consumer shared-memory buffers (plan_tc counts them, shrinking the
 // A ring), issued by warp 2 + c as soon as a buffer is free; otherwise each thread loads them into registers before
 // issuing the tile's MMAs.
-// NB >= 64 loads each channel pair where it is used.  The compile-time kernels up to NB = 48 with a plain 16-bit output
-// write the tile into a per-consumer shared-memory buffer and store it with one TMA box store (p.out_tma): a tile's 24
-// channel-pair stores per thread, each behind its own bounds branches, made the epilogue the longest phase of a tile.
+// NB >= 64 loads each channel pair where it is used.  The kernels up to NB = 48 with a plain 16-bit output (compile-time
+// and runtime tap loops alike) write the tile into a per-consumer shared-memory buffer and store it with one TMA box
+// store (p.out_tma): a tile's channel-pair stores per thread, each behind its own bounds branches, made the epilogue the
+// longest phase of a tile.
 // In every compile-time kernel the two consumers also take turns issuing their MMA batches, so that each epilogue
 // overlaps the other consumer's MMAs.  Other epilogues store from registers.  The upsampling
-// convs (3 x 3, NB = 96, pixel shuffle into a 16-bit map, no gate / residual; p.ps_vec) run a twin of the compile-time
-// kernel (PSV) whose epilogue exchanges column pairs between lanes q and q ^ 2, so that each thread holds the 24
-// consecutive channels of one output pixel and writes them as three 16-byte vectors instead of 24 2-byte stores.
+// convs (3 x 3, 48 -> 192 = 2 NB, pixel shuffle into a 16-bit map, no gate / residual; p.ps_vec) are packed in the
+// HR-row column order (ps_order 1, see below TcP): column block a is HR sub-row a of both sub-pixels and all 48 channels, so
+// a CTA writes whole 96-byte HR pixels and every L2 sector of the map gets one full write (in the conv's own order, each
+// block wrote half of every pixel, and the other half came from the other block at some other time).  They run a twin of
+// the compile-time kernel (PSV) in which each lane's accumulators form 16-byte vectors of one HR pixel with no lane
+// exchange.  Each 8-row half of a tile goes into a per-consumer [8 rows][16 HR pixels][48] shared-memory buffer and out
+// by one TMA box store; when those buffers do not fit, the vectors are 16-byte global stores.
 #include <algorithm>
 #include <cstdlib>
 
@@ -71,10 +78,16 @@ struct TcP {
   int epi_depth;                 // tiles of those buffers per consumer (1 or 2)
   uint32_t epi_bytes, epi_tx;    // bytes of one such buffer ([128 pixels][NB] 16-bit) / of all buffers of one tile
   int fixed;                     // MODE 1 with FIX_KS x FIX_KS taps and FIX_KST K-steps in every chunk (compile-time loop)
-  int ps_vec;                    // pixel shuffle: each output pixel's NB / 4 channels as 16-byte stores (PSV kernel)
+  int ps_order;                  // pixel shuffle, HR-row column order (rv_conv_desc::ps_order, see below)
+  int ps_vec;                    // pixel shuffle in that order: HR rows as 16-byte vectors or TMA boxes (PSV kernel)
   int out_tma;                   // the output tile is staged in a per-consumer shared-memory buffer and written by TMA
-  uint32_t out_off;              // byte offset of those buffers from the ring ([128 pixels][NB] 16-bit each)
+  uint32_t out_off, out_bytes;   // byte offset of those buffers from the ring / bytes of one
 };
+
+// HR-row column order of the pixel-shuffle convs (ps_order 1, cout = 2 NB, packing.ps_rows_order): column nl of block
+// nblk is HR sub-row a = nblk.  Lane q of a wgmma accumulator holds the column pairs nl = 8 j + 2 q, + 1; its pairs
+// j = 4 g .. 4 g + 3 are the 8 consecutive channels 8 c8 .. 8 c8 + 7 of sub-pixel b, (b, c8) = divmod(4 g + q, NB / 16), so
+// each is one 16-byte vector with no lane exchange.  Only the PSV kernel knows this order: the plan refuses it elsewhere.
 
 // MODE 1 shapes whose tap / K-step loops are unrolled at compile time: KS x KS taps and KST K = 16 steps in every channel
 // chunk (3 x 3 over 48-channel chunks: the trunk, fusions, pixel shuffles and the HR tail), at the NB the window uses.
@@ -234,7 +247,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
   constexpr bool BF = std::is_same<TI, __nv_bfloat16>::value;
   extern __shared__ uint8_t smem_raw[];
   __shared__ uint64_t bar_full[NCONS][MAX_SLOTS], bar_empty[NCONS][MAX_SLOTS], bar_w, bar_turn[NCONS];
-  __shared__ uint64_t bar_efull[NCONS][MAX_EPI], bar_eempty[NCONS][MAX_EPI];
+  __shared__ uint64_t bar_efull[NCONS][MAX_EPI], bar_eempty[NCONS][MAX_EPI], bar_fill[NCONS];
   __shared__ __align__(16) float bias_s[MAX_NB];
 
   const uint32_t raw = tc::smem_u32(smem_raw);
@@ -265,6 +278,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
         tc::mbar_init(&bar_eempty[c][i], 1);   // released by one consumer thread after a named barrier
       }
     for (int c = 0; c < NCONS; ++c) tc::mbar_init(&bar_turn[c], 4);   // one arrival per warp of the other consumer
+    for (int c = 0; c < NCONS; ++c) tc::mbar_init(&bar_fill[c], 1);   // the other A producer warp's start-up hand-off
     tc::fence_barrier_init();
     tc::prefetch_tmap(&tm0);
     if (p.nch1 || p.nq1) tc::prefetch_tmap(&tm1);
@@ -334,10 +348,24 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
       return;
     }
     const uint32_t tx_bytes = p.a_tx + (p.resident ? 0u : p.w_bytes);
+    // Start-up hand-off (compile-time kernels): the two A warps issue the tiles of their first ring fill alternately
+    // (consumer 0's tile 0, consumer 1's tile 0, consumer 0's tile 1, ...), so that consumer 1's first box does not queue
+    // behind consumer 0's whole fill.  Tile it of warp 1 follows tile it of warp 0, tile it of warp 0 follows tile it - 1 of
+    // warp 1; after the first `lead` tiles (at most two) each waits on its own consumer's slots only.  The runtime-loop
+    // kernels (7 x 7, 1 x 1, 64-channel chunks) measured slower with it and keep independent fills.
+    const int lead = KS > 0 ? min(2, (p.slots + p.S - 1) / p.S) : 0;
+    const int rest = ntiles - (int)blockIdx.x - (pc ^ 1) * (int)gridDim.x;
+    const int n_other = rest > 0 ? (rest + NCONS * gridDim.x - 1) / (NCONS * gridDim.x) : 0;   // tiles of the other warp
+    uint32_t fph = 0;
     int slot = 0, it = 0;
     uint32_t ph = 0;
     for (int tile = blockIdx.x + pc * gridDim.x; tile < ntiles; tile += NCONS * gridDim.x, ++it) {
       if (RV_TL_DIAG == 3 || (RV_TL_DIAG != 0 && it >= 1)) break;   // diagnostics: only the resident slot / nothing
+      const int after = it - (pc == 0 ? 1 : 0);                     // the other warp's tile this one follows
+      if (it < lead && after >= 0 && after < n_other) {
+        tc::mbar_wait(&bar_fill[pc], fph);
+        fph ^= 1u;
+      }
       const int ty0 = tile / p.tiles_x, tx0 = tile - ty0 * p.tiles_x;
       const int yc = ty0 * p.th - p.pad, xc = tx0 * p.tw - p.pad;
       int kx = 0, ch = 0;
@@ -367,6 +395,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
         else if (++ch == nchunks) { ch = 0; kx += (MODE == 1) ? 0 : 1; }
         if (++slot == p.slots) { slot = 0; ph ^= 1u; }
       }
+      const int next = it + (pc == 0 ? 0 : 1);                      // the other warp's tile that follows this one
+      if (next < lead && next < n_other && tl0) tc::mbar_arrive(&bar_fill[pc ^ 1]);
     }
   } else {
     // ============================ consumers ================================
@@ -390,12 +420,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
     float acc[2][NB / 2];
     int ebuf = 0;
     uint32_t eph = 0;
-    // p.out_tma (compile-time 3 x 3 kernels up to NB = 48 with a 16-bit output TMA can address): the epilogue writes the
-    // tile's values into this consumer's [128 pixels][NB] buffer with no bounds branches, and one thread stores the buffer
-    // with TMA, which clips edge tiles and channels >= cout.  Otherwise each thread stores its channel pairs itself.
-    constexpr bool OUT_TMA_OK = KS > 0 && !PSV && EARLY && sizeof(TO) == 2;
+    // p.out_tma (kernels up to NB = 48 with a 16-bit output TMA can address, and the PSV kernel): the epilogue writes the
+    // tile's values into this consumer's buffer with no bounds branches, and one thread stores the buffer with TMA, which
+    // clips edge tiles and channels >= cout.  Otherwise each thread stores its values itself.
+    constexpr bool OUT_TMA_OK = (EARLY || PSV) && sizeof(TO) == 2;
     const bool out_tma = OUT_TMA_OK && p.out_tma;
-    uint8_t* out_s = ring + p.out_off + (size_t)cons * p.epi_bytes;
+    uint8_t* out_s = ring + p.out_off + (size_t)cons * p.out_bytes;
     if (out_tma && t == 0) tc::prefetch_tmap(&tmo);
     int it = 0;
     const bool tl0 = t == 0;
@@ -504,50 +534,70 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
 
       // ---- epilogue: thread t holds rows 64 h + 16 wq + lane / 4 (+ 8) and column pairs 8 j + 2 (lane % 4) ----
       if constexpr (PSV) {
-        // Pixel shuffle into a 16-bit map without gate / residual.  n = 4c + 2a + b  ->  out[(2oy+a, 2ox+b)][c].  Lane
-        // q = lane % 4 holds (c, a) = (2j + q / 2, q % 2) for b = 0, 1; one exchange with lane q ^ 2 (same row, same a)
-        // leaves it pixel (a, b) = (q % 2, q / 2) for c = 2j, 2j + 1 of every j: the block's NB / 4 consecutive channels
-        // of one output pixel, stored as 16-byte vectors.  The general epilogue below is not compiled into this kernel.
-        static_assert(sizeof(TO) == 2 && (NB / 4) % 8 == 0, "16-byte pixel-shuffle rows need 16-bit outputs, NB % 32 == 0");
-        const int a = lane & 1, b = (lane >> 1) & 1;
-        // own (b = 0 | b = 1) word and the partner's: b = 0 keeps both low halves, b = 1 both high halves (c = 2j first)
-        const uint32_t sel = b ? 0x3276u : 0x5410u;
+        // Pixel shuffle into a 16-bit map without gate / residual, columns in the HR-row order (after TcP): block nblk is
+        // HR sub-row a = nblk, and lane q's column pairs j = 4 g .. 4 g + 3 are 8 consecutive channels of sub-pixel b, one
+        // 16-byte vector.  The CTA writes whole HR pixels: tile row r gives the 2 tw pixels x NB / 2 channels of HR row
+        // 2 (ty0 th + r) + a from 2 tx0 tw on, contiguous in memory.  With p.out_tma each 8-row half of the tile goes
+        // into this consumer's [8 rows][2 tw pixels][NB / 2] buffer and out by one TMA box store (4-D map over
+        // (channel, HR x, a, LR y)); otherwise each vector is a 16-byte global store.  The general epilogue below is not
+        // compiled into this kernel.
+        static_assert(sizeof(TO) == 2 && NB % 32 == 0, "16-byte pixel-shuffle rows need 16-bit outputs, NB % 32 == 0");
+        constexpr int CV = NB / 16;                     // 16-byte vectors per HR pixel
+        const int q = lane & 3;
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
+          if (out_tma) {
+            RV_TL(tl0 && h == 0, NCONS + cons, it, 6);
+            if (t == 0) tc::bulk_wait_read<0>();      // this consumer's previous store has read the buffer
+            asm volatile("bar.sync %0, 128;" ::"r"(1 + cons) : "memory");
+            RV_TL(tl0 && h == 0, NCONS + cons, it, 7);
+          }
 #pragma unroll
           for (int r2 = 0; r2 < 2; ++r2) {
             const int m = 64 * h + 16 * wq + (lane >> 2) + 8 * r2;
-            const int oy = ty0 * p.th + (m >> p.tw_shift), ox = tx0 * p.tw + (m & (p.tw - 1));
-            const bool in = oy < p.Ho && ox < p.Wo;     // the same for both partners of the exchange
+            const int r = m >> p.tw_shift, x = m & (p.tw - 1);
+            const int oy = ty0 * p.th + r, ox = tx0 * p.tw + x;
+            const bool in = oy < p.Ho && ox < p.Wo;
 #pragma unroll
-            for (int i = 0; i < NJ / 4; ++i) {          // channels 8 i .. 8 i + 7 of the pixel: column pairs j = 4 i .. 4 i + 3
+            for (int g = 0; g < NB / 32; ++g) {
+              const int J = 4 * g + q, b = J >= CV ? 1 : 0, c8 = J - b * CV;
               uint32_t pk[4];
 #pragma unroll
               for (int jj = 0; jj < 4; ++jj) {
-                const int j = 4 * i + jj;
+                const int j = 4 * g + jj;
                 float v[2];
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
-                  const float x = acc[h][4 * j + 2 * r2 + e] + bias_s[8 * j + 2 * (lane & 3) + e];
-                  v[e] = fmaxf(x, x * p.pre_slope);
+                  const float xv = acc[h][4 * j + 2 * r2 + e] + bias_s[8 * j + 2 * q + e];
+                  v[e] = fmaxf(xv, xv * p.pre_slope);
                   v[e] = fmaxf(v[e], v[e] * p.post_slope);
                   if (p.post_clamp3) v[e] = fminf(fmaxf(v[e], -3.f), 3.f);
                 }
-                const uint32_t own = pack2<TO>(v[0], v[1]);
-                const uint32_t got = __shfl_xor_sync(0xffffffffu, own, 2);
-                pk[jj] = __byte_perm(own, got, sel);
+                pk[jj] = pack2<TO>(v[0], v[1]);
               }
-              if (in) {
-                TO* o = out + ((size_t)(2 * oy + a) * (2 * p.Wo) + 2 * ox + b) * p.out_cs + nblk * (NB / 4) + 8 * i;
-                *reinterpret_cast<uint4*>(o) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+              const uint4 vec = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+              if (out_tma) {
+                const uint32_t pix = (uint32_t)(r - 8 * h) * 2 * p.tw + 2 * x + b;
+                *reinterpret_cast<uint4*>(out_s + (pix * (NB / 2) + 8 * c8) * 2u) = vec;
+              } else if (in) {
+                TO* o = out + ((size_t)(2 * oy + nblk) * (2 * p.Wo) + 2 * ox + b) * p.out_cs + 8 * c8;
+                *reinterpret_cast<uint4*>(o) = vec;
               }
+            }
+          }
+          if (out_tma) {
+            tc::fence_proxy_async();                  // the buffer's writes, before the async proxy reads them
+            asm volatile("bar.sync %0, 128;" ::"r"(1 + cons) : "memory");
+            if (t == 0) {
+              tc::tma_store_4d(&tmo, out_s, 0, 2 * tx0 * p.tw, nblk, ty0 * p.th + 8 * h);
+              tc::bulk_commit();
             }
           }
         }
         RV_TL(tl0, NCONS + cons, it, 8);
         continue;
       }
-      if constexpr (OUT_TMA_OK) {
+      if constexpr (OUT_TMA_OK && !PSV) {
         if (out_tma) {
           RV_TL(tl0, NCONS + cons, it, 6);
           if (t == 0) tc::bulk_wait_read<0>();      // this consumer's previous store has read the buffer
@@ -678,6 +728,23 @@ static int make_tmap_3d(CUtensorMap* m, const void* ptr, int C, int W, int H, in
   return RV_OK;
 }
 
+// the 16-bit pixel-shuffled output [2 Ho][2 Wo][cs] of an LR Ho x Wo map as (channel, HR x, sub-row a, LR y), so that one
+// box of C x 2 tw x 1 x rows is HR rows 2 y + a of `rows` LR rows; out-of-bounds elements are not written
+static int make_ps_rows_tmap(CUtensorMap* m, const void* ptr, int C, int cs, int Wo, int Ho, int tw, int rows, int fmt) {
+  PFN_tmapEncodeTiled enc = get_tmap_encoder();
+  if (!enc) return fail(RV_E_CUDA, "cuTensorMapEncodeTiled entry point not available");
+  const cuuint64_t px = (cuuint64_t)cs * 2;
+  cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)2 * Wo, 2, (cuuint64_t)Ho};
+  cuuint64_t gstr[3] = {px, 2 * Wo * px, 4 * Wo * px};
+  cuuint32_t box[4] = {(cuuint32_t)C, (cuuint32_t)2 * tw, 1, (cuuint32_t)rows};
+  cuuint32_t estr[4] = {1, 1, 1, 1};
+  CUresult r = enc(m, fmt ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(ptr), gdim,
+                   gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail(RV_E_CUDA, "cuTensorMapEncodeTiled (HR rows) failed (%d) C=%d W=%d H=%d", (int)r, C, Wo, Ho);
+  return RV_OK;
+}
+
 static int make_act_tmap(CUtensorMap* m, const void* ptr, int C, int W, int H, int box_w, int box_rows, int fmt, int sw32 = 0) {
   return make_tmap_3d(m, ptr, C, W, H, sw32 ? 16 : 64, box_w, box_rows, fmt, sw32 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_128B);
 }
@@ -686,6 +753,8 @@ static int g_num_sms = 0;
 static int g_max_smem = 0;
 static int g_cta_cap = 0;          // rv_set_conv_cta_cap: upper bound of the persistent grid (0 = one CTA per SM)
 int set_conv_cta_cap(int cap) { const int old = g_cta_cap; g_cta_cap = cap > 0 ? cap : 0; return old; }
+static int g_smem_cap = 0;         // rv_set_conv_smem_cap: upper bound of a launch's shared memory (0 = the device's opt-in limit)
+int set_conv_smem_cap(int bytes) { const int old = g_smem_cap; g_smem_cap = bytes > 0 ? bytes : 0; return old; }
 
 template <typename TI, typename TR, typename TO, int MODE, int NB, int KS = 0, int KST = 0, bool PSV = false>
 static int launch_tc_mode(const CUtensorMap* tm, const TcP& p, dim3 grid, size_t smem, cudaStream_t st) {
@@ -751,6 +820,9 @@ static int plan_tc(const rv_conv_desc* d, TcP& p, size_t& smem_out, int& nblk_ou
   RV_REQUIRE(!d->pixel_shuffle || d->cout % 4 == 0, "rv_conv2d: pixel_shuffle needs cout %% 4 == 0");
   RV_REQUIRE(d->layout >= 0 && d->layout <= 3, "rv_conv2d(tc): unknown layout %d", d->layout);
   RV_REQUIRE(g_num_sms > 0 && g_max_smem > 0, "rv_conv2d(tc): device limits not set");
+  RV_REQUIRE(d->ps_order == 0 || (d->ps_order == 1 && d->pixel_shuffle && d->cout == 2 * d->nb && d->nb % 32 == 0),
+             "rv_conv2d(tc): ps_order=%d needs a pixel shuffle with cout == 2 * nb and nb %% 32 == 0 (cout=%d nb=%d ps=%d)",
+             d->ps_order, d->cout, d->nb, d->pixel_shuffle);
   p.Ho = d->H + 2 * d->pad - d->kh + 1;
   p.Wo = d->W + 2 * d->pad - d->kw + 1;
   RV_REQUIRE(p.Ho > 0 && p.Wo > 0, "rv_conv2d: empty output");
@@ -760,7 +832,9 @@ static int plan_tc(const rv_conv_desc* d, TcP& p, size_t& smem_out, int& nblk_ou
   p.nq0 = p.nq1 = 0; p.q_bytes = 0;
   p.NB = d->nb; p.cout = d->cout;
   const int nblk = (d->cout + p.NB - 1) / p.NB;
-  const size_t budget = (size_t)g_max_smem - 1024 /*alignment*/ - 2048 /*static: barriers, bias*/;
+  const int smem_lim = g_smem_cap > 0 ? std::min(g_smem_cap, g_max_smem) : g_max_smem;
+  RV_REQUIRE(smem_lim > 3072, "rv_conv2d(tc): shared-memory limit %d too small", smem_lim);
+  const size_t budget = (size_t)smem_lim - 1024 /*alignment*/ - 2048 /*static: barriers, bias*/;
   p.mode = (d->layout == 1 || d->layout == 3) ? 1 : d->layout;
   if (p.mode == 1) {
     RV_REQUIRE(d->kh == d->kw && (d->kh == 1 || d->kh == 3 || d->kh == 5 || d->kh == 7), "rv_conv2d(tc): layout 1 needs a square 1/3/5/7 kernel");
@@ -809,12 +883,23 @@ static int plan_tc(const rv_conv_desc* d, TcP& p, size_t& smem_out, int& nblk_ou
     const int crem = (ch < p.nch0) ? (p.c0 - ch * 64) : (p.c1 - (ch - p.nch0) * 64);
     p.fixed = (std::min(crem, 64) + 15) / 16 == FIX_KST;
   }
-  // TMA-store epilogue: compile-time kernels up to NB = 48 writing a plain (not pixel-shuffled) map of the input's 16-bit
-  // type whose base and pixel stride TMA can address, when a [128 pixels][NB] buffer per consumer fits next to the
-  // resident weights, the gate / residual buffers and the minimal ring
-  p.out_tma = p.fixed && p.NB <= 48 && !d->pixel_shuffle && d->out_dtype == d->in_dtype && d->out != nullptr &&
-              tma_ok(d->out, d->out_cs) && w_all + ring_min + epi_all + (size_t)NCONS * p.epi_bytes <= budget;
-  const size_t out_all = p.out_tma ? (size_t)NCONS * p.epi_bytes : 0;
+  // the upsampling convs (compile-time 3 x 3 loop, NB = 96, pixel shuffle in the HR-row column order into a 16-bit map, no
+  // gate / residual) run the PSV kernel when the HR pixel rows stay 16-byte aligned; other pixel shuffles keep the 2-byte
+  // stores of the general epilogue
+  p.ps_order = d->ps_order;
+  p.ps_vec = p.fixed && d->pixel_shuffle && d->ps_order && p.NB == 96 && dtype_size(d->out_dtype) == 2 && !d->gate &&
+             !d->res && d->out != nullptr && (uintptr_t)d->out % 16 == 0 && (d->out_cs * 2) % 16 == 0;
+  RV_REQUIRE(!d->ps_order || p.ps_vec, "rv_conv2d(tc): ps_order=1 needs the 3x3 48-channel nb=96 kernel with a 16-bit output "
+             "whose HR pixel rows are 16-byte aligned (out_cs=%d), no gate / residual", d->out_cs);
+  // TMA-store epilogue, when its buffer per consumer fits next to the resident weights, the gate / residual buffers and the
+  // minimal ring: kernels up to NB = 48 writing a plain (not pixel-shuffled) map of the input's 16-bit type whose base
+  // and pixel stride TMA can address ([128 pixels][NB] buffer, th x tw of the layout mode), and the PSV kernel (half a tile of HR rows,
+  // [8 rows][16 pixels][NB / 2]: a whole tile's buffers would leave one A slot per consumer next to the 108 KB of weights)
+  const bool out_plain = p.NB <= 48 && !d->pixel_shuffle && d->out_dtype == d->in_dtype && d->out != nullptr &&
+                         tma_ok(d->out, d->out_cs);
+  p.out_bytes = p.ps_vec ? p.epi_bytes / 2 : p.epi_bytes;
+  p.out_tma = (out_plain || p.ps_vec) && w_all + ring_min + epi_all + (size_t)NCONS * p.out_bytes <= budget;
+  const size_t out_all = p.out_tma ? (size_t)NCONS * p.out_bytes : 0;
   if (w_all + ring_min + epi_all + out_all <= budget) {
     p.resident = 1;
     p.slot_bytes = p.a_bytes;
@@ -843,11 +928,6 @@ static int plan_tc(const rv_conv_desc* d, TcP& p, size_t& smem_out, int& nblk_ou
   auto al = [](const void* q, int cs, int dt) { return q == nullptr || (((uintptr_t)q % (2 * dtype_size(dt)) == 0) && cs % 2 == 0); };
   p.pair_ok = al(d->out, d->out_cs, d->out_dtype) && al(d->gate, d->gate_cs, d->in_dtype) && al(d->res, d->res_cs, rdt);
   p.fmt = d->in_dtype == RV_BF16 ? 1 : 0;
-  // the upsampling convs (compile-time 3 x 3 loop, NB = 96, pixel shuffle into a 16-bit map, no gate / residual): a thread
-  // gathers one output pixel's 24 channels and stores them as three 16-byte vectors, when every channel of the block
-  // exists and the pixel rows stay 16-byte aligned; other pixel shuffles keep the 2-byte stores
-  p.ps_vec = p.fixed && p.pixel_shuffle && p.NB == 96 && dtype_size(d->out_dtype) == 2 && d->cout % p.NB == 0 &&
-             !d->gate && !d->res && (uintptr_t)d->out % 16 == 0 && (d->out_cs * 2) % 16 == 0;
   smem_out = smem;
   nblk_out = nblk;
   return RV_OK;
@@ -883,7 +963,10 @@ int conv2d_tc(const rv_conv_desc* d, cudaStream_t st) {
   if (p.epi_tma && d->res && (rc = make_tmap_3d(&tm[3], d->res, d->res_cs, p.Wo, p.Ho, p.NB, p.tw, p.th, p.fmt, CU_TENSOR_MAP_SWIZZLE_NONE)))
     return rc;
   // output tiles [th][tw][NB] of the TMA-store epilogue; channels >= cout (and pixels outside the map) are not written
-  if (p.out_tma && (rc = make_tmap_3d(&tm[4], d->out, d->cout, p.Wo, p.Ho, p.NB, p.tw, p.th, p.fmt, CU_TENSOR_MAP_SWIZZLE_NONE, d->out_cs)))
+  if (p.out_tma && !p.ps_vec &&
+      (rc = make_tmap_3d(&tm[4], d->out, d->cout, p.Wo, p.Ho, p.NB, p.tw, p.th, p.fmt, CU_TENSOR_MAP_SWIZZLE_NONE, d->out_cs)))
+    return rc;
+  if (p.out_tma && p.ps_vec && (rc = make_ps_rows_tmap(&tm[4], d->out, d->cout / 4, d->out_cs, p.Wo, p.Ho, p.tw, p.th / 2, p.fmt)))
     return rc;
   const int ntiles = p.tiles_x * p.tiles_y;
   int gx = std::min(ntiles, std::max(1, g_num_sms / nblk));
@@ -900,11 +983,11 @@ int conv2d_tc(const rv_conv_desc* d, cudaStream_t st) {
 // weights resident, S, consumer warpgroups, accumulator sets, nb, smem bytes}.  mode: 0 boxes per (kx, chunk), 1 single box,
 // 2 32B-swizzled quads.
 static int plan_for(const rv_conv_desc* d, int max_smem, int num_sms, TcP& p, size_t& smem) {
-  const int s0 = g_num_sms, s1 = g_max_smem;
-  g_num_sms = num_sms; g_max_smem = max_smem;
+  const int s0 = g_num_sms, s1 = g_max_smem, s2 = g_smem_cap;
+  g_num_sms = num_sms; g_max_smem = max_smem; g_smem_cap = 0;
   int nblk = 1;
   const int rc = plan_tc(d, p, smem, nblk);
-  g_num_sms = s0; g_max_smem = s1;
+  g_num_sms = s0; g_max_smem = s1; g_smem_cap = s2;
   return rc;
 }
 
@@ -925,6 +1008,17 @@ int conv2d_tc_epi_depth(const rv_conv_desc* d, int max_smem, int num_sms, int* d
   const int rc = plan_for(d, max_smem, num_sms, p, smem);
   if (rc) return rc;
   *depth = p.epi_tma ? p.epi_depth : 0;
+  return RV_OK;
+}
+
+// host-only: how that plan stores the output -> *kind = 0 per-thread stores from registers, 1 TMA boxes of [th][tw][NB]
+// NHWC tiles, 2 TMA boxes of pixel-shuffled HR rows (PSV), 3 pixel-shuffled HR rows as 16-byte stores from registers (PSV)
+int conv2d_tc_out_store(const rv_conv_desc* d, int max_smem, int num_sms, int* kind) {
+  TcP p;
+  size_t smem = 0;
+  const int rc = plan_for(d, max_smem, num_sms, p, smem);
+  if (rc) return rc;
+  *kind = p.ps_vec ? (p.out_tma ? 2 : 3) : (p.out_tma ? 1 : 0);
   return RV_OK;
 }
 

@@ -31,7 +31,7 @@ class rv_conv_desc(C.Structure):
         ('res', C.c_void_p), ('res_cs', C.c_int32), ('res_dtype', C.c_int32),
         ('out', C.c_void_p), ('out_cs', C.c_int32), ('out_dtype', C.c_int32),
         ('pixel_shuffle', C.c_int32), ('impl', C.c_int32), ('nb', C.c_int32), ('k_real', C.c_int32),
-        ('layout', C.c_int32),
+        ('layout', C.c_int32), ('ps_order', C.c_int32),
     ]
 
 
@@ -67,6 +67,8 @@ SIGNATURES = {
     'rv_set_conv_cta_cap': (_I, [_I]),
     'rv_conv2d_tc_plan': (_I, [C.POINTER(rv_conv_desc), _I, _I, C.POINTER(C.c_int32)]),
     'rv_conv2d_tc_epi_depth': (_I, [C.POINTER(rv_conv_desc), _I, _I, C.POINTER(C.c_int32)]),
+    'rv_conv2d_tc_out_store': (_I, [C.POINTER(rv_conv_desc), _I, _I, C.POINTER(C.c_int32)]),
+    'rv_set_conv_smem_cap': (_I, [_I]),
     'rv_resblock': (_I, [C.POINTER(rv_resblock_desc), _P]),
     'rv_conv_chain': (_I, [C.POINTER(rv_conv_chain_desc), _P]),
     'rv_space_to_depth2': (_I, [_P, _I, _I, _I, _I, _P, _P]),
@@ -152,6 +154,10 @@ class CudaOps:
         """persistent-grid bound of the following tensor-core conv launches (0 = one CTA per SM); returns the previous value"""
         return int(self.lib.rv_set_conv_cta_cap(int(cap)))
 
+    def set_conv_smem_cap(self, nbytes):
+        """shared-memory bound the following tensor-core conv launches plan with (0 = the device's limit); returns the previous value"""
+        return int(self.lib.rv_set_conv_smem_cap(int(nbytes)))
+
     # -- convolution ------------------------------------------------------------------------------
     def conv2d(self, layer, src0, src1, out, gate=None, res=None, act_pre=ACT_NONE, act_post=ACT_NONE,
                pixel_shuffle=False):
@@ -184,6 +190,7 @@ class CudaOps:
         d.nb = layer.nb
         d.k_real = layer.k_real
         d.layout = getattr(layer, 'layout', 0)
+        d.ps_order = getattr(layer, 'ps_order', 0)
         _check(self.lib, self.lib.rv_conv2d(C.byref(d), self._stream()), f'rv_conv2d[{layer.name}]')
 
     def resblock(self, rb, src, out, act_mid, act_post=ACT_NONE):

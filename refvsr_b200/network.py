@@ -176,9 +176,11 @@ class Network(nn.Module):
         self._state.clear()
         self.frame_itr_num = 0
 
-    def _layer(self, name, srcs, stride=1, pad=None, bias_add=0.0, s2d=False):
-        """Packed weights of conv `name` (attribute path under self) for the given source layout."""
-        key = (name, tuple(srcs), s2d)
+    def _layer(self, name, srcs, stride=1, pad=None, bias_add=0.0, s2d=False, ps_rows=False):
+        """Packed weights of conv `name` (attribute path under self) for the given source layout.  ps_rows: the conv feeds a
+        pixel shuffle, and the engine's own packing puts its columns in the HR-row order (packing.ps_rows_order); ops that
+        pack their own layers keep the conv's order."""
+        key = (name, tuple(srcs), s2d, ps_rows)
         hit = self._packed.get(key)
         if hit is not None:
             return hit
@@ -188,8 +190,11 @@ class Network(nn.Module):
         pad = k // 2 if pad is None else pad
         if s2d:
             weight, srcs = packing.s2d_weights(weight, srcs, k // 2)
-        pack = self.ops.pack_conv if hasattr(self.ops, 'pack_conv') else packing.pack_conv
-        pc = pack(name, weight, mod.bias, srcs, stride, pad, self.act_dtype, self._device, self.prefer_tc, bias_add)
+        if hasattr(self.ops, 'pack_conv'):
+            pc = self.ops.pack_conv(name, weight, mod.bias, srcs, stride, pad, self.act_dtype, self._device, self.prefer_tc, bias_add)
+        else:
+            pc = packing.pack_conv(name, weight, mod.bias, srcs, stride, pad, self.act_dtype, self._device, self.prefer_tc, bias_add,
+                                   ps_rows=ps_rows)
         self._packed[key] = pc
         return pc
 
@@ -217,7 +222,7 @@ class Network(nn.Module):
             self.ops.conv2d(layer, z0, z1, out, gate=gate, res=res, act_pre=act_pre, act_post=act_post,
                             pixel_shuffle=pixel_shuffle)
             return out
-        layer = self._layer(name, srcs, stride, pad, bias_add)
+        layer = self._layer(name, srcs, stride, pad, bias_add, ps_rows=pixel_shuffle)
         self.ops.conv2d(layer, src0, src1, out, gate=gate, res=res, act_pre=act_pre, act_post=act_post,
                         pixel_shuffle=pixel_shuffle)
         return out

@@ -36,6 +36,7 @@ class PackedConv:
     wpack: torch.Tensor
     bias: torch.Tensor
     layout: int = 0
+    ps_order: int = 0        # 1: pixel-shuffle columns in the HR-row order (ps_rows_order), 0: the conv's own order
 
 
 def _expand_inputs(weight, srcs):
@@ -163,6 +164,20 @@ def pack_tc(weight, srcs, dtype, nb, layout=0):
     return out.view(nblk, S, kh_eff, nb, 64).to(dtype).contiguous()
 
 
+def ps_rows_order(nb):
+    """HR-row column order of a x2 pixel-shuffle conv with cout = 2 * nb (rv_conv_desc.ps_order = 1): entry n' is the conv
+    output channel n = 4c + 2a + b that packed column n' computes.  Column block a is HR sub-row a.  Within it, column
+    nl = 8j + 2q + e (the wgmma accumulator pair e of lane q, column group j) is sub-pixel b, channel
+    c = 8 c8 + 2 (j % 4) + e with (b, c8) = divmod(4 (j // 4) + q, nb // 16), so that a lane's pairs j = 4g .. 4g + 3 are 8
+    consecutive channels of one HR pixel (the PSV kernel of conv_tc.cu)."""
+    assert nb % 32 == 0, nb
+    nl = torch.arange(nb)
+    j, q, e = nl // 8, (nl // 2) % 4, nl % 2
+    b, c8 = torch.div(4 * (j // 4) + q, nb // 16, rounding_mode='floor'), (4 * (j // 4) + q) % (nb // 16)
+    c = 8 * c8 + 2 * (j % 4) + e
+    return torch.cat([4 * c + 2 * a + b for a in range(2)])
+
+
 DEFAULT_TC_LAYOUT = 1                    # 1: one box per tile (falls back to 0 when the taps do not fit), 0: boxes per (kx, chunk),
                                          # 2: 32B-swizzled 16-channel quads
 SMEM_BUDGET = 232448 - 1024 - 4096      # opt-in shared memory per CTA minus alignment and static (conv_tc.cu)
@@ -197,38 +212,40 @@ def _cache_dir():
     return d if d not in ('', '0') else None
 
 
-def _pack_key(weight, bias, srcs, stride, pad, act_dtype, prefer_tc, bias_add, tc_layout):
+def _pack_key(weight, bias, srcs, stride, pad, act_dtype, prefer_tc, bias_add, tc_layout, ps_rows=False):
     """sha256 over the layer's parameters, every packing argument and this file's source (a change of the packing code
     invalidates the cache by itself); environment switches that steer the layout choice are part of the key."""
     h = hashlib.sha256()
     h.update(_SELF_DIGEST)
     h.update(repr((tuple(weight.shape), str(weight.dtype), [tuple(x) for x in srcs], stride, pad, str(act_dtype), bool(prefer_tc),
-                   float(bias_add), tc_layout, os.environ.get('REFVSR_TC_LAYOUT', ''))).encode())
+                   float(bias_add), tc_layout, os.environ.get('REFVSR_TC_LAYOUT', ''), bool(ps_rows))).encode())
     h.update(weight.detach().contiguous().cpu().numpy().tobytes())
     h.update(bias.detach().float().contiguous().cpu().numpy().tobytes())
     return h.hexdigest()
 
 
-def pack_conv(name, weight, bias, srcs, stride, pad, act_dtype, device, prefer_tc=True, bias_add=0.0, tc_layout=None):
+def pack_conv(name, weight, bias, srcs, stride, pad, act_dtype, device, prefer_tc=True, bias_add=0.0, tc_layout=None,
+              ps_rows=False):
     """pack_conv_uncached behind the optional on-disk cache: a hit loads the packed operand image and bias instead of
     re-deriving them (bit-identical by construction: what is stored is the output of the same function)."""
     cdir = _cache_dir()
     if cdir is None:
-        return pack_conv_uncached(name, weight, bias, srcs, stride, pad, act_dtype, device, prefer_tc, bias_add, tc_layout)
-    path = os.path.join(cdir, _pack_key(weight, bias, srcs, stride, pad, act_dtype, prefer_tc, bias_add, tc_layout) + '.pt')
+        return pack_conv_uncached(name, weight, bias, srcs, stride, pad, act_dtype, device, prefer_tc, bias_add, tc_layout, ps_rows)
+    path = os.path.join(cdir, _pack_key(weight, bias, srcs, stride, pad, act_dtype, prefer_tc, bias_add, tc_layout, ps_rows) + '.pt')
     if os.path.isfile(path):
         try:
             d = torch.load(path, map_location='cpu')
             return PackedConv(name, d['cout'], d['kh'], d['kw'], d['stride'], d['pad'], d['alloc0'], d['alloc1'], d['impl'], d['nb'],
-                              d['k_real'], d['wpack'].to(device), d['bias'].to(device), d['layout'])
+                              d['k_real'], d['wpack'].to(device), d['bias'].to(device), d['layout'], d.get('ps_order', 0))
         except Exception:                       # unreadable / truncated entry: fall through and rewrite it
             pass
-    pc = pack_conv_uncached(name, weight, bias, srcs, stride, pad, act_dtype, 'cpu', prefer_tc, bias_add, tc_layout)
+    pc = pack_conv_uncached(name, weight, bias, srcs, stride, pad, act_dtype, 'cpu', prefer_tc, bias_add, tc_layout, ps_rows)
     try:
         os.makedirs(cdir, exist_ok=True)
         tmp = f'{path}.{os.getpid()}.tmp'
         torch.save(dict(cout=pc.cout, kh=pc.kh, kw=pc.kw, stride=pc.stride, pad=pc.pad, alloc0=pc.alloc0, alloc1=pc.alloc1,
-                        impl=pc.impl, nb=pc.nb, k_real=pc.k_real, wpack=pc.wpack, bias=pc.bias, layout=pc.layout), tmp)
+                        impl=pc.impl, nb=pc.nb, k_real=pc.k_real, wpack=pc.wpack, bias=pc.bias, layout=pc.layout,
+                        ps_order=pc.ps_order), tmp)
         os.replace(tmp, path)                   # atomic: concurrent ranks may pack the same layer
     except OSError:
         pass                                    # read-only / full cache directory: the cache is an optimisation only
@@ -236,8 +253,11 @@ def pack_conv(name, weight, bias, srcs, stride, pad, act_dtype, device, prefer_t
     return pc
 
 
-def pack_conv_uncached(name, weight, bias, srcs, stride, pad, act_dtype, device, prefer_tc=True, bias_add=0.0, tc_layout=None):
-    """Pick the implementation and build the packed tensors.  `srcs` = [(real, alloc), ...] (1 or 2)."""
+def pack_conv_uncached(name, weight, bias, srcs, stride, pad, act_dtype, device, prefer_tc=True, bias_add=0.0, tc_layout=None,
+                       ps_rows=False):
+    """Pick the implementation and build the packed tensors.  `srcs` = [(real, alloc), ...] (1 or 2).  ps_rows: the conv
+    feeds a x2 pixel shuffle; a tensor-core layer with cout = 2 * nb then gets its weight and bias rows in the HR-row order
+    (ps_rows_order), in which each CTA writes whole HR pixels."""
     cout, _, kh, kw = weight.shape
     alloc0 = srcs[0][1]
     alloc1 = srcs[1][1] if len(srcs) > 1 else 0
@@ -247,10 +267,16 @@ def pack_conv_uncached(name, weight, bias, srcs, stride, pad, act_dtype, device,
     if tc_ok:
         nb = choose_nb(cout)
         layout = choose_layout(kh, kw, srcs, nb) if tc_layout is None else tc_layout
-        wp = (pack_tc_sw32(weight.detach(), srcs, act_dtype, nb) if layout == 2
-              else pack_tc(weight.detach(), srcs, act_dtype, nb, layout)).to(device)
+        w = weight.detach()
+        # only the 3 x 3, 48-channel, nb = 96 kernel of conv_tc.cu stores this order (rv_conv2d refuses it elsewhere)
+        ps_order = int(bool(ps_rows) and cout == 2 * nb == 192 and layout in (1, 3) and kh == kw == 3 and len(srcs) == 1
+                       and 32 < srcs[0][1] <= 48)
+        if ps_order:
+            perm = ps_rows_order(nb)
+            w, b = w[perm.to(w.device)], b[perm.to(b.device)]
+        wp = (pack_tc_sw32(w, srcs, act_dtype, nb) if layout == 2 else pack_tc(w, srcs, act_dtype, nb, layout)).to(device)
         return PackedConv(name, cout, kh, kw, stride, pad, alloc0, alloc1, IMPL_TC, nb,
-                          kh * kw * (alloc0 + alloc1), wp, b.to(device).contiguous(), layout)
+                          kh * kw * (alloc0 + alloc1), wp, b.to(device).contiguous(), layout, ps_order)
     wp = pack_simt(weight.detach(), srcs).to(device)
     return PackedConv(name, cout, kh, kw, stride, pad, alloc0, alloc1, IMPL_SIMT, 0,
                       kh * kw * (alloc0 + alloc1), wp, b.to(device).contiguous())

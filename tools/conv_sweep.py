@@ -27,7 +27,7 @@ def case(cin, cout, k, res=True, calloc=None, hw=(H, W), gate=False, cin1=0, shu
     cout_alloc = cout_alloc or cout
     wgt = torch.randn(cout, cin + cin1, k, k) * 0.05
     srcs = [(cin, calloc)] + ([(cin1, cin1)] if cin1 else [])
-    layer = packing.pack_conv('x', wgt, torch.zeros(cout), srcs, 1, k // 2, dt, 'cuda', True)
+    layer = packing.pack_conv('x', wgt, torch.zeros(cout), srcs, 1, k // 2, dt, 'cuda', True, ps_rows=shuffle)
     nrot = 6
     oshape = (2 * h, 2 * w, cout // 4) if shuffle else (h, w, cout_alloc)
     xs = [torch.randn((h, w, calloc), device='cuda').to(dt) for _ in range(nrot)]

@@ -57,6 +57,7 @@ def shapes():
             ('48->48 res 540x960', 48, 48, 540, 960, True, False, False),
             ('48->48 gate+res 270x480', 48, 48, 270, 480, True, False, True),
             ('conv_hr 1080x1920', 48, 48, 1080, 1920, False, False, False),
+            ('upsample1 270x480', 48, 192, 270, 480, False, True, False),
             ('upsample2 540x960', 48, 192, 540, 960, False, True, False)]
 
 
@@ -199,7 +200,7 @@ def main():
             continue
         torch.manual_seed(0)
         wgt = torch.randn(cout, cin, 3, 3) * 0.05
-        layer = packing.pack_conv('x', wgt, torch.zeros(cout), [(cin, cin)], 1, 1, dt, 'cuda', True)
+        layer = packing.pack_conv('x', wgt, torch.zeros(cout), [(cin, cin)], 1, 1, dt, 'cuda', True, ps_rows=ps)
         nrot = 3
         xs = [torch.randn((h, w, cin), device='cuda').to(dt) for _ in range(nrot)]
         rs = [torch.randn((h, w, cout), device='cuda').to(dt) for _ in range(nrot)] if res else None
