@@ -105,7 +105,9 @@ __host__ __device__ constexpr bool fixed_nb(int nb) { return nb == 16 || nb == 4
 //             8 epilogue end
 // tl_diag splits the cost (S = 1 convs only): 1 = MMA-only (every tile re-issues its batch on the consumer's first,
 // resident slot: no full-slot waits after the first, no slot release, no epilogue), 2 = the same with every A view on a
-// 1024-byte swizzle atom (wrong values, same wgmma count), 3 = epilogue-only (no A loads, no MMAs).
+// 1024-byte swizzle atom (wrong values, same wgmma count), 3 = epilogue-only (no A loads, no MMAs), 4 = the full pipeline
+// with an epilogue that touches no shared memory (TMA-store epilogue only: the gate / residual buffers are waited for and
+// released but not read, the values are folded into a register instead of the staging buffer, no TMA store).
 #ifdef RV_CONV_TIMELINE
 static constexpr int TL_TILES = 128, TL_EV = 10, TL_ROLES = 2 * NCONS;
 __device__ long long* g_tl;
@@ -123,10 +125,12 @@ __device__ __forceinline__ void tl_stamp(long long* tl, int role, int it, int ev
 #define RV_TL_INIT long long* const tl_buf = g_tl; const int tl_diag = g_tl_diag
 #define RV_TL(on, role, it, ev) do { if (on) tl_stamp(tl_buf, role, it, ev); } while (0)
 #define RV_TL_DIAG tl_diag
+#define RV_TL_MMA_ONLY (tl_diag == 1 || tl_diag == 2)
 #else
 #define RV_TL_INIT do { } while (0)
 #define RV_TL(on, role, it, ev) do { } while (0)
 #define RV_TL_DIAG 0
+#define RV_TL_MMA_ONLY false
 #endif
 
 // All MMAs of one pipeline stage into both 64-row halves.  Descriptor start addresses are in 16-byte units: +2 per
@@ -322,7 +326,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
     (void)tl0;
     if (warp_u >= NCONS) {
       // MMA-only diagnostics run no epilogue, so nothing would free the buffers
-      if (!epi_tma || RV_TL_DIAG == 1 || RV_TL_DIAG == 2) return;
+      if (!epi_tma || RV_TL_MMA_ONLY) return;
       if (tc::elect_one()) {
         tc::prefetch_tmap(&tmg);
         tc::prefetch_tmap(&tmr);
@@ -360,7 +364,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
     int slot = 0, it = 0;
     uint32_t ph = 0;
     for (int tile = blockIdx.x + pc * gridDim.x; tile < ntiles; tile += NCONS * gridDim.x, ++it) {
-      if (RV_TL_DIAG == 3 || (RV_TL_DIAG != 0 && it >= 1)) break;   // diagnostics: only the resident slot / nothing
+      if (RV_TL_DIAG == 3 || (RV_TL_MMA_ONLY && it >= 1)) break;   // diagnostics: only the resident slot / nothing
       const int after = it - (pc == 0 ? 1 : 0);                     // the other warp's tile this one follows
       if (it < lead && after >= 0 && after < n_other) {
         tc::mbar_wait(&bar_fill[pc], fph);
@@ -471,7 +475,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
         }
         if (RV_TL_DIAG == 3) break;
         RV_TL(tl0 && s == 0, NCONS + cons, it, 0);
-        if (RV_TL_DIAG == 0 || it == 0) tc::mbar_wait(&bar_full[cons][slot], ph);
+        if (!RV_TL_MMA_ONLY || it == 0) tc::mbar_wait(&bar_full[cons][slot], ph);
         RV_TL(tl0 && s == 0, NCONS + cons, it, 1);
         if (TURNS && s == 0 && (cons != 0 || it != 0)) {
           tc::mbar_wait(&bar_turn[cons], tph);
@@ -486,7 +490,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
         else issue_stage<MODE, BF, NB, KS, KST>(p, acc, a_addr, b_addr, s, ksteps);
         tc::wgmma_commit();
         if (TURNS && s == p.S - 1 && lane == 0) tc::mbar_arrive(&bar_turn[cons ^ 1]);   // the other consumer's turn
-        if (RV_TL_DIAG != 0) continue;    // MMA-only: the slot stays resident (S = 1)
+        if (RV_TL_MMA_ONLY) continue;    // MMA-only: the slot stays resident (S = 1)
         if (p.slots == 1) {
           // a single slot is refilled only after these MMAs have read it
           tc::wgmma_wait<0>();
@@ -501,7 +505,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
       }
       tc::wgmma_wait<0>();
       RV_TL(tl0, NCONS + cons, it, 4);
-      if (RV_TL_DIAG == 1 || RV_TL_DIAG == 2) continue;
+      if (RV_TL_MMA_ONLY) continue;
       if (prev >= 0 && lane == 0) tc::mbar_arrive(&bar_empty[cons][prev]);
       if constexpr (TMA_OK) {
         if (epi_tma) {
@@ -517,6 +521,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
               for (int j = 0; j < NJ; ++j) {
                 const int m = 64 * h + 16 * wq + (lane >> 2) + 8 * r2;
                 const uint32_t off = (uint32_t)(m * NB + 8 * j + 2 * (lane & 3)) * 2u;
+                if (RV_TL_DIAG == 4) {
+                  gv[h][r2][j] = rv[h][r2][j] = 0x3c003c00u ^ off;
+                  continue;
+                }
                 if (gate != nullptr) gv[h][r2][j] = *reinterpret_cast<const uint32_t*>(epi_g + off);
                 if (res != nullptr) rv[h][r2][j] = *reinterpret_cast<const uint32_t*>(epi_r + off);
               }
@@ -600,39 +608,75 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
       if constexpr (OUT_TMA_OK && !PSV) {
         if (out_tma) {
           RV_TL(tl0, NCONS + cons, it, 6);
-          if (t == 0) tc::bulk_wait_read<0>();      // this consumer's previous store has read the buffer
-          asm volatile("bar.sync %0, 128;" ::"r"(1 + cons) : "memory");
+          if (RV_TL_DIAG != 4) {
+            if (t == 0) tc::bulk_wait_read<0>();      // this consumer's previous store has read the buffer
+            asm volatile("bar.sync %0, 128;" ::"r"(1 + cons) : "memory");
+          }
           RV_TL(tl0, NCONS + cons, it, 7);
+          uint32_t fold = 0;    // tl_diag 4: the epilogue's values, kept live without a shared-memory store
+          (void)fold;
+          // HG / HR / HP: the conv may have a gate / a residual / a post-activation or clamp.  The compile-time kernels run
+          // the variant of exactly what the conv applies: with runtime tests only, every value of a plain conv also issued
+          // the predicated-off gate and residual conversions and the identity post-activation and clamp, more than half
+          // of the pass's instructions, on the consumer's critical path.  The runtime-loop kernels keep the general one.
+          auto values = [&](auto hg, auto hr, auto hp) {
+            constexpr bool HG = decltype(hg)::value, HR = decltype(hr)::value, HP = decltype(hp)::value;
 #pragma unroll
-          for (int h = 0; h < 2; ++h)
+            for (int h = 0; h < 2; ++h)
 #pragma unroll
-            for (int r2 = 0; r2 < 2; ++r2) {
-              const int m = 64 * h + 16 * wq + (lane >> 2) + 8 * r2;
+              for (int r2 = 0; r2 < 2; ++r2) {
+                const int m = 64 * h + 16 * wq + (lane >> 2) + 8 * r2;
 #pragma unroll
-              for (int j = 0; j < NJ; ++j) {
-                const int nl = 8 * j + 2 * (lane & 3);
-                float v[2];
+                for (int j = 0; j < NJ; ++j) {
+                  const int nl = 8 * j + 2 * (lane & 3);
+                  float v[2];
 #pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                  const float x = acc[h][4 * j + 2 * r2 + e] + bias_s[nl + e];
-                  v[e] = fmaxf(x, x * p.pre_slope);
+                  for (int e = 0; e < 2; ++e) {
+                    const float x = acc[h][4 * j + 2 * r2 + e] + bias_s[nl + e];
+                    v[e] = fmaxf(x, x * p.pre_slope);
+                  }
+                  if (HG && gate != nullptr) {
+                    // __fmul_rn: never contracted with the residual add into one FMA, whose single rounding would change
+                    // the bits of gate + residual convs (with runtime tests the two were separate predicated instructions)
+                    const float2 g = raw2_to_f2<TI>(gv[h][r2][j]);
+                    v[0] = __fmul_rn(v[0], g.x); v[1] = __fmul_rn(v[1], g.y);
+                  }
+                  if (HR && res != nullptr) {
+                    const float2 r = raw2_to_f2<TR>(rv[h][r2][j]);
+                    v[0] += r.x; v[1] += r.y;
+                  }
+                  if (HP) {
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                      v[e] = fmaxf(v[e], v[e] * p.post_slope);
+                      if (p.post_clamp3) v[e] = fminf(fmaxf(v[e], -3.f), 3.f);
+                    }
+                  }
+                  if (RV_TL_DIAG == 4) fold ^= pack2<TO>(v[0], v[1]);
+                  else *reinterpret_cast<uint32_t*>(out_s + (uint32_t)(m * NB + nl) * 2u) = pack2<TO>(v[0], v[1]);
                 }
-                if (gate != nullptr) {
-                  const float2 g = raw2_to_f2<TI>(gv[h][r2][j]);
-                  v[0] *= g.x; v[1] *= g.y;
-                }
-                if (res != nullptr) {
-                  const float2 r = raw2_to_f2<TR>(rv[h][r2][j]);
-                  v[0] += r.x; v[1] += r.y;
-                }
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                  v[e] = fmaxf(v[e], v[e] * p.post_slope);
-                  if (p.post_clamp3) v[e] = fminf(fmaxf(v[e], -3.f), 3.f);
-                }
-                *reinterpret_cast<uint32_t*>(out_s + (uint32_t)(m * NB + nl) * 2u) = pack2<TO>(v[0], v[1]);
               }
+          };
+          using Y = std::true_type;
+          using N = std::false_type;
+          if constexpr (KS > 0) {
+            // post slope 1 without clamp is the identity: skipping it leaves every finite value's bits unchanged
+            const bool hp = p.post_slope != 1.f || p.post_clamp3;
+            if (gate != nullptr) {
+              if (res != nullptr) { if (hp) values(Y{}, Y{}, Y{}); else values(Y{}, Y{}, N{}); }
+              else { if (hp) values(Y{}, N{}, Y{}); else values(Y{}, N{}, N{}); }
+            } else {
+              if (res != nullptr) { if (hp) values(N{}, Y{}, Y{}); else values(N{}, Y{}, N{}); }
+              else { if (hp) values(N{}, N{}, Y{}); else values(N{}, N{}, N{}); }
             }
+          } else {
+            values(Y{}, Y{}, Y{});
+          }
+          if (RV_TL_DIAG == 4) {
+            if (fold == 0x7fc00001u) out[0] = from_f<TO>(0.f);   // practically never taken: keeps the values live
+            RV_TL(tl0, NCONS + cons, it, 8);
+            continue;
+          }
           tc::fence_proxy_async();                  // the buffer's writes, before the async proxy reads them
           asm volatile("bar.sync %0, 128;" ::"r"(1 + cons) : "memory");
           if (t == 0) {

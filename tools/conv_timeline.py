@@ -4,9 +4,10 @@ Builds conv_tc.cu with -DRV_CONV_TIMELINE into a separate library (linked with t
 build(), which must have run), loads it in place of librefvsr_b200.so and runs the 3x3 convs that dominate a window.
 The instrumented kernel writes clock64 stamps per CTA, per role and per local tile (see RV_TL in conv_tc.cu); this prints,
 per phase, the median and p90 cycles per tile, the time per tile per CTA, and the share of each CTA's span in which at
-least one consumer has wgmmas in flight.  Besides the product kernel (`full`) it runs three diagnostic variants that split
+least one consumer has wgmmas in flight.  Besides the product kernel (`full`) it runs four diagnostic variants that split
 the cost: `mma` (the consumers re-issue the 54-wgmma batch on a resident slot: no slot waits, no epilogue), `mma_aligned`
-(the same count with every A view on a 1024-byte swizzle atom) and `epi` (epilogue only).  The variants need convs with
+(the same count with every A view on a 1024-byte swizzle atom), `epi` (epilogue only) and `nosmem_epi` (the full
+pipeline with an epilogue that neither reads nor writes shared memory; TMA-store kernels only).  The variants need convs with
 one pipeline stage per tile (one channel chunk), which all shapes here are.
 
     python tools/conv_timeline.py [--csrc DIR] [--tag NAME] [--json FILE] [--out DIR] [--build-only | --prebuilt]
@@ -27,7 +28,7 @@ import tempfile
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-VARIANTS = {'full': 0, 'mma': 1, 'mma_aligned': 2, 'epi': 3}
+VARIANTS = {'full': 0, 'mma': 1, 'mma_aligned': 2, 'epi': 3, 'nosmem_epi': 4}
 
 
 def build_lib(csrc, out_dir):
