@@ -99,6 +99,13 @@ typedef struct rv_conv_desc {
                          /*   (packing.ps_rows_order: cout = 2*nb, block a = HR sub-row a, */
                          /*   both sub-pixels x all cout/4 channels; weights and bias      */
                          /*   permuted to match).  Other descs must leave it 0.            */
+  /* Batch: n images through one launch, each computed exactly as alone (a tile never reads across an image's border).   */
+  /* n = 0 or 1: one image, the strides are ignored.  n > 1: image i of an operand starts i * bs_* ELEMENTS after its     */
+  /* pointer; every stride of a non-null operand must be > 0 (TC: src0 / src1 strides multiples of 8).  The tensor-core   */
+  /* path runs all n x tiles in one persistent launch with the weights loaded once per CTA; the SIMT path issues one       */
+  /* launch per image.                                                                                                    */
+  int32_t n;
+  int64_t bs_src0, bs_src1, bs_gate, bs_res, bs_out;
 } rv_conv_desc;
 
 int rv_conv2d(const rv_conv_desc* d, void* stream);
@@ -233,6 +240,11 @@ int rv_flow_resize(const float* flow, int H, int W, float* out, int h, int w, vo
  * ------------------------------------------------------------------------------------------------ */
 int rv_warp(const void* src, int Hi, int Wi, int C, int dtype, const float* flow, int hf, int wf,
             int flow_up2, void* out, void* stream);
+/* Batched entry points (`*_batched`): the same arguments plus `n`, the number of images, before `stream`.  Every operand
+ * holds n images back to back ([n][...] in the layout of the one-image call), and image i is computed exactly as the
+ * one-image call on the i-th slices would compute it, in one launch (the image is gridDim.z).  1 <= n <= 65535. */
+int rv_warp_batched(const void* src, int Hi, int Wi, int C, int dtype, const float* flow, int hf, int wf,
+                    int flow_up2, void* out, int n, void* stream);
 /* The three warps of one propagation step fused into ONE launch (RefVSR.py:216-220 backward branch, :256-260 steady forward
  * step): out_feat = warp(feat, flow), out_conf = warp(conf, flow), out_featUP = warp(featUP, interpolate(flow, x2, bilinear,
  * align_corners=True) * 2).  feat (h,w,C), featUP (2h,2w,C) f16/bf16, conf (h,w) fp32, flow (h,w,2) fp32.  The flow is read
@@ -240,6 +252,8 @@ int rv_warp(const void* src, int Hi, int Wi, int C, int dtype, const float* flow
  * reads the OUTPUT of the LR warp.) */
 int rv_warp3(const void* feat, const void* featUP, const float* conf, const float* flow, int h, int w, int C, int dtype,
              void* out_feat, void* out_featUP, float* out_conf, void* stream);
+int rv_warp3_batched(const void* feat, const void* featUP, const float* conf, const float* flow, int h, int w, int C, int dtype,
+                     void* out_feat, void* out_featUP, float* out_conf, int n, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Matching (models/archs/RefVSR_/attention.py:69-91)
@@ -281,6 +295,8 @@ int rv_bicubic_up2_image(const float* src_nchw, int H, int W, void* out, int out
  * clamped to [0,1].  a,b planar fp32 (h,w). */
 int rv_conf_pair(const float* a, const float* b, int h, int w, int up2, void* out, int out_c,
                  int out_dtype, void* stream);
+int rv_conf_pair_batched(const float* a, const float* b, int h, int w, int up2, void* out, int out_c,
+                         int out_dtype, int n, void* stream);   /* see rv_warp_batched */
 int rv_conf_max(const float* a, const float* b, float* out, int n, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
@@ -298,6 +314,8 @@ int rv_frames_differ(const void* const* a, const void* const* b, const uint64_t*
  * ------------------------------------------------------------------------------------------------ */
 int rv_reconstruct(const void* x, int xc, int x_dtype, const float* lr_nchw, int h, int w, int scale,
                    int clamp01, float* out_nchw, void* stream);
+int rv_reconstruct_batched(const void* x, int xc, int x_dtype, const float* lr_nchw, int h, int w, int scale,
+                           int clamp01, float* out_nchw, int n, void* stream);   /* see rv_warp_batched */
 
 #ifdef __cplusplus
 }

@@ -82,6 +82,11 @@ struct TcP {
   int ps_vec;                    // pixel shuffle in that order: HR rows as 16-byte vectors or TMA boxes (PSV kernel)
   int out_tma;                   // the output tile is staged in a per-consumer shared-memory buffer and written by TMA
   uint32_t out_off, out_bytes;   // byte offset of those buffers from the ring / bytes of one
+  // Batch (rv_conv_desc::n): the persistent loop runs over nimg x tiles_x x tiles_y tiles, image-major.  With nimg > 1 every
+  // tensor map has the image as its last dimension, so a box never reaches into a neighbouring image (TMA's out-of-bounds fill
+  // is each image's own zero padding); per-thread loads and stores step by these element strides.  nimg = 1 keeps the 3-D maps.
+  int nimg;
+  long long bs_gate, bs_res, bs_out;
 };
 
 // HR-row column order of the pixel-shuffle convs (ps_order 1, cout = 2 NB, packing.ps_rows_order): column nl of block
@@ -243,7 +248,8 @@ __device__ __forceinline__ uint32_t pack2(float a, float b) {
 
 // NB: output channels per CTA (= p.NB); KS, KST: compile-time taps and K-steps of MODE 1 (0: the runtime loop, p.fixed = 0);
 // PSV: the 16-byte pixel-shuffle epilogue (p.ps_vec), which has no gate / residual
-template <typename TI, typename TR, typename TO, int MODE, int NB, int KS, int KST, bool PSV>
+// BATCH: p.nimg > 1 (a separate instantiation, so that one image keeps its single-image tile loop and addressing)
+template <typename TI, typename TR, typename TO, bool BATCH, int MODE, int NB, int KS, int KST, bool PSV>
 __global__ void __launch_bounds__(128 * (1 + NCONS), 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1,
                const __grid_constant__ CUtensorMap tmg, const __grid_constant__ CUtensorMap tmr,
@@ -261,7 +267,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
   const int warp = threadIdx.x >> 5;
   const int warp_u = __shfl_sync(0xffffffffu, warp, 0);
   const int nblk = blockIdx.y;
-  const int ntiles = p.tiles_x * p.tiles_y;
+  const int tiles_img = p.tiles_x * p.tiles_y;
+  const int ntiles = BATCH ? tiles_img * p.nimg : tiles_img;
+  constexpr bool batched = BATCH;
   const int nchunks = p.nch0 + p.nch1;
   RV_TL_INIT;
 
@@ -334,7 +342,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
       int buf = 0, it = 0;
       uint32_t eph = 0;
       for (int tile = blockIdx.x + pc * gridDim.x; tile < ntiles; tile += NCONS * gridDim.x, ++it) {
-        const int ty = tile / p.tiles_x, tx = tile - ty * p.tiles_x;
+        const int img = BATCH ? tile / tiles_img : 0, ti = BATCH ? tile - img * tiles_img : tile;
+        const int ty = ti / p.tiles_x, tx = ti - ty * p.tiles_x;
         RV_TL(tl0, pc, it, 3);
         tc::mbar_wait(&bar_eempty[pc][buf], eph ^ 1u);
         RV_TL(tl0, pc, it, 4);
@@ -342,8 +351,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
           uint64_t* bar = &bar_efull[pc][buf];
           uint8_t* g = epi_buf(pc, buf);
           tc::mbar_expect_tx(bar, p.epi_tx);
-          if (gate_p != nullptr) tc::tma_load_3d(&tmg, bar, g, nblk * NB, tx * p.tw, ty * p.th);
-          if (p.res != nullptr) tc::tma_load_3d(&tmr, bar, epi_res(g), nblk * NB, tx * p.tw, ty * p.th);
+          if (batched) {
+            if (gate_p != nullptr) tc::tma_load_4d(&tmg, bar, g, nblk * NB, tx * p.tw, ty * p.th, img);
+            if (p.res != nullptr) tc::tma_load_4d(&tmr, bar, epi_res(g), nblk * NB, tx * p.tw, ty * p.th, img);
+          } else {
+            if (gate_p != nullptr) tc::tma_load_3d(&tmg, bar, g, nblk * NB, tx * p.tw, ty * p.th);
+            if (p.res != nullptr) tc::tma_load_3d(&tmr, bar, epi_res(g), nblk * NB, tx * p.tw, ty * p.th);
+          }
         }
         __syncwarp();
         RV_TL(tl0, pc, it, 5);
@@ -370,7 +384,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
         tc::mbar_wait(&bar_fill[pc], fph);
         fph ^= 1u;
       }
-      const int ty0 = tile / p.tiles_x, tx0 = tile - ty0 * p.tiles_x;
+      const int img = BATCH ? tile / tiles_img : 0, ti = BATCH ? tile - img * tiles_img : tile;
+      const int ty0 = ti / p.tiles_x, tx0 = ti - ty0 * p.tiles_x;
       const int yc = ty0 * p.th - p.pad, xc = tx0 * p.tw - p.pad;
       int kx = 0, ch = 0;
       for (int s = 0; s < p.S; ++s) {
@@ -381,14 +396,18 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
           uint64_t* bar = &bar_full[pc][slot];
           uint8_t* dst = ring + ((size_t)pc * p.slots + slot) * p.slot_bytes;
           tc::mbar_expect_tx(bar, tx_bytes);
+          auto load = [&](const CUtensorMap* m, uint8_t* d, int c) {
+            if (batched) tc::tma_load_4d(m, bar, d, c, xc + kx, yc, img);
+            else tc::tma_load_3d(m, bar, d, c, xc + kx, yc);
+          };
           if constexpr (MODE == 2) {
             for (int qd = 0; qd < p.nq0 + p.nq1; ++qd) {
-              if (qd < p.nq0) tc::tma_load_3d(&tm0, bar, dst + (size_t)qd * p.q_bytes, qd * 16, xc + kx, yc);
-              else tc::tma_load_3d(&tm1, bar, dst + (size_t)qd * p.q_bytes, (qd - p.nq0) * 16, xc + kx, yc);
+              if (qd < p.nq0) load(&tm0, dst + (size_t)qd * p.q_bytes, qd * 16);
+              else load(&tm1, dst + (size_t)qd * p.q_bytes, (qd - p.nq0) * 16);
             }
           } else {
-            if (ch < p.nch0) tc::tma_load_3d(&tm0, bar, dst, ch * 64, xc + kx, yc);
-            else tc::tma_load_3d(&tm1, bar, dst, (ch - p.nch0) * 64, xc + kx, yc);
+            if (ch < p.nch0) load(&tm0, dst, ch * 64);
+            else load(&tm1, dst, (ch - p.nch0) * 64);
           }
           if (!p.resident) tc::bulk_load(wsrc + (size_t)s * p.w_bytes, bar, dst + p.a_bytes, p.w_bytes);
         }
@@ -406,9 +425,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
     // ============================ consumers ================================
     const int cons = (warp_u >> 2) - 1;
     const int t = threadIdx.x & 127, wq = t >> 5, lane = t & 31;
-    const TI* gate = reinterpret_cast<const TI*>(p.gate);
-    const TR* res = reinterpret_cast<const TR*>(p.res);
-    TO* out = reinterpret_cast<TO*>(p.out);
+    const TI* const gate0 = reinterpret_cast<const TI*>(p.gate);
+    const TR* const res0 = reinterpret_cast<const TR*>(p.res);
+    TO* const out0 = reinterpret_cast<TO*>(p.out);
     const uint32_t ring_addr = tc::smem_u32(ring + (size_t)cons * p.slots * p.slot_bytes);
     const uint32_t w_addr = tc::smem_u32(smemW);
     if (p.resident) tc::mbar_wait(&bar_w, 0);
@@ -435,7 +454,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
     const bool tl0 = t == 0;
     (void)tl0;
     for (int tile = blockIdx.x + cons * gridDim.x; tile < ntiles; tile += NCONS * gridDim.x, ++it) {
-      const int ty0 = tile / p.tiles_x, tx0 = tile - ty0 * p.tiles_x;
+      const int img = BATCH ? tile / tiles_img : 0, ti = BATCH ? tile - img * tiles_img : tile;
+      const int ty0 = ti / p.tiles_x, tx0 = ti - ty0 * p.tiles_x;
+      const TI* const gate = BATCH && gate0 != nullptr ? gate0 + img * p.bs_gate : gate0;
+      const TR* const res = BATCH && res0 != nullptr ? res0 + img * p.bs_res : res0;
+      TO* const out = BATCH ? out0 + img * p.bs_out : out0;
       if (RV_TL_DIAG == 3) {
 #pragma unroll
         for (int h = 0; h < 2; ++h)
@@ -588,8 +611,16 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
                 const uint32_t pix = (uint32_t)(r - 8 * h) * 2 * p.tw + 2 * x + b;
                 *reinterpret_cast<uint4*>(out_s + (pix * (NB / 2) + 8 * c8) * 2u) = vec;
               } else if (in) {
-                TO* o = out + ((size_t)(2 * oy + nblk) * (2 * p.Wo) + 2 * ox + b) * p.out_cs + 8 * c8;
-                *reinterpret_cast<uint4*>(o) = vec;
+                if constexpr (BATCH) {
+                  // in 16-byte units from the image's base (out_cs and the image stride are multiples of 8), so that the
+                  // store stays one 16-byte access
+                  uint4* o = reinterpret_cast<uint4*>(out0) + (size_t)img * (p.bs_out >> 3) +
+                             ((size_t)(2 * oy + nblk) * (2 * p.Wo) + 2 * ox + b) * (p.out_cs >> 3) + c8;
+                  *o = vec;
+                } else {
+                  TO* o = out + ((size_t)(2 * oy + nblk) * (2 * p.Wo) + 2 * ox + b) * p.out_cs + 8 * c8;
+                  *reinterpret_cast<uint4*>(o) = vec;
+                }
               }
             }
           }
@@ -597,7 +628,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
             tc::fence_proxy_async();                  // the buffer's writes, before the async proxy reads them
             asm volatile("bar.sync %0, 128;" ::"r"(1 + cons) : "memory");
             if (t == 0) {
-              tc::tma_store_4d(&tmo, out_s, 0, 2 * tx0 * p.tw, nblk, ty0 * p.th + 8 * h);
+              if (batched) tc::tma_store_5d(&tmo, out_s, 0, 2 * tx0 * p.tw, nblk, ty0 * p.th + 8 * h, img);
+              else tc::tma_store_4d(&tmo, out_s, 0, 2 * tx0 * p.tw, nblk, ty0 * p.th + 8 * h);
               tc::bulk_commit();
             }
           }
@@ -680,7 +712,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
           tc::fence_proxy_async();                  // the buffer's writes, before the async proxy reads them
           asm volatile("bar.sync %0, 128;" ::"r"(1 + cons) : "memory");
           if (t == 0) {
-            tc::tma_store_3d(&tmo, out_s, nblk * NB, tx0 * p.tw, ty0 * p.th);
+            if (batched) tc::tma_store_4d(&tmo, out_s, nblk * NB, tx0 * p.tw, ty0 * p.th, img);
+            else tc::tma_store_3d(&tmo, out_s, nblk * NB, tx0 * p.tw, ty0 * p.th);
             tc::bulk_commit();
           }
           RV_TL(tl0, NCONS + cons, it, 8);
@@ -755,17 +788,18 @@ PFN_tmapEncodeTiled get_tmap_encoder() {
 }
 
 // 16-bit NHWC map [H][W][C] with `cs` (default C) channels between pixels, boxes of box_c x box_w x box_rows;
-// out-of-bounds elements read as zero and are not written
+// out-of-bounds elements read as zero and are not written.  n > 1: [n][H][W][C] with `bs` elements between images, a 4th
+// dimension of box size 1, so that a box stops at its own image's border.
 static int make_tmap_3d(CUtensorMap* m, const void* ptr, int C, int W, int H, int box_c, int box_w, int box_rows, int fmt,
-                        CUtensorMapSwizzle swz, int cs = 0) {
+                        CUtensorMapSwizzle swz, int cs = 0, int n = 1, long long bs = 0) {
   PFN_tmapEncodeTiled enc = get_tmap_encoder();
   if (!enc) return fail(RV_E_CUDA, "cuTensorMapEncodeTiled entry point not available");
   if (cs == 0) cs = C;
-  cuuint64_t gdim[3] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H};
-  cuuint64_t gstr[2] = {(cuuint64_t)cs * 2, (cuuint64_t)W * cs * 2};
-  cuuint32_t box[3] = {(cuuint32_t)box_c, (cuuint32_t)box_w, (cuuint32_t)box_rows};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(m, fmt ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3,
+  cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)n};
+  cuuint64_t gstr[3] = {(cuuint64_t)cs * 2, (cuuint64_t)W * cs * 2, (cuuint64_t)bs * 2};
+  cuuint32_t box[4] = {(cuuint32_t)box_c, (cuuint32_t)box_w, (cuuint32_t)box_rows, 1};
+  cuuint32_t estr[4] = {1, 1, 1, 1};
+  CUresult r = enc(m, fmt ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, n > 1 ? 4 : 3,
                    const_cast<void*>(ptr), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(RV_E_CUDA, "cuTensorMapEncodeTiled failed (%d) C=%d W=%d H=%d", (int)r, C, W, H);
@@ -773,24 +807,28 @@ static int make_tmap_3d(CUtensorMap* m, const void* ptr, int C, int W, int H, in
 }
 
 // the 16-bit pixel-shuffled output [2 Ho][2 Wo][cs] of an LR Ho x Wo map as (channel, HR x, sub-row a, LR y), so that one
-// box of C x 2 tw x 1 x rows is HR rows 2 y + a of `rows` LR rows; out-of-bounds elements are not written
-static int make_ps_rows_tmap(CUtensorMap* m, const void* ptr, int C, int cs, int Wo, int Ho, int tw, int rows, int fmt) {
+// box of C x 2 tw x 1 x rows is HR rows 2 y + a of `rows` LR rows; out-of-bounds elements are not written.  n > 1: the image
+// is a 5th dimension, `bs` elements apart.
+static int make_ps_rows_tmap(CUtensorMap* m, const void* ptr, int C, int cs, int Wo, int Ho, int tw, int rows, int fmt,
+                             int n = 1, long long bs = 0) {
   PFN_tmapEncodeTiled enc = get_tmap_encoder();
   if (!enc) return fail(RV_E_CUDA, "cuTensorMapEncodeTiled entry point not available");
   const cuuint64_t px = (cuuint64_t)cs * 2;
-  cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)2 * Wo, 2, (cuuint64_t)Ho};
-  cuuint64_t gstr[3] = {px, 2 * Wo * px, 4 * Wo * px};
-  cuuint32_t box[4] = {(cuuint32_t)C, (cuuint32_t)2 * tw, 1, (cuuint32_t)rows};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  CUresult r = enc(m, fmt ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(ptr), gdim,
+  cuuint64_t gdim[5] = {(cuuint64_t)C, (cuuint64_t)2 * Wo, 2, (cuuint64_t)Ho, (cuuint64_t)n};
+  cuuint64_t gstr[4] = {px, 2 * Wo * px, 4 * Wo * px, (cuuint64_t)bs * 2};
+  cuuint32_t box[5] = {(cuuint32_t)C, (cuuint32_t)2 * tw, 1, (cuuint32_t)rows, 1};
+  cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+  CUresult r = enc(m, fmt ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, n > 1 ? 5 : 4, const_cast<void*>(ptr), gdim,
                    gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(RV_E_CUDA, "cuTensorMapEncodeTiled (HR rows) failed (%d) C=%d W=%d H=%d", (int)r, C, Wo, Ho);
   return RV_OK;
 }
 
-static int make_act_tmap(CUtensorMap* m, const void* ptr, int C, int W, int H, int box_w, int box_rows, int fmt, int sw32 = 0) {
-  return make_tmap_3d(m, ptr, C, W, H, sw32 ? 16 : 64, box_w, box_rows, fmt, sw32 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_128B);
+static int make_act_tmap(CUtensorMap* m, const void* ptr, int C, int W, int H, int box_w, int box_rows, int fmt, int sw32,
+                         int n, long long bs) {
+  return make_tmap_3d(m, ptr, C, W, H, sw32 ? 16 : 64, box_w, box_rows, fmt, sw32 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_128B,
+                      0, n, bs);
 }
 
 static int g_num_sms = 0;
@@ -802,11 +840,12 @@ int set_conv_smem_cap(int bytes) { const int old = g_smem_cap; g_smem_cap = byte
 
 template <typename TI, typename TR, typename TO, int MODE, int NB, int KS = 0, int KST = 0, bool PSV = false>
 static int launch_tc_mode(const CUtensorMap* tm, const TcP& p, dim3 grid, size_t smem, cudaStream_t st) {
-  auto kern = conv_tc_kernel<TI, TR, TO, MODE, NB, KS, KST, PSV>;
-  static size_t configured = 0;   // per template instantiation
-  if (smem > configured) {
+  const int batch = p.nimg > 1 ? 1 : 0;
+  auto kern = batch ? conv_tc_kernel<TI, TR, TO, true, MODE, NB, KS, KST, PSV> : conv_tc_kernel<TI, TR, TO, false, MODE, NB, KS, KST, PSV>;
+  static size_t configured[2] = {0, 0};   // per template instantiation
+  if (smem > configured[batch]) {
     RV_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured = smem;
+    configured[batch] = smem;
   }
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
@@ -870,6 +909,14 @@ static int plan_tc(const rv_conv_desc* d, TcP& p, size_t& smem_out, int& nblk_ou
   p.Ho = d->H + 2 * d->pad - d->kh + 1;
   p.Wo = d->W + 2 * d->pad - d->kw + 1;
   RV_REQUIRE(p.Ho > 0 && p.Wo > 0, "rv_conv2d: empty output");
+  p.nimg = d->n > 1 ? d->n : 1;
+  const bool batched = p.nimg > 1;
+  // the activation maps' image strides must keep every image's base 16-byte aligned (TMA global strides)
+  RV_REQUIRE(!batched || (d->bs_src0 % 8 == 0 && (!d->src1 || d->bs_src1 % 8 == 0)),
+             "rv_conv2d(tc): n=%d needs image strides of src0 / src1 that are multiples of 8 elements", d->n);
+  p.bs_gate = batched && d->gate ? d->bs_gate : 0;
+  p.bs_res = batched && d->res ? d->bs_res : 0;
+  p.bs_out = batched ? d->bs_out : 0;
   p.kh = d->kh; p.kw = d->kw; p.pad = d->pad;
   p.c0 = d->c0; p.c1 = d->src1 ? d->c1 : 0;
   p.nch0 = (p.c0 + 63) / 64; p.nch1 = (p.c1 + 63) / 64;
@@ -911,11 +958,13 @@ static int plan_tc(const rv_conv_desc* d, TcP& p, size_t& smem_out, int& nblk_ou
   // TMA epilogue: 16-bit gate / residual whose boxes TMA can address (16-byte aligned base and pixel stride), tiles the
   // register epilogue keeps whole (NB <= 48), and room for the buffers next to resident weights and the minimal ring
   const int rdt0 = d->res ? d->res_dtype : d->in_dtype;
-  auto tma_ok = [](const void* q, int cs) { return q == nullptr || ((uintptr_t)q % 16 == 0 && cs > 0 && cs % 8 == 0); };
+  auto tma_ok = [batched](const void* q, int cs, long long bs) {
+    return q == nullptr || ((uintptr_t)q % 16 == 0 && cs > 0 && cs % 8 == 0 && (!batched || bs % 8 == 0));
+  };
   p.epi_bytes = (uint32_t)p.th * p.tw * p.NB * 2;
   p.epi_tx = (uint32_t)((d->gate ? 1 : 0) + (d->res ? 1 : 0)) * p.epi_bytes;
-  p.epi_tma = (d->gate || d->res) && p.NB <= 48 && rdt0 == d->in_dtype && tma_ok(d->gate, d->gate_cs) &&
-              tma_ok(d->res, d->res_cs) && w_all + ring_min + (size_t)NCONS * p.epi_tx <= budget;
+  p.epi_tma = (d->gate || d->res) && p.NB <= 48 && rdt0 == d->in_dtype && tma_ok(d->gate, d->gate_cs, d->bs_gate) &&
+              tma_ok(d->res, d->res_cs, d->bs_res) && w_all + ring_min + (size_t)NCONS * p.epi_tx <= budget;
   // a second buffer lets the boxes arrive up to two tiles ahead of the epilogue; it is taken only while two A slots and the
   // output buffer per consumer still fit (gate + residual at NB = 48 keeps two A slots and one buffer)
   p.epi_depth = p.epi_tma && w_all + (size_t)NCONS * (2 * p.a_bytes + MAX_EPI * p.epi_tx + p.epi_bytes) <= budget ? MAX_EPI : 1;
@@ -932,7 +981,7 @@ static int plan_tc(const rv_conv_desc* d, TcP& p, size_t& smem_out, int& nblk_ou
   // stores of the general epilogue
   p.ps_order = d->ps_order;
   p.ps_vec = p.fixed && d->pixel_shuffle && d->ps_order && p.NB == 96 && dtype_size(d->out_dtype) == 2 && !d->gate &&
-             !d->res && d->out != nullptr && (uintptr_t)d->out % 16 == 0 && (d->out_cs * 2) % 16 == 0;
+             !d->res && d->out != nullptr && (uintptr_t)d->out % 16 == 0 && (d->out_cs * 2) % 16 == 0 && (!batched || d->bs_out % 8 == 0);
   RV_REQUIRE(!d->ps_order || p.ps_vec, "rv_conv2d(tc): ps_order=1 needs the 3x3 48-channel nb=96 kernel with a 16-bit output "
              "whose HR pixel rows are 16-byte aligned (out_cs=%d), no gate / residual", d->out_cs);
   // TMA-store epilogue, when its buffer per consumer fits next to the resident weights, the gate / residual buffers and the
@@ -940,7 +989,7 @@ static int plan_tc(const rv_conv_desc* d, TcP& p, size_t& smem_out, int& nblk_ou
   // and pixel stride TMA can address ([128 pixels][NB] buffer, th x tw of the layout mode), and the PSV kernel (half a tile of HR rows,
   // [8 rows][16 pixels][NB / 2]: a whole tile's buffers would leave one A slot per consumer next to the 108 KB of weights)
   const bool out_plain = p.NB <= 48 && !d->pixel_shuffle && d->out_dtype == d->in_dtype && d->out != nullptr &&
-                         tma_ok(d->out, d->out_cs);
+                         tma_ok(d->out, d->out_cs, d->bs_out);
   p.out_bytes = p.ps_vec ? p.epi_bytes / 2 : p.epi_bytes;
   p.out_tma = (out_plain || p.ps_vec) && w_all + ring_min + epi_all + (size_t)NCONS * p.out_bytes <= budget;
   const size_t out_all = p.out_tma ? (size_t)NCONS * p.out_bytes : 0;
@@ -994,25 +1043,32 @@ int conv2d_tc(const rv_conv_desc* d, cudaStream_t st) {
   const int rdt = d->res ? d->res_dtype : d->out_dtype;
   const int sw32 = p.mode == 2;
   CUtensorMap tm[5];    // src0, src1, gate, res, out (unused ones: copies of src0)
-  int rc = make_act_tmap(&tm[0], d->src0, p.c0, d->W, d->H, p.mode == 1 ? p.tw + d->kw - 1 : p.tw, p.th + d->kh - 1, p.fmt, sw32);
+  const int n = p.nimg;
+  int rc = make_act_tmap(&tm[0], d->src0, p.c0, d->W, d->H, p.mode == 1 ? p.tw + d->kw - 1 : p.tw, p.th + d->kh - 1, p.fmt, sw32,
+                         n, d->bs_src0);
   if (rc) return rc;
   tm[1] = tm[2] = tm[3] = tm[4] = tm[0];
   if (p.c1) {
-    rc = make_act_tmap(&tm[1], d->src1, p.c1, d->W, d->H, p.mode == 1 ? p.tw + d->kw - 1 : p.tw, p.th + d->kh - 1, p.fmt, sw32);
+    rc = make_act_tmap(&tm[1], d->src1, p.c1, d->W, d->H, p.mode == 1 ? p.tw + d->kw - 1 : p.tw, p.th + d->kh - 1, p.fmt, sw32,
+                       n, d->bs_src1);
     if (rc) return rc;
   }
   // gate / residual boxes for the TMA epilogue: [th][tw][NB], unswizzled, so box pixel m sits at m * NB channels
-  if (p.epi_tma && d->gate && (rc = make_tmap_3d(&tm[2], d->gate, d->gate_cs, p.Wo, p.Ho, p.NB, p.tw, p.th, p.fmt, CU_TENSOR_MAP_SWIZZLE_NONE)))
+  if (p.epi_tma && d->gate &&
+      (rc = make_tmap_3d(&tm[2], d->gate, d->gate_cs, p.Wo, p.Ho, p.NB, p.tw, p.th, p.fmt, CU_TENSOR_MAP_SWIZZLE_NONE, 0, n, d->bs_gate)))
     return rc;
-  if (p.epi_tma && d->res && (rc = make_tmap_3d(&tm[3], d->res, d->res_cs, p.Wo, p.Ho, p.NB, p.tw, p.th, p.fmt, CU_TENSOR_MAP_SWIZZLE_NONE)))
+  if (p.epi_tma && d->res &&
+      (rc = make_tmap_3d(&tm[3], d->res, d->res_cs, p.Wo, p.Ho, p.NB, p.tw, p.th, p.fmt, CU_TENSOR_MAP_SWIZZLE_NONE, 0, n, d->bs_res)))
     return rc;
   // output tiles [th][tw][NB] of the TMA-store epilogue; channels >= cout (and pixels outside the map) are not written
   if (p.out_tma && !p.ps_vec &&
-      (rc = make_tmap_3d(&tm[4], d->out, d->cout, p.Wo, p.Ho, p.NB, p.tw, p.th, p.fmt, CU_TENSOR_MAP_SWIZZLE_NONE, d->out_cs)))
+      (rc = make_tmap_3d(&tm[4], d->out, d->cout, p.Wo, p.Ho, p.NB, p.tw, p.th, p.fmt, CU_TENSOR_MAP_SWIZZLE_NONE, d->out_cs,
+                         n, d->bs_out)))
     return rc;
-  if (p.out_tma && p.ps_vec && (rc = make_ps_rows_tmap(&tm[4], d->out, d->cout / 4, d->out_cs, p.Wo, p.Ho, p.tw, p.th / 2, p.fmt)))
+  if (p.out_tma && p.ps_vec &&
+      (rc = make_ps_rows_tmap(&tm[4], d->out, d->cout / 4, d->out_cs, p.Wo, p.Ho, p.tw, p.th / 2, p.fmt, n, d->bs_out)))
     return rc;
-  const int ntiles = p.tiles_x * p.tiles_y;
+  const int ntiles = p.tiles_x * p.tiles_y * n;
   int gx = std::min(ntiles, std::max(1, g_num_sms / nblk));
   if (g_cta_cap > 0) gx = std::min(gx, std::max(1, g_cta_cap / nblk));     // two capped launches on different streams share the SMs
   dim3 grid(gx, nblk);

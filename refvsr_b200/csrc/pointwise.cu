@@ -311,6 +311,9 @@ __global__ void warp_kernel(const T* __restrict__ src, int Hi, int Wi, int C,
                             T* __restrict__ out) {
   const int Ho = flow_up2 ? 2 * hf : hf, Wo = flow_up2 ? 2 * wf : wf;
   const int cv = C / V;
+  src += (size_t)blockIdx.z * Hi * Wi * C;           // image blockIdx.z of a batch (rv_warp_batched)
+  flow += (size_t)blockIdx.z * hf * wf * 2;
+  out += (size_t)blockIdx.z * Ho * Wo * C;
   long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)Ho * Wo * cv) return;
   int vc = (int)(i % cv);
@@ -390,6 +393,9 @@ __global__ void __launch_bounds__(256) warp_vec_kernel(const T* __restrict__ src
   __shared__ int4 s_o[256];
   const int Ho = flow_up2 ? 2 * hf : hf, Wo = flow_up2 ? 2 * wf : wf;
   const int cv = C / (V * NV);      // threads per pixel; each moves NV consecutive 16-byte vectors
+  src += (size_t)blockIdx.z * Hi * Wi * C;           // image blockIdx.z of a batch (rv_warp_batched)
+  flow += (size_t)blockIdx.z * hf * wf * 2;
+  out += (size_t)blockIdx.z * Ho * Wo * C;
   const int npix = Ho * Wo;
   const int p0 = blockIdx.x * ppb;
   if (threadIdx.x < ppb && p0 + threadIdx.x < npix) {
@@ -498,6 +504,11 @@ __global__ void __launch_bounds__(256) warp3_kernel(const T* __restrict__ feat, 
   const int tiles_x = (w + W3_TW - 1) / W3_TW;
   const int ty0 = (blockIdx.x / tiles_x) * W3_TH, tx0 = (blockIdx.x % tiles_x) * W3_TW;
   const int H2 = 2 * h, W2 = 2 * w;
+  {                                                  // image blockIdx.z of a batch (rv_warp3_batched)
+    const size_t px = (size_t)blockIdx.z * h * w;
+    feat += px * C; o_feat += px * C; featUP += 4 * px * C; o_featUP += 4 * px * C;
+    conf += px; o_conf += px; flow += 2 * px;
+  }
   // ---- phase 0: LR flow tile with a one-pixel halo (the x2 flow of a tile reads rows / columns ty0 - 1 .. ty0 + TH)
   for (int i = threadIdx.x; i < (W3_TH + 2) * (W3_TW + 2); i += blockDim.x) {
     const int yy = clampi(ty0 - 1 + i / (W3_TW + 2), 0, h - 1), xx = clampi(tx0 - 1 + i % (W3_TW + 2), 0, w - 1);
@@ -932,6 +943,9 @@ template <typename T>
 __global__ void conf_pair_kernel(const float* __restrict__ a, const float* __restrict__ b, int h,
                                  int w, int up2, T* __restrict__ out, int out_c) {
   int Ho = up2 ? 2 * h : h, Wo = up2 ? 2 * w : w;
+  a += (size_t)blockIdx.z * h * w;                   // image blockIdx.z of a batch (rv_conf_pair_batched)
+  b += (size_t)blockIdx.z * h * w;
+  out += (size_t)blockIdx.z * Ho * Wo * out_c;
   int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= Ho * Wo) return;
   float va, vb;
@@ -960,6 +974,9 @@ __global__ void reconstruct_kernel(const T* __restrict__ x, int xc, const float*
                                    int h, int w, int scale, int clamp01,
                                    float* __restrict__ out) {
   int Ho = scale * h, Wo = scale * w;
+  x += (size_t)blockIdx.z * Ho * Wo * xc;            // image blockIdx.z of a batch (rv_reconstruct_batched)
+  lr += (size_t)blockIdx.z * 3 * h * w;
+  out += (size_t)blockIdx.z * 3 * Ho * Wo;
   int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= Ho * Wo) return;
   int Y = p / Wo, X = p % Wo;
@@ -1005,6 +1022,9 @@ __global__ void frames_differ_kernel(const CmpPairs P, int* __restrict__ flag) {
 // vectors of the planar result.  Weights, tap order and summation order are those of bicubic_planar (bit-identical).
 __global__ void __launch_bounds__(128) reconstruct4_kernel(const float4* __restrict__ x, const float* __restrict__ lr, int h, int w,
                                                            int clamp01, float* __restrict__ out) {
+  x += (size_t)blockIdx.z * 16 * h * w;              // image blockIdx.z of a batch (rv_reconstruct_batched)
+  lr += (size_t)blockIdx.z * 3 * h * w;
+  out += (size_t)blockIdx.z * 48 * h * w;
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= h * w) return;
   const int ly = p / w, lx = p - ly * w;
@@ -1079,6 +1099,9 @@ __device__ __forceinline__ float row4(const float* wt, float v0, float v1, float
 // compile-time constants, which would otherwise let the compiler fuse the other product of a row).
 __global__ void __launch_bounds__(128) reconstruct2_kernel(const float4* __restrict__ x, const float* __restrict__ lr, int h, int w,
                                                            int clamp01, float* __restrict__ out) {
+  x += (size_t)blockIdx.z * 4 * h * w;               // image blockIdx.z of a batch (rv_reconstruct_batched)
+  lr += (size_t)blockIdx.z * 3 * h * w;
+  out += (size_t)blockIdx.z * 12 * h * w;
   const int p = blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= h * w) return;
   const int ly = p / w, lx = p - ly * w;
@@ -1205,34 +1228,41 @@ extern "C" int rv_flow_resize(const float* flow, int H, int W, float* out, int h
 
 template <typename T>
 static int warp_launch(const void* src, int Hi, int Wi, int C, const float* flow, int hf, int wf,
-                       int up2, void* out, cudaStream_t st) {
+                       int up2, void* out, int nimg, cudaStream_t st) {
   constexpr int VMAX = 16 / sizeof(T);
   long long px = (long long)(up2 ? 4 : 1) * hf * wf;
   bool aligned = ((uintptr_t)src % 16 == 0) && ((uintptr_t)out % 16 == 0);
   if (false && C % (2 * VMAX) == 0 && aligned && C / (2 * VMAX) <= 256) {   // 32 B / thread variant: disabled
     const int cv = C / (2 * VMAX), ppb = 256 / cv;   // pixels per block, 32 bytes per thread
-    warp_vec_kernel<T, VMAX, 2><<<cdiv(px, ppb), 256, 0, st>>>((const T*)src, Hi, Wi, C, flow, hf, wf, up2, (T*)out, ppb);
+    warp_vec_kernel<T, VMAX, 2><<<dim3(cdiv(px, ppb), 1, nimg), 256, 0, st>>>((const T*)src, Hi, Wi, C, flow, hf, wf, up2, (T*)out, ppb);
   } else if (C % VMAX == 0 && aligned && C / VMAX <= 256) {
     const int cv = C / VMAX, ppb = 256 / cv;
-    warp_vec_kernel<T, VMAX, 1><<<cdiv(px, ppb), 256, 0, st>>>((const T*)src, Hi, Wi, C, flow, hf, wf, up2, (T*)out, ppb);
+    warp_vec_kernel<T, VMAX, 1><<<dim3(cdiv(px, ppb), 1, nimg), 256, 0, st>>>((const T*)src, Hi, Wi, C, flow, hf, wf, up2, (T*)out, ppb);
   } else {
     long long n = px * C;
-    warp_kernel<T, 1><<<cdiv(n, 256), 256, 0, st>>>((const T*)src, Hi, Wi, C, flow, hf, wf, up2, (T*)out);
+    warp_kernel<T, 1><<<dim3(cdiv(n, 256), 1, nimg), 256, 0, st>>>((const T*)src, Hi, Wi, C, flow, hf, wf, up2, (T*)out);
   }
   RV_LAUNCH_CHECK("warp");
   return RV_OK;
 }
 
-extern "C" int rv_warp(const void* src, int Hi, int Wi, int C, int dtype, const float* flow, int hf,
-                       int wf, int flow_up2, void* out, void* stream) {
+extern "C" int rv_warp_batched(const void* src, int Hi, int Wi, int C, int dtype, const float* flow, int hf,
+                               int wf, int flow_up2, void* out, int n, void* stream) {
   RV_REQUIRE(src && flow && out && Hi > 1 && Wi > 1 && C > 0 && hf > 0 && wf > 0, "rv_warp: bad arguments");
+  RV_REQUIRE(n >= 1 && n <= 65535, "rv_warp: n=%d images out of range", n);
   RV_REQUIRE((uintptr_t)flow % 8 == 0, "rv_warp: flow must be 8-byte aligned");
-  RV_DISPATCH_DTYPE(dtype, T, return (warp_launch<T>(src, Hi, Wi, C, flow, hf, wf, flow_up2, out, (cudaStream_t)stream)));
+  RV_DISPATCH_DTYPE(dtype, T, return (warp_launch<T>(src, Hi, Wi, C, flow, hf, wf, flow_up2, out, n, (cudaStream_t)stream)));
   return RV_OK;
 }
 
-extern "C" int rv_warp3(const void* feat, const void* featUP, const float* conf, const float* flow, int h, int w, int C,
-                        int dtype, void* out_feat, void* out_featUP, float* out_conf, void* stream) {
+extern "C" int rv_warp(const void* src, int Hi, int Wi, int C, int dtype, const float* flow, int hf,
+                       int wf, int flow_up2, void* out, void* stream) {
+  return rv_warp_batched(src, Hi, Wi, C, dtype, flow, hf, wf, flow_up2, out, 1, stream);
+}
+
+extern "C" int rv_warp3_batched(const void* feat, const void* featUP, const float* conf, const float* flow, int h, int w, int C,
+                                int dtype, void* out_feat, void* out_featUP, float* out_conf, int n, void* stream) {
+  RV_REQUIRE(n >= 1 && n <= 65535, "rv_warp3: n=%d images out of range", n);
   RV_REQUIRE(feat && featUP && conf && flow && out_feat && out_featUP && out_conf && h > 0 && w > 0, "rv_warp3: bad arguments");
   RV_REQUIRE(dtype == RV_F16 || dtype == RV_BF16, "rv_warp3: f16 / bf16 features only (use rv_warp for fp32)");
   RV_REQUIRE(C > 0 && C % 8 == 0, "rv_warp3: C=%d must be a multiple of 8", C);
@@ -1246,7 +1276,7 @@ extern "C" int rv_warp3(const void* feat, const void* featUP, const float* conf,
     constexpr int TH = decltype(thtag)::value, TW = 16;
     const int tiles = ((h + TH - 1) / TH) * ((w + TW - 1) / TW);
     const int threads = TH == 2 ? 160 : 256;
-    warp3_kernel<T, decltype(cvtag)::value, TH, TW><<<tiles, threads, 0, (cudaStream_t)stream>>>(
+    warp3_kernel<T, decltype(cvtag)::value, TH, TW><<<dim3(tiles, 1, n), threads, 0, (cudaStream_t)stream>>>(
         (const T*)feat, (const T*)featUP, conf, flow, h, w, C, (T*)out_feat, (T*)out_featUP, out_conf);
   };
   auto by_tile = [&](auto tag, auto cvtag) {
@@ -1264,6 +1294,11 @@ extern "C" int rv_warp3(const void* feat, const void* featUP, const float* conf,
   else by_cv(__nv_bfloat16{});
   RV_LAUNCH_CHECK("warp3");
   return RV_OK;
+}
+
+extern "C" int rv_warp3(const void* feat, const void* featUP, const float* conf, const float* flow, int h, int w, int C,
+                        int dtype, void* out_feat, void* out_featUP, float* out_conf, void* stream) {
+  return rv_warp3_batched(feat, featUP, conf, flow, h, w, C, dtype, out_feat, out_featUP, out_conf, 1, stream);
 }
 
 extern "C" int rv_patch_pack(const void* feat, int H, int W, int C, int dtype, int mode, void* out,
@@ -1402,14 +1437,20 @@ extern "C" int rv_resize_planes(const float* src, int n, int H, int W, float inv
   return RV_OK;
 }
 
-extern "C" int rv_conf_pair(const float* a, const float* b, int h, int w, int up2, void* out,
-                            int out_c, int out_dtype, void* stream) {
+extern "C" int rv_conf_pair_batched(const float* a, const float* b, int h, int w, int up2, void* out,
+                                    int out_c, int out_dtype, int nimg, void* stream) {
   RV_REQUIRE(a && b && out && h > 0 && w > 0 && out_c >= 2, "rv_conf_pair: bad arguments");
+  RV_REQUIRE(nimg >= 1 && nimg <= 65535, "rv_conf_pair: n=%d images out of range", nimg);
   long long n = (long long)(up2 ? 4 : 1) * h * w;
-  RV_DISPATCH_DTYPE(out_dtype, T, (conf_pair_kernel<T><<<cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(
+  RV_DISPATCH_DTYPE(out_dtype, T, (conf_pair_kernel<T><<<dim3(cdiv(n, 256), 1, nimg), 256, 0, (cudaStream_t)stream>>>(
                                       a, b, h, w, up2, (T*)out, out_c)));
   RV_LAUNCH_CHECK("conf_pair");
   return RV_OK;
+}
+
+extern "C" int rv_conf_pair(const float* a, const float* b, int h, int w, int up2, void* out,
+                            int out_c, int out_dtype, void* stream) {
+  return rv_conf_pair_batched(a, b, h, w, up2, out, out_c, out_dtype, 1, stream);
 }
 
 extern "C" int rv_conf_max(const float* a, const float* b, float* out, int n, void* stream) {
@@ -1419,20 +1460,26 @@ extern "C" int rv_conf_max(const float* a, const float* b, float* out, int n, vo
   return RV_OK;
 }
 
-extern "C" int rv_reconstruct(const void* x, int xc, int x_dtype, const float* lr, int h, int w,
-                              int scale, int clamp01, float* out, void* stream) {
+extern "C" int rv_reconstruct_batched(const void* x, int xc, int x_dtype, const float* lr, int h, int w,
+                                      int scale, int clamp01, float* out, int nimg, void* stream) {
   RV_REQUIRE(x && lr && out && h > 0 && w > 0 && xc >= 3 && (scale == 2 || scale == 4),
              "rv_reconstruct: bad arguments");
+  RV_REQUIRE(nimg >= 1 && nimg <= 65535, "rv_reconstruct: n=%d images out of range", nimg);
   long long n = (long long)scale * h * scale * w;
   static const bool fast_ok = getenv("REFVSR_NO_FAST_POINTWISE") == nullptr;
   if (fast_ok && scale == 4 && x_dtype == RV_F32 && xc == 4 && (uintptr_t)x % 16 == 0 && (uintptr_t)out % 16 == 0) {
-    reconstruct4_kernel<<<cdiv((long long)h * w, 128), 128, 0, (cudaStream_t)stream>>>((const float4*)x, lr, h, w, clamp01, out);
+    reconstruct4_kernel<<<dim3(cdiv((long long)h * w, 128), 1, nimg), 128, 0, (cudaStream_t)stream>>>((const float4*)x, lr, h, w, clamp01, out);
   } else if (fast_ok && scale == 2 && x_dtype == RV_F32 && xc == 4 && (uintptr_t)x % 16 == 0 && (uintptr_t)out % 8 == 0) {
-    reconstruct2_kernel<<<cdiv((long long)h * w, 128), 128, 0, (cudaStream_t)stream>>>((const float4*)x, lr, h, w, clamp01, out);
+    reconstruct2_kernel<<<dim3(cdiv((long long)h * w, 128), 1, nimg), 128, 0, (cudaStream_t)stream>>>((const float4*)x, lr, h, w, clamp01, out);
   } else {
-    RV_DISPATCH_DTYPE(x_dtype, T, (reconstruct_kernel<T><<<cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(
+    RV_DISPATCH_DTYPE(x_dtype, T, (reconstruct_kernel<T><<<dim3(cdiv(n, 256), 1, nimg), 256, 0, (cudaStream_t)stream>>>(
                                       (const T*)x, xc, lr, h, w, scale, clamp01, out)));
   }
   RV_LAUNCH_CHECK("reconstruct");
   return RV_OK;
+}
+
+extern "C" int rv_reconstruct(const void* x, int xc, int x_dtype, const float* lr, int h, int w,
+                              int scale, int clamp01, float* out, void* stream) {
+  return rv_reconstruct_batched(x, xc, x_dtype, lr, h, w, scale, clamp01, out, 1, stream);
 }

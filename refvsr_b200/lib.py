@@ -32,6 +32,8 @@ class rv_conv_desc(C.Structure):
         ('out', C.c_void_p), ('out_cs', C.c_int32), ('out_dtype', C.c_int32),
         ('pixel_shuffle', C.c_int32), ('impl', C.c_int32), ('nb', C.c_int32), ('k_real', C.c_int32),
         ('layout', C.c_int32), ('ps_order', C.c_int32),
+        ('n', C.c_int32),
+        ('bs_src0', C.c_int64), ('bs_src1', C.c_int64), ('bs_gate', C.c_int64), ('bs_res', C.c_int64), ('bs_out', C.c_int64),
     ]
 
 
@@ -81,6 +83,10 @@ SIGNATURES = {
     'rv_flow_resize': (_I, [_P, _I, _I, _P, _I, _I, _P]),
     'rv_warp': (_I, [_P, _I, _I, _I, _I, _P, _I, _I, _I, _P, _P]),
     'rv_warp3': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P]),
+    'rv_warp_batched': (_I, [_P, _I, _I, _I, _I, _P, _I, _I, _I, _P, _I, _P]),
+    'rv_warp3_batched': (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _I, _P]),
+    'rv_conf_pair_batched': (_I, [_P, _P, _I, _I, _I, _P, _I, _I, _I, _P]),
+    'rv_reconstruct_batched': (_I, [_P, _I, _I, _P, _I, _I, _I, _I, _P, _I, _P]),
     'rv_patch_pack': (_I, [_P, _I, _I, _I, _I, _I, _P, _I, _P]),
     'rv_match_argmax': (_I, [_P, _I, _P, _I, _I, _F, _P, _P, _I, _P]),
     'rv_gather_blocks': (_I, [_P, _I, _I, _I, _I, _P, _I, _I, _I, _P, _P]),
@@ -136,6 +142,7 @@ class CudaOps:
     fp32; flows (H, W, 2) fp32; confidence maps (H, W) fp32; index maps (H*W,) int32."""
 
     name = 'cuda'
+    batched = True      # conv2d and the propagation-step operators also take (n, ...) operands (network.py's batched windows)
 
     def __init__(self, device='cuda'):
         if not torch.cuda.is_available():
@@ -161,29 +168,39 @@ class CudaOps:
     # -- convolution ------------------------------------------------------------------------------
     def conv2d(self, layer, src0, src1, out, gate=None, res=None, act_pre=ACT_NONE, act_post=ACT_NONE,
                pixel_shuffle=False):
-        """`layer` is a packing.PackedConv.  Output geometry is checked by the caller (engine)."""
+        """`layer` is a packing.PackedConv.  Output geometry is checked by the caller (engine).  Operands are (H, W, C) maps, or
+        (n, H, W, C) for a batch of n images through one launch (every operand then has the batch dimension)."""
         _chk_dev(src0, src1, out, gate, res)
         d = rv_conv_desc()
+        if src0.dim() == 4:
+            ops = (src0, src1, gate, res, out)
+            assert all(t is None or (t.dim() == 4 and t.shape[0] == src0.shape[0]) for t in ops), \
+                f'{layer.name}: a batched conv needs (n, H, W, C) operands of one n'
+            d.n = src0.shape[0]
+            d.bs_src0, d.bs_out = src0.stride(0), out.stride(0)
+            d.bs_src1 = src1.stride(0) if src1 is not None else 0
+            d.bs_gate = gate.stride(0) if gate is not None else 0
+            d.bs_res = res.stride(0) if res is not None else 0
         d.src0 = src0.data_ptr()
         d.src1 = src1.data_ptr() if src1 is not None else None
-        d.c0 = src0.shape[2]
-        d.c1 = src1.shape[2] if src1 is not None else 0
+        d.c0 = src0.shape[-1]
+        d.c1 = src1.shape[-1] if src1 is not None else 0
         assert (d.c0, d.c1) == (layer.alloc0, layer.alloc1), \
             f'{layer.name}: source channels {(d.c0, d.c1)} != packed layout {(layer.alloc0, layer.alloc1)}'
         d.in_dtype = DTYPE_CODE[src0.dtype]
-        d.H, d.W = src0.shape[0], src0.shape[1]
+        d.H, d.W = src0.shape[-3], src0.shape[-2]
         d.wpack = layer.wpack.data_ptr()
         d.bias = layer.bias.data_ptr()
         d.cout = layer.cout
         d.kh, d.kw, d.stride, d.pad = layer.kh, layer.kw, layer.stride, layer.pad
         d.act_pre, d.act_post = act_pre, act_post
         d.gate = gate.data_ptr() if gate is not None else None
-        d.gate_cs = gate.shape[2] if gate is not None else 0
+        d.gate_cs = gate.shape[-1] if gate is not None else 0
         d.res = res.data_ptr() if res is not None else None
-        d.res_cs = res.shape[2] if res is not None else 0
+        d.res_cs = res.shape[-1] if res is not None else 0
         d.res_dtype = DTYPE_CODE[res.dtype] if res is not None else 0
         d.out = out.data_ptr()
-        d.out_cs = out.shape[2]
+        d.out_cs = out.shape[-1]
         d.out_dtype = DTYPE_CODE[out.dtype]
         d.pixel_shuffle = 1 if pixel_shuffle else 0
         d.impl = layer.impl
@@ -230,6 +247,8 @@ class CudaOps:
 
     def space_to_depth2(self, src, out):
         _chk_dev(src, out)
+        if src.dim() == 4:     # (n, H, W, C) with H even: the batch is one map of n*H rows
+            src, out = src.view(-1, src.shape[2], src.shape[3]), out.view(-1, out.shape[2], out.shape[3])
         _check(self.lib, self.lib.rv_space_to_depth2(_ptr(src), src.shape[0], src.shape[1], src.shape[2],
                                                      DTYPE_CODE[src.dtype], _ptr(out), self._stream()),
                'rv_space_to_depth2')
@@ -284,6 +303,13 @@ class CudaOps:
     # -- warp -------------------------------------------------------------------------------------
     def warp(self, src, flow, out, flow_up2=False):
         _chk_dev(src, flow, out)
+        if flow.dim() == 4:                        # a batch of n images: (n, ...) operands, one launch
+            n = flow.shape[0]
+            Hi, Wi, Cc = (src.shape[1], src.shape[2], 1) if src.dim() == 3 else src.shape[1:]
+            assert src.shape[0] == out.shape[0] == n
+            _check(self.lib, self.lib.rv_warp_batched(_ptr(src), Hi, Wi, Cc, DTYPE_CODE[src.dtype], _ptr(flow), flow.shape[1],
+                                                      flow.shape[2], int(flow_up2), _ptr(out), n, self._stream()), 'rv_warp')
+            return
         if src.dim() == 2:
             Hi, Wi, Cc = src.shape[0], src.shape[1], 1
         else:
@@ -294,11 +320,18 @@ class CudaOps:
     def warp3(self, feat, featUP, conf, flow, out_feat, out_featUP, out_conf):
         """the three warps of one propagation step in one launch (16-bit features)"""
         _chk_dev(feat, featUP, conf, flow, out_feat, out_featUP, out_conf)
-        h, w, Cc = feat.shape
-        assert tuple(featUP.shape) == (2 * h, 2 * w, Cc) and tuple(conf.shape) == (h, w) and tuple(flow.shape) == (h, w, 2)
+        n = flow.shape[0] if flow.dim() == 4 else 0   # a batch of n images: (n, ...) operands, one launch
+        h, w, Cc = feat.shape[-3:]
+        lead = (n,) if n else ()
+        assert tuple(featUP.shape) == lead + (2 * h, 2 * w, Cc) and tuple(conf.shape) == lead + (h, w)
+        assert tuple(flow.shape) == lead + (h, w, 2) and tuple(feat.shape) == lead + (h, w, Cc)
         assert feat.dtype == featUP.dtype == out_feat.dtype == out_featUP.dtype and conf.dtype == torch.float32
-        _check(self.lib, self.lib.rv_warp3(_ptr(feat), _ptr(featUP), _ptr(conf), _ptr(flow), h, w, Cc, DTYPE_CODE[feat.dtype],
-                                           _ptr(out_feat), _ptr(out_featUP), _ptr(out_conf), self._stream()), 'rv_warp3')
+        args = (_ptr(feat), _ptr(featUP), _ptr(conf), _ptr(flow), h, w, Cc, DTYPE_CODE[feat.dtype],
+                _ptr(out_feat), _ptr(out_featUP), _ptr(out_conf))
+        if n:
+            _check(self.lib, self.lib.rv_warp3_batched(*args, n, self._stream()), 'rv_warp3')
+        else:
+            _check(self.lib, self.lib.rv_warp3(*args, self._stream()), 'rv_warp3')
 
     # -- matching ---------------------------------------------------------------------------------
     def patch_pack(self, feat, out, mode):
@@ -336,6 +369,12 @@ class CudaOps:
     # -- confidence maps --------------------------------------------------------------------------
     def conf_pair(self, a, b, out, up2=False):
         _chk_dev(a, b, out)
+        if out.dim() == 4:                         # a batch of n images: (n, ...) operands, one launch
+            assert a.shape[0] == b.shape[0] == out.shape[0]
+            _check(self.lib, self.lib.rv_conf_pair_batched(_ptr(a), _ptr(b), a.shape[1], a.shape[2], int(up2), _ptr(out),
+                                                           out.shape[3], DTYPE_CODE[out.dtype], out.shape[0], self._stream()),
+                   'rv_conf_pair')
+            return
         _check(self.lib, self.lib.rv_conf_pair(_ptr(a), _ptr(b), a.shape[0], a.shape[1], int(up2), _ptr(out),
                                                out.shape[2], DTYPE_CODE[out.dtype], self._stream()), 'rv_conf_pair')
 
@@ -359,6 +398,12 @@ class CudaOps:
     # -- tail -------------------------------------------------------------------------------------
     def reconstruct(self, x, lr, scale, clamp01, out):
         _chk_dev(x, lr, out)
+        if lr.dim() == 4:                          # a batch of n images: (n, ...) operands, one launch
+            assert x.shape[0] == out.shape[0] == lr.shape[0]
+            _check(self.lib, self.lib.rv_reconstruct_batched(_ptr(x), x.shape[3], DTYPE_CODE[x.dtype], _ptr(lr), lr.shape[2],
+                                                             lr.shape[3], scale, int(clamp01), _ptr(out), lr.shape[0],
+                                                             self._stream()), 'rv_reconstruct')
+            return
         _check(self.lib, self.lib.rv_reconstruct(_ptr(x), x.shape[2], DTYPE_CODE[x.dtype], _ptr(lr), lr.shape[1],
                                                  lr.shape[2], scale, int(clamp01), _ptr(out), self._stream()),
                'rv_reconstruct')

@@ -112,6 +112,7 @@ class Network(nn.Module):
         if self.reuse_check not in ('sync', 'async', 'off'):
             raise ValueError("b200_reuse_check must be 'sync', 'async' or 'off'")
         self.reuse_fallbacks = 0      # calls that violated the sliding contract and were recomputed from scratch
+        self.batch_fallbacks = 0      # calls of n > 1 windows whose elements needed different schedules (run one by one)
         self.use_graphs = bool(_cget(config, 'b200_cuda_graphs', True))
         # residual blocks through the fused rv_resblock kernel (one launch per block) -> opt-in
         self.fuse_resblocks = bool(_cget(config, 'b200_fuse_resblocks', False))
@@ -143,6 +144,8 @@ class Network(nn.Module):
         self._bufs = {}
         self._device = torch.device('cpu')
         self._b = 0
+        self._bn = 1                  # windows of the current call: ring slots and carried state are [bn][...] tensors
+        self._bmode = False           # enqueueing the batched steps of a call: every scratch buffer has the batch dimension
         self.executed_kernels = 0     # kernels of librefvsr_b200.so actually executed (eager launches + graph nodes)
         self.register_load_state_dict_post_hook(lambda module, incompatible: module._invalidate())
 
@@ -198,7 +201,9 @@ class Network(nn.Module):
         self._packed[key] = pc
         return pc
 
-    def _buf(self, tag, shape, dtype):
+    def _buf(self, tag, shape, dtype, whole=False):
+        if self._bmode and not whole:
+            tag, shape = f'B{self._bn}.{tag}', (self._bn,) + tuple(shape)
         key = (tag, tuple(shape), dtype)
         b = self._bufs.get(key)
         if b is None or b.device != self._device:
@@ -206,17 +211,26 @@ class Network(nn.Module):
             self._bufs[key] = b
         return b
 
+    def _sbuf(self, kind, rest, shape, dtype):
+        """Per-stream state of batch element self._b: ring slots (kind 'ring') and the carried forward state (kind 'prev').  In a
+        call of n > 1 windows each buffer is ONE [n][...] tensor: the per-element products write their slice of it and the batched
+        steps (self._bmode) read and write it whole."""
+        if self._bn > 1:
+            full = self._buf(f'{kind}B{self._bn}.{rest}', (self._bn,) + tuple(shape), dtype, whole=True)
+            return full if self._bmode else full[self._b]
+        return self._buf(f'{kind}{self._b}.{rest}', shape, dtype)
+
     def _conv(self, name, src0, src1, out, srcs, act_pre=ACT_NONE, act_post=ACT_NONE, gate=None, res=None,
               pixel_shuffle=False, stride=1, pad=None, bias_add=0.0):
         k = self.get_submodule(name).weight.shape[2]
         if (stride == 2 and self.prefer_tc and self.act_dtype != torch.float32 and k in (3, 5)
-                and (pad is None or pad == k // 2) and src0.shape[0] % 2 == 0 and src0.shape[1] % 2 == 0):
+                and (pad is None or pad == k // 2) and src0.shape[-3] % 2 == 0 and src0.shape[-2] % 2 == 0):
             # stride-2 conv as a stride-1 3x3 conv over the space-to-depth input -> tensor-core kernel
-            z0 = self._buf(f's2d.{name}.0', (src0.shape[0] // 2, src0.shape[1] // 2, 4 * src0.shape[2]), src0.dtype)
+            z0 = self._buf(f's2d.{name}.0', (src0.shape[-3] // 2, src0.shape[-2] // 2, 4 * src0.shape[-1]), src0.dtype)
             self.ops.space_to_depth2(src0, z0)
             z1 = None
             if src1 is not None:
-                z1 = self._buf(f's2d.{name}.1', (src1.shape[0] // 2, src1.shape[1] // 2, 4 * src1.shape[2]), src1.dtype)
+                z1 = self._buf(f's2d.{name}.1', (src1.shape[-3] // 2, src1.shape[-2] // 2, 4 * src1.shape[-1]), src1.dtype)
                 self.ops.space_to_depth2(src1, z1)
             layer = self._layer(name, srcs, 1, 1, bias_add, s2d=True)
             self.ops.conv2d(layer, z0, z1, out, gate=gate, res=res, act_pre=act_pre, act_post=act_post,
@@ -233,7 +247,7 @@ class Network(nn.Module):
     def _resblock(self, conv1, conv2, x, out, tmp, act_mid, act_post=ACT_NONE):
         """out = act_post(x + conv2(act_mid(conv1(x)))): rv_resblock when the block qualifies
         (16-bit activations, C <= 64), otherwise two convolutions through the scratch buffer `tmp`."""
-        C = x.shape[2]
+        C = x.shape[-1]
         m1, m2 = self.get_submodule(conv1), self.get_submodule(conv2)
         if (self.fuse_resblocks and self.prefer_tc and hasattr(self.ops, 'resblock')
                 and packing.resblock_fusable(m1.weight, m2.weight, C, self.act_dtype)):
@@ -270,8 +284,7 @@ class Network(nn.Module):
 
     def _reslist(self, prefix, n, x, out, tag):
         """ResList (RefVSR_/common.py:64-82): n x [x + conv2(lrelu0.2(conv1(x)))], conv_tail, + input."""
-        C = x.shape[2]
-        H, W = x.shape[0], x.shape[1]
+        H, W, C = x.shape[-3:]
         t = self._buf(tag + '.t', (H, W, C), x.dtype)
         s = [self._buf(tag + '.s0', (H, W, C), x.dtype), self._buf(tag + '.s1', (H, W, C), x.dtype)]
         names = [f'{prefix}.RBs.{i}.conv{j}' for i in range(n) for j in (1, 2)] + [f'{prefix}.conv_tail']
@@ -297,7 +310,7 @@ class Network(nn.Module):
     def _prop_resblocks(self, prefix, lr8, feat, out, tag):
         """ResidualBlocksWithInputConv (RefVSR.py:327-360) on cat[lr, feat] (RefVSR.py:225-226,266-267)."""
         C = self.mid_channels
-        H, W = feat.shape[0], feat.shape[1]
+        H, W = feat.shape[-3], feat.shape[-2]
         nblk = self.config.num_blocks
         t = self._buf(tag + '.t', (H, W, C), feat.dtype)
         s = [self._buf(tag + '.s0', (H, W, C), feat.dtype), self._buf(tag + '.s1', (H, W, C), feat.dtype)]
@@ -330,7 +343,7 @@ class Network(nn.Module):
     def _pyramid(self, img, slot):
         """img (3,h,w) fp32 -> 6 normalised levels, coarsest first, each (H,W,3) fp32, in ring slot `slot`."""
         shapes = self._pyr_shapes(img.shape[1], img.shape[2])
-        lv = [self._buf(f'ring{self._b}.pyr{l}.{slot}', (H, W, 3), torch.float32) for l, (H, W) in enumerate(shapes)]
+        lv = [self._sbuf('ring', f'pyr{l}.{slot}', (H, W, 3), torch.float32) for l, (H, W) in enumerate(shapes)]
         self.ops.spynet_resize_norm(img, lv[5])
         for l in range(4, -1, -1):
             self.ops.avgpool2(lv[l + 1], lv[l])
@@ -476,13 +489,12 @@ class Network(nn.Module):
     def _frame_slot(self, slot, h, w):
         """ring buffers of one frame"""
         C, dt = self.mid_channels, self.act_dtype
-        r = f'ring{self._b}'
         f = self._match_step()
-        return {'conf': self._buf(f'{r}.conf.{slot}', (h, w), torch.float32),
-                'idx': self._buf(f'{r}.idx.{slot}', ((h // f) * (w // f),), torch.int32),
-                'aligned': self._buf(f'{r}.al.{slot}', (h, w, C), dt),
-                'aligned_up': self._buf(f'{r}.alup.{slot}', (2 * h, 2 * w, C), dt),
-                'lr8': self._buf(f'{r}.lr8.{slot}', (h, w, 8), dt)}
+        return {'conf': self._sbuf('ring', f'conf.{slot}', (h, w), torch.float32),
+                'idx': self._sbuf('ring', f'idx.{slot}', ((h // f) * (w // f),), torch.int32),
+                'aligned': self._sbuf('ring', f'al.{slot}', (h, w, C), dt),
+                'aligned_up': self._sbuf('ring', f'alup.{slot}', (2 * h, 2 * w, C), dt),
+                'lr8': self._sbuf('ring', f'lr8.{slot}', (h, w, 8), dt)}
 
     def _frame_alignment(self, lr, ref, slot):
         """Everything the RAP module needs from one (LR, Ref) frame pair, all pure functions of the frame
@@ -507,7 +519,7 @@ class Network(nn.Module):
     def _rap(self, fp, conf_prop, feat_prop, feat_prop_UP, tag):
         C, dt = self.mid_channels, self.act_dtype
         conf, aligned, aligned_up = fp['conf'], fp['aligned'], fp['aligned_up']
-        h, w = conf.shape
+        h, w = conf.shape[-2:]
         # scratch maps: one set per branch when the two branches may run concurrently (tag = 'bw.rap0' / 'fw.rap1' ...)
         sc = (tag.split('.')[0] + '.rap') if self.overlap_branches else 'rap'
         # level 1 (reference alignment already done per frame, see _frame_alignment)
@@ -545,7 +557,7 @@ class Network(nn.Module):
     # ---- upsampling tail (RefVSR.py:104-119,288,297) -------------------------------------------------
     def _compute_up(self, bw_up, fw_up, conf_bw, conf_fw, lr_center, clamp01):
         C, dt = self.mid_channels, self.act_dtype
-        H2, W2 = bw_up.shape[0], bw_up.shape[1]
+        H2, W2 = bw_up.shape[-3], bw_up.shape[-2]
         h, w = H2 // 2, W2 // 2
         cp8 = self._buf('up.cp8', (H2, W2, 8), dt)
         self.ops.conf_pair(conf_bw, conf_fw, cp8, up2=True)
@@ -618,7 +630,7 @@ class Network(nn.Module):
         return self._ring_mod or t
 
     def _ring(self, kind, a, t, shape, dtype=torch.float32):
-        return self._buf(f'ring{self._b}.{kind}.{a % self._rm(t)}', shape, dtype)
+        return self._sbuf('ring', f'{kind}.{a % self._rm(t)}', shape, dtype)
 
     def _run_products(self, work, t, h, w, hr, wr):
         """Pyramids first, then the flows and the per-frame alignment products, which are independent of each other.  With
@@ -626,8 +638,8 @@ class Network(nn.Module):
         side streams - alternating, each with its own scratch maps - and fill the SMs the matching / alignment kernels of the
         main stream leave idle; everything is joined before this returns.  Same kernels and inputs: bit-identical."""
         def flow(kind, a, sp):
-            pa = [self._buf(f'ring{self._b}.pyr{l}.{a % self._rm(t)}', (H, W, 3), torch.float32) for l, (H, W) in enumerate(self._pyr_shapes(h, w))]
-            pb = [self._buf(f'ring{self._b}.pyr{l}.{(a + 1) % self._rm(t)}', (H, W, 3), torch.float32) for l, (H, W) in enumerate(self._pyr_shapes(h, w))]
+            pa = [self._sbuf('ring', f'pyr{l}.{a % self._rm(t)}', (H, W, 3), torch.float32) for l, (H, W) in enumerate(self._pyr_shapes(h, w))]
+            pb = [self._sbuf('ring', f'pyr{l}.{(a + 1) % self._rm(t)}', (H, W, 3), torch.float32) for l, (H, W) in enumerate(self._pyr_shapes(h, w))]
             out = self._ring(kind, a, t, (h, w, 2))
             if kind == 'fw':
                 self._spynet(pb, pa, out, sp)      # Flow(frame a+1, frame a)
@@ -666,6 +678,11 @@ class Network(nn.Module):
     # forward (RefVSR.py:151-325)
     # ------------------------------------------------------------------------------------------
     def forward(self, lrs, refs, is_first_frame, is_log=False, is_train=False):
+        """lrs / refs (n, t, 3, h, w) / (n, t, 3, hr, wr) -> outs['result'] (n, 3, scale*h, scale*w).  n > 1 windows run as ONE
+        window schedule: the per-frame products (SPyNet, matching, alignment) once per element, every propagation step and the
+        upsampling tail once for the whole batch, in one CUDA graph, bit-identical to running each element alone.  Elements whose
+        schedules differ (e.g. the reuse guard finds that one did not slide) run one by one instead (`batch_fallbacks`), as do
+        is_log / is_train calls.  A stream keeps its batch size: a call with another n starts new streams (is_first_frame)."""
         outs = collections.OrderedDict()
         if is_log:
             outs['vis'] = collections.OrderedDict()
@@ -691,6 +708,10 @@ class Network(nn.Module):
             # trainers/trainer.py:159-172 would call loss.backward() on the result: fail here, with a clear message
             raise NotImplementedError('refvsr_b200 is inference only: forward(is_train=True) builds no autograd graph '
                                       '(call it under torch.no_grad() for a training-mode forward without gradients)')
+        if n != self._bn:
+            # the ring slots and carried state of a call of n windows are [n][...] tensors: another n starts new streams
+            self._state.clear()
+            self._bn = n
 
         caller_first = bool(is_first_frame)
         if not is_train:                                                     # RefVSR.py:168-170
@@ -699,12 +720,17 @@ class Network(nn.Module):
 
         with torch.no_grad():
             results, vis = [], None
-            for b in range(n):
-                res_b, vis_b = self._forward_one(b, lrs[b], refs[b], bool(is_first_frame), caller_first,
-                                                 bool(is_log), bool(is_train))
-                results.append(res_b)
-                vis = vis_b if vis is None else vis
-            out = torch.stack(results, 0)
+            if n > 1 and self._batchable(is_log, is_train):
+                fresh, shape = self._batch_fresh(lrs, refs, caller_first)
+                out = self._run_batch(fresh, [lrs[b] for b in range(n)], [refs[b] for b in range(n)], shape,
+                                      bool(is_first_frame))
+            else:
+                for b in range(n):
+                    res_b, vis_b = self._forward_one(b, lrs[b], refs[b], bool(is_first_frame), caller_first,
+                                                     bool(is_log), bool(is_train))
+                    results.append(res_b)
+                    vis = vis_b if vis is None else vis
+                out = torch.stack(results, 0)
 
         if not is_train:                                                     # RefVSR.py:292-297
             if is_first_frame:
@@ -717,13 +743,13 @@ class Network(nn.Module):
                 outs['eval_vis'] = vis['eval_vis']
         return outs
 
-    def push_frame(self, lr, ref, b=0):
-        """Streaming entry (SURVEY 8f row 2: a decoded-frame ring buffer feeding the per-frame pipeline): the window slides by one
-        and ONLY the entering frame is handed over - lr (3, h, w), ref (3, hr, wr) in [0, 1], the frame that would have been
-        lrs[b, t-1] / refs[b, t-1] of the next forward() call.  The other t-1 frames are the engine's own staged ring slots, so there
-        is nothing to verify (no reuse-guard launch, no host sync) and the caller moves 1/t of the window's bytes.  Returns the
-        same tensor forward()['result'][b] would: (3, scale*h, scale*w).  Needs a previous forward() call on this batch slot (the clip's first
-        window, is_first_frame=True); forced resets (reset_branch) follow the same counter as forward()."""
+    def _batchable(self, is_log, is_train):
+        """n > 1 windows can share one schedule: an operator set that takes (n, ...) operands, and none of the per-element-only
+        options (debug outputs, training mode, the opt-in fused residual-block / chain kernels)"""
+        return (getattr(self.ops, 'batched', False) and not is_log and not is_train and not self.use_chain
+                and not self.fuse_resblocks and self._ring_mod is None)
+
+    def _push_state(self, b, lr, ref):
         if lr.dim() != 3 or ref.dim() != 3 or lr.size(0) != 3 or ref.size(0) != 3:
             raise ValueError('push_frame takes one LR frame (3, h, w) and one Ref frame (3, hr, wr)')
         st = self._state.get(b)
@@ -732,6 +758,17 @@ class Network(nn.Module):
         t, h, w, hr, wr = st['shape']
         if tuple(lr.shape[1:]) != (h, w) or tuple(ref.shape[1:]) != (hr, wr) or lr.device != self._device:
             raise ValueError(f'push_frame: frame shapes / device differ from the running stream {(h, w)} / {(hr, wr)} on {self._device}')
+        return st
+
+    def push_frame(self, lr, ref, b=0):
+        """Streaming entry (SURVEY 8f row 2: a decoded-frame ring buffer feeding the per-frame pipeline): the window slides by one
+        and ONLY the entering frame is handed over - lr (3, h, w), ref (3, hr, wr) in [0, 1], the frame that would have been
+        lrs[b, t-1] / refs[b, t-1] of the next forward() call.  The other t-1 frames are the engine's own staged ring slots, so there
+        is nothing to verify (no reuse-guard launch, no host sync) and the caller moves 1/t of the window's bytes.  Returns the
+        same tensor forward()['result'][b] would: (3, scale*h, scale*w).  Needs a previous forward() call on this batch slot (the clip's first
+        window, is_first_frame=True); forced resets (reset_branch) follow the same counter as forward()."""
+        st = self._push_state(b, lr, ref)
+        t = st['shape'][0]
         is_first_frame = self.max_frame_itr_num is not None and self.frame_itr_num == self.max_frame_itr_num   # RefVSR.py:168-170
         self._b = b
         win_lr, win_ref = _NewestOnly(lr, t), _NewestOnly(ref, t)
@@ -742,10 +779,38 @@ class Network(nn.Module):
         self.frame_itr_num += 1
         return out
 
-    def _forward_one(self, b, lrs, refs, is_first_frame, caller_first, is_log, is_train):
+    def push_frames(self, lrs, refs):
+        """push_frame for all n windows of the running batch at once: lrs (n, 3, h, w), refs (n, 3, hr, wr), element b being
+        the frame entering window b.  The same contract per element as push_frame; returns what forward()['result'] would,
+        (n, 3, scale*h, scale*w), computed by one batched window schedule like forward()."""
+        if lrs.dim() != 4 or refs.dim() != 4 or lrs.size(0) != refs.size(0):
+            raise ValueError('push_frames takes LR frames (n, 3, h, w) and Ref frames (n, 3, hr, wr)')
+        n = lrs.size(0)
+        if n != self._bn:
+            raise ValueError(f'push_frames: {n} frames for a stream of {self._bn} windows')
+        sts = [self._push_state(b, lrs[b], refs[b]) for b in range(n)]
+        shape = sts[0]['shape']
+        t = shape[0]
+        is_first_frame = self.max_frame_itr_num is not None and self.frame_itr_num == self.max_frame_itr_num   # RefVSR.py:168-170
+        with torch.no_grad():
+            wl, wr = [_NewestOnly(lrs[b], t) for b in range(n)], [_NewestOnly(refs[b], t) for b in range(n)]
+            if n > 1 and self._batchable(False, False):
+                out = self._run_batch([False] * n, wl, wr, shape, bool(is_first_frame))
+            else:
+                outs = []
+                for b in range(n):
+                    self._b = b
+                    outs.append(self._do_window(b, sts[b], False, wl[b], wr[b], shape, bool(is_first_frame), False, False)[0])
+                out = torch.stack(outs, 0)
+        if is_first_frame:                                                   # RefVSR.py:292-297
+            self.frame_itr_num = 0
+        self.frame_itr_num += 1
+        return out
+
+    def _is_fresh(self, b, lrs, refs, caller_first, is_train):
+        """(state, fresh, shape) of batch element b's stream: fresh = its cached per-frame products cannot be reused"""
         t, _, h, w = lrs.shape
         hr, wr = refs.shape[2], refs.shape[3]
-        mid = t // 2
         self._b = b           # ring / state namespace of this batch element
 
         # stream bookkeeping for exact reuse: a caller-declared first frame starts a new stream; forced
@@ -755,13 +820,43 @@ class Network(nn.Module):
         fresh = (st is None or caller_first or not self.reuse or is_train or st.get('shape') != shape)
         if not fresh and self.reuse_check != 'off':
             fresh = not self._window_slid_by_one(st, lrs, refs, t, h, w, hr, wr)
+        return st, fresh, shape
+
+    def _batch_fresh(self, lrs, refs, caller_first):
+        """_is_fresh for the n elements of a batched call; with b200_reuse_check='sync' the n reuse-guard verdicts are read back
+        in ONE device-to-host copy (one host sync per call, not per element).  -> ([fresh per element], shape)"""
+        n, t, _, h, w = lrs.shape
+        hr, wr = refs.shape[3], refs.shape[4]
+        shape = (t, h, w, hr, wr)
+        fresh, pending = [], []
+        for b in range(n):
+            if self.reuse_check != 'sync':
+                fresh.append(self._is_fresh(b, lrs[b], refs[b], caller_first, False)[1])
+                continue
+            self._b = b
+            st = self._state.get(b)
+            f = st is None or caller_first or not self.reuse or st.get('shape') != shape
+            if not f:
+                pending.append((b, self._enqueue_overlap_compare(st, lrs[b], refs[b], t, h, w, hr, wr)))
+            fresh.append(f)
+        if pending:
+            for (b, _), differs in zip(pending, torch.cat([flag for _, flag in pending]).tolist()):
+                if differs:                   # the staged frames of the previous call are the reference
+                    self.reuse_fallbacks += 1
+                    fresh[b] = True
+        return fresh, shape
+
+    def _forward_one(self, b, lrs, refs, is_first_frame, caller_first, is_log, is_train):
+        st, fresh, shape = self._is_fresh(b, lrs, refs, caller_first, is_train)
         return self._do_window(b, st, fresh, lrs, refs, shape, is_first_frame, is_log, is_train)
 
-    def _do_window(self, b, st, fresh, lrs, refs, shape, is_first_frame, is_log, is_train):
+    def _prepare_window(self, b, st, fresh, lrs, refs, shape, is_first_frame, is_train, a0_fresh=0):
+        """Bookkeeping of element b's next window: stream position, staging of the entering frames, product work list.
+        A fresh stream starts at position a0_fresh (any value: only a % t addresses the ring)."""
         t, h, w, hr, wr = shape
         mid = t // 2
         if fresh:
-            st = {'a0': 0, 'pyr': set(), 'fw': set(), 'bw': set(), 'frame': set(), 'staged': set(),
+            st = {'a0': a0_fresh, 'pyr': set(), 'fw': set(), 'bw': set(), 'frame': set(), 'staged': set(),
                   'has_prev': bool(st and st.get('has_prev')) and st.get('shape') == shape, 'shape': shape}
             self._state[b] = st
         else:
@@ -785,31 +880,97 @@ class Network(nn.Module):
                 st['staged'].add(a0 + j)
 
         work = self._plan_products(st, a0, t, range_start)
-        variant = 'first' if is_first_frame else 'steady'
-        args = (b, st, a0, t, h, w, hr, wr, work, is_first_frame, range_start, is_log, is_train)
-        use_graph = (self.use_graphs and not fresh and not is_log and not is_train and lrs.is_cuda
-                     and hasattr(torch.cuda, 'CUDAGraph'))
-        if use_graph:
-            key = (b, shape, a0 % t, variant, tuple((k, a - a0) for k, a in work))
-            entry = self._graphs.get(key)
-            if entry is None:
-                torch.cuda.synchronize()
-                graph = torch.cuda.CUDAGraph()
-                n0 = self.ops.launch_count()
-                with torch.cuda.graph(graph):
-                    out_static, _ = self._run_window(*args)
-                entry = (graph, out_static, self.ops.launch_count() - n0)
-                self._graphs[key] = entry
-            entry[0].replay()
-            self.executed_kernels += entry[2]          # kernel nodes of librefvsr_b200.so replayed by the graph
-            out, vis = entry[1].clone(), None
-        else:
+        return st, a0, range_start, work
+
+    def _execute(self, key, fn):
+        """fn() enqueues one window and returns (static output, vis).  key None: run eagerly; otherwise the window is captured
+        into a CUDA graph once per key and replayed."""
+        if key is None:
             n0 = self.ops.launch_count()
-            out_static, vis = self._run_window(*args)
+            out_static, vis = fn()
             self.executed_kernels += self.ops.launch_count() - n0
-            out = out_static.clone()
+            return out_static.clone(), vis
+        entry = self._graphs.get(key)
+        if entry is None:
+            torch.cuda.synchronize()
+            graph = torch.cuda.CUDAGraph()
+            n0 = self.ops.launch_count()
+            with torch.cuda.graph(graph):
+                out_static, _ = fn()
+            entry = (graph, out_static, self.ops.launch_count() - n0)
+            self._graphs[key] = entry
+        entry[0].replay()
+        self.executed_kernels += entry[2]          # kernel nodes of librefvsr_b200.so replayed by the graph
+        return entry[1].clone(), None
+
+    def _graph_ok(self, fresh, is_log, is_train, lrs):
+        return (self.use_graphs and not fresh and not is_log and not is_train and lrs.is_cuda
+                and hasattr(torch.cuda, 'CUDAGraph'))
+
+    def _do_window(self, b, st, fresh, lrs, refs, shape, is_first_frame, is_log, is_train):
+        t, h, w, hr, wr = shape
+        st, a0, range_start, work = self._prepare_window(b, st, fresh, lrs, refs, shape, is_first_frame, is_train)
+        variant = 'first' if is_first_frame else 'steady'
+        key = None
+        if self._graph_ok(fresh, is_log, is_train, lrs):
+            key = (b, self._bn, shape, a0 % t, variant, tuple((k, a - a0) for k, a in work))
+        out, vis = self._execute(key, lambda: self._run_window(b, st, a0, t, h, w, hr, wr, work, is_first_frame, range_start,
+                                                                is_log, is_train))
         st['has_prev'] = True
         return out, vis
+
+    def _run_batch(self, fresh, lrs, refs, shape, is_first_frame):
+        """One window for each of the n elements (lrs[b] / refs[b]: element b's window frames).  When every element has the same
+        schedule (same ring phase, product work and fresh decision) the products are enqueued per element and every step once
+        for the batch; otherwise each element runs alone.  -> (n, 3, scale*h, scale*w)"""
+        n = len(fresh)
+        t, h, w, hr, wr = shape
+        # a stream that starts afresh takes the ring phase of the batch's sliding streams, so that their next windows line up
+        slid = [self._state[b]['a0'] + 1 for b in range(n) if not fresh[b]]
+        preps = []
+        for b in range(n):
+            self._b = b
+            preps.append(self._prepare_window(b, self._state.get(b), fresh[b], lrs[b], refs[b], shape, is_first_frame, False,
+                                              slid[0] if slid else 0))
+        sigs = {(a0 % t, rs, tuple((k, a - a0) for k, a in work)) for _, a0, rs, work in preps}
+        variant = 'first' if is_first_frame else 'steady'
+        if len(sigs) > 1 or len(set(fresh)) > 1:
+            self.batch_fallbacks += 1
+            outs = []
+            for b, (st, a0, rs, work) in enumerate(preps):
+                self._b = b
+                key = None
+                if self._graph_ok(fresh[b], False, False, lrs[b]):
+                    key = (b, self._bn, shape, a0 % t, variant, tuple((k, a - a0) for k, a in work))
+                outs.append(self._execute(key, lambda: self._run_window(b, st, a0, t, h, w, hr, wr, work, is_first_frame, rs,
+                                                                         False, False))[0])
+                st['has_prev'] = True
+            return torch.stack(outs, 0)
+
+        st0, a0, range_start, work = preps[0]
+
+        def products():
+            # per element: SPyNet, matching and the alignment products (each writes its slice of the ring)
+            self._bmode = False
+            try:
+                for b, p in enumerate(preps):
+                    self._b = b
+                    self._run_products(p[3], t, h, w, hr, wr)
+            finally:
+                self._bmode = True
+
+        key = None
+        if self._graph_ok(fresh[0], False, False, lrs[0]):
+            key = ('batch', n, shape, a0 % t, variant, tuple((k, a - a0) for k, a in work))
+        self._bmode = True
+        try:
+            out, _ = self._execute(key, lambda: self._run_window(0, st0, a0, t, h, w, hr, wr, work, is_first_frame, range_start,
+                                                                  False, False, products=products))
+        finally:
+            self._bmode = False
+        for st, *_ in preps:
+            st['has_prev'] = True
+        return out
 
     def _enqueue_overlap_compare(self, st, lrs, refs, t, h, w, hr, wr):
         """Reuse guard, device side: frames 0..t-2 of this call must be frames 1..t-1 of the previous one, i.e. equal to the
@@ -914,19 +1075,23 @@ class Network(nn.Module):
         agg = self._prop_resblocks('forward_resblocks', fp['lr8'], feat_prop, self._buf('fw.agg', (h, w, C), dt), 'fw.rb')
         return self._rap(fp, conf_prop, agg, feat_prop_UP, f'fw.rap{tagi % 2}')
 
-    def _run_window(self, b, st, a0, t, h, w, hr, wr, work, is_first_frame, range_start, is_log, is_train):
-        """All kernel launches of one window.  Reads / writes static buffers only (graph-capturable)."""
+    def _run_window(self, b, st, a0, t, h, w, hr, wr, work, is_first_frame, range_start, is_log, is_train, products=None):
+        """All kernel launches of one window.  Reads / writes static buffers only (graph-capturable).  products: enqueues the
+        per-frame products (default: this element's work list); in a batched window it runs them for every element."""
         C, dt = self.mid_channels, self.act_dtype
         mid = t // 2
         vis = {'vis': collections.OrderedDict()} if is_log else None
+        if products is None:
+            def products():
+                self._run_products(work, t, h, w, hr, wr)
 
         def lr32(i):
             return self._ring('lr32', a0 + i, t, (3, h, w))
 
         if is_first_frame:
             range_start = 0
-        prev = {'feat': self._buf(f'prev{b}.feat', (h, w, C), dt), 'featUP': self._buf(f'prev{b}.featUP', (2 * h, 2 * w, C), dt),
-                'conf': self._buf(f'prev{b}.conf', (h, w), torch.float32), 'flow': self._buf(f'prev{b}.flow', (h, w, 2), torch.float32)}
+        prev = {'feat': self._sbuf('prev', 'feat', (h, w, C), dt), 'featUP': self._sbuf('prev', 'featUP', (2 * h, 2 * w, C), dt),
+                'conf': self._sbuf('prev', 'conf', (h, w), torch.float32), 'flow': self._sbuf('prev', 'flow', (h, w, 2), torch.float32)}
 
         def carry_flow(i):
             if (a0 + i) in st['fw']:
@@ -974,7 +1139,7 @@ class Network(nn.Module):
                 with torch.cuda.stream(side):
                     feat_prop_UP, conf_prop = forward_branch(copy_flow=False)
                 ops.set_conv_cta_cap(self.overlap_main_cap)
-                self._run_products(work, t, h, w, hr, wr)
+                products()
 
                 def after_step(k):
                     if k + 1 == self.overlap_bw_steps:
@@ -987,7 +1152,7 @@ class Network(nn.Module):
                 main.wait_stream(side)                               # join
             carry_flow(mid)
         else:
-            self._run_products(work, t, h, w, hr, wr)
+            products()
             # ---------------- backward branch (RefVSR.py:211-238) ----------------
             backward_feat_UP, conf_bw = self._backward_branch(a0, t, h, w, vis)
             # (the forward branch writes 'fw.*' buffers only, so these stay intact)
@@ -1022,6 +1187,7 @@ class Network(nn.Module):
                              'frame 0, i.e. a pure pipeline - run replicas over different clips instead')
         self._device = frames_lr.device
         self._b = 0
+        self._bn = 1
         self._ring_mod = (own[1] - own[0]) + t - 1
         self._shard = {'pyr': set(), 'fw': set(), 'bw': set(), 'frame': set(), 'staged': set(), 'geom': (t, h, w, hr, wr),
                        'g0': g0, 'n': num_frames, 'own': tuple(own), 'lr': frames_lr, 'ref': frames_ref, 'fw_out': {}}

@@ -57,3 +57,8 @@ class SRNet(nn.Module):
         """streaming twin of forward() for callers that keep their own decoded-frame ring: after the clip's first window, hand
         over only the entering (LR, Ref) frame -> (3, scale*h, scale*w); see Network.push_frame (no counterpart in the reference)"""
         return self.Network.push_frame(lr, ref)
+
+    def push_frames(self, lrs, refs):
+        """push_frame for a batch of n streams: the entering frames (n, 3, h, w) / (n, 3, hr, wr) -> (n, 3, scale*h, scale*w), one
+        batched window schedule; see Network.push_frames"""
+        return self.Network.push_frames(lrs, refs)
