@@ -119,9 +119,14 @@ int rv_set_conv_cta_cap(int cap);
  * opt-in limit.  Returns the previous value.  A smaller bound takes the plan branches of a device with less shared memory (fewer
  * ring slots, no TMA output buffer), so that each can be run and compared on one device. */
 int rv_set_conv_smem_cap(int bytes);
+/* 2: the following rv_conv2d (tensor-core) launches run every conv on the two-consumer kernel; 0 (or any other value)
+ * restores the plan's choice, which runs the single-source 48 -> 48 3x3 convs (plain or with a residual) on three consumer
+ * warpgroups when their buffers fit.  Returns the previous value.  Lets the two kernels be compared on one device. */
+int rv_set_conv_consumers(int n);
 
 /* Host-only: the launch plan rv_conv2d's tensor-core path would use on a device with `max_smem_optin` bytes of opt-in shared memory
- * per block and `num_sms` SMs -> out8 = {mode, smem slots per consumer, weights resident, stages per tile, consumer
+ * per block and `num_sms` SMs, with the two-consumer kernel (rv_set_conv_consumers(2); rv_conv2d_tc_consumers gives the plan
+ * of a three-consumer launch) -> out8 = {mode, smem slots per consumer, weights resident, stages per tile, consumer
  * warpgroups, accumulator sets, nb, dynamic smem bytes}.  No CUDA call is made (pointers in `d` are only tested for null / alignment).  Lets the
  * ring invariants (every issuing warp owns its slots and accumulators) be checked without a GPU. */
 int rv_conv2d_tc_plan(const rv_conv_desc* d, int max_smem_optin, int num_sms, int32_t* out8);
@@ -132,6 +137,9 @@ int rv_conv2d_tc_epi_depth(const rv_conv_desc* d, int max_smem_optin, int num_sm
  * in shared memory, 2 TMA boxes of pixel-shuffled HR rows staged in shared memory (ps_order 1), 3 pixel-shuffled HR rows as
  * 16-byte stores from registers (ps_order 1, when the staging buffers do not fit). */
 int rv_conv2d_tc_out_store(const rv_conv_desc* d, int max_smem_optin, int num_sms, int32_t* kind);
+/* Host-only: the plan a launch takes under the current rv_set_conv_consumers setting -> out4 = {consumer warpgroups (2 or 3),
+ * smem slots per consumer, gate / residual TMA buffers per consumer (0: none), dynamic smem bytes}. */
+int rv_conv2d_tc_consumers(const rv_conv_desc* d, int max_smem_optin, int num_sms, int32_t* out4);
 
 /* ------------------------------------------------------------------------------------------------
  * rv_resblock - residual block  out = act_post( x + conv2( act_mid( conv1(x) ) ) ), 3x3 / stride 1 / pad 1,

@@ -25,6 +25,8 @@ int conv2d_tc_epi_depth(const rv_conv_desc* d, int max_smem, int num_sms, int* d
 int conv2d_tc_out_store(const rv_conv_desc* d, int max_smem, int num_sms, int* kind);
 int set_conv_cta_cap(int cap);
 int set_conv_smem_cap(int bytes);
+int set_conv_consumers(int n);
+int conv2d_tc_consumers(const rv_conv_desc* d, int max_smem, int num_sms, int* out);
 
 }  // namespace rv
 
@@ -72,6 +74,7 @@ extern "C" int rv_conv2d(const rv_conv_desc* d, void* stream) {
 
 extern "C" int rv_set_conv_cta_cap(int cap) { return rv::set_conv_cta_cap(cap); }
 extern "C" int rv_set_conv_smem_cap(int bytes) { return rv::set_conv_smem_cap(bytes); }
+extern "C" int rv_set_conv_consumers(int n) { return rv::set_conv_consumers(n); }
 
 extern "C" int rv_conv2d_tc_plan(const rv_conv_desc* d, int max_smem_optin, int num_sms, int32_t* out8) {
   RV_REQUIRE(d != nullptr && out8 != nullptr && max_smem_optin > 0 && num_sms > 0, "rv_conv2d_tc_plan: bad arguments");
@@ -89,4 +92,10 @@ extern "C" int rv_conv2d_tc_out_store(const rv_conv_desc* d, int max_smem_optin,
   RV_REQUIRE(d != nullptr && kind != nullptr && max_smem_optin > 0 && num_sms > 0, "rv_conv2d_tc_out_store: bad arguments");
   if (const int rc = check_batch(d)) return rc;
   return rv::conv2d_tc_out_store(d, max_smem_optin, num_sms, kind);
+}
+
+extern "C" int rv_conv2d_tc_consumers(const rv_conv_desc* d, int max_smem_optin, int num_sms, int32_t* out4) {
+  RV_REQUIRE(d != nullptr && out4 != nullptr && max_smem_optin > 0 && num_sms > 0, "rv_conv2d_tc_consumers: bad arguments");
+  if (const int rc = check_batch(d)) return rc;
+  return rv::conv2d_tc_consumers(d, max_smem_optin, num_sms, out4);
 }

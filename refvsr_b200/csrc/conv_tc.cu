@@ -17,13 +17,19 @@
 // the HR tail) at NB 16 / 48 / 96 run a kernel whose tap and K-step loops are unrolled at compile time (p.fixed): a stage
 // is then one fence, 54 wgmmas with no branch between them and one commit, where the runtime loop makes ptxas fence and
 // wait on every wgmma.  Other shapes (8 + 48 channels, 7 x 7) keep the runtime loop; both issue the same MMAs in the same order.
-// Warp roles (384 threads): warpgroup 0 = TMA producers, warpgroups 1 and 2 = consumers.  Consumer c owns the CTA's local
-// tiles c, c + 2, ... and its own ring of shared-memory slots, so one consumer's MMAs overlap the other's epilogue
-// (bias / act / gate / residual / act / NHWC or pixel-shuffled store straight from the accumulator registers).  Producer
-// warp c fills consumer c's ring only and warp 2 + c its gate / residual buffers only, each with its own slot and phase
-// state, so a consumer that is slow to free a slot never holds back the other consumer's fills.  In the compile-time
-// kernels the two A warps still issue their first ring fills alternately (a start-up hand-off through bar_fill), as the
-// single producer before them did, so that consumer 1's first box does not queue behind all of consumer 0's.
+// Warp roles (128 (1 + NCONS) threads): warpgroup 0 = TMA producers, warpgroups 1 .. NCONS = consumers.  Consumer c owns the
+// CTA's local tiles c, c + NCONS, ... and its own ring of shared-memory slots, so one consumer's MMAs overlap the others'
+// epilogues (bias / act / gate / residual / act / NHWC or pixel-shuffled store straight from the accumulator registers).
+// Producer warp c fills consumer c's ring only, each with its own slot and phase state, so a consumer that is slow to free a
+// slot never holds back another consumer's fills.  The gate / residual buffers are filled by warp 2 + c for consumer c
+// with two consumers, and by warp 3 for all three, in tile order, with three.  In the compile-time kernels the A warps
+// still issue their first ring fills round-robin (a start-up hand-off through bar_fill), as the single producer before them
+// did, so that consumer 1's first box does not queue behind all of consumer 0's.
+// NCONS is 2 everywhere but in the single-source 48 -> 48 3 x 3 kernel (conv_tc3_kernel: the trunk convs and conv_hr,
+// plain or with a residual), whose epilogue (about 2 000 - 2 600 cycles, latency-bound) is longer than its 54-wgmma batch
+// (about 1 750): with two consumers taking turns a tile costs about MMA + epilogue, with three each batch covers the other
+// two consumers' epilogues.  Its 512 threads get 128 registers each, so its epilogue reads the gate / residual values from
+// their TMA buffer where they are used instead of copying them to registers first.
 // Up to NB = 48 the epilogue never waits on a global load of the gate / residual: with 16-bit, 16-byte aligned operands
 // they arrive as TMA boxes in a ring of epi_depth per-consumer shared-memory buffers (plan_tc counts them, shrinking the
 // A ring), issued by warp 2 + c as soon as a buffer is free; otherwise each thread loads them into registers before
@@ -50,7 +56,6 @@
 namespace rv {
 
 static constexpr int TH = 8, TW = 16;
-static constexpr int NCONS = 2;      // consumer warpgroups
 static constexpr int MAX_SLOTS = 6;  // ring slots per consumer
 static constexpr int MAX_EPI = 2;    // gate / residual buffers per consumer
 static constexpr int MAX_NB = 96;
@@ -82,6 +87,7 @@ struct TcP {
   int ps_vec;                    // pixel shuffle in that order: HR rows as 16-byte vectors or TMA boxes (PSV kernel)
   int out_tma;                   // the output tile is staged in a per-consumer shared-memory buffer and written by TMA
   uint32_t out_off, out_bytes;   // byte offset of those buffers from the ring / bytes of one
+  int ncons;                     // consumer warpgroups (3: conv_tc3_kernel, see plan_tc)
   // Batch (rv_conv_desc::n): the persistent loop runs over nimg x tiles_x x tiles_y tiles, image-major.  With nimg > 1 every
   // tensor map has the image as its last dimension, so a box never reaches into a neighbouring image (TMA's out-of-bounds fill
   // is each image's own zero padding); per-thread loads and stores step by these element strides.  nimg = 1 keeps the 3-D maps.
@@ -102,7 +108,8 @@ __host__ __device__ constexpr bool fixed_nb(int nb) { return nb == 16 || nb == 4
 // Timeline instrumentation, compiled only with -DRV_CONV_TIMELINE into a separate library (tools/conv_timeline.py); the
 // product library has none of it.  Lane 0 of each role writes clock64 stamps of consumer c's i-th local tile:
 // tl[cta][role][i][event], cta = blockIdx.y * gridDim.x + blockIdx.x, role c = the producer warps of consumer c (A warp
-// events 0-2, gate / residual warp events 3-5), role NCONS + c = consumer c.
+// events 0-2, gate / residual warp events 3-5), role TL_MAX_CONS + c = consumer c (a two-consumer kernel leaves roles 2 and 5
+// empty).
 //   producer: 0 empty-slot wait start, 1 wait end, 2 A box (all stages of the tile) issued,
 //             3 empty epilogue-buffer wait start, 4 wait end, 5 gate / residual boxes issued
 //   consumer: 0 full-slot wait start, 1 full-slot wait end, 2 turn wait end, 3 first wgmma issued,
@@ -114,7 +121,7 @@ __host__ __device__ constexpr bool fixed_nb(int nb) { return nb == 16 || nb == 4
 // with an epilogue that touches no shared memory (TMA-store epilogue only: the gate / residual buffers are waited for and
 // released but not read, the values are folded into a register instead of the staging buffer, no TMA store).
 #ifdef RV_CONV_TIMELINE
-static constexpr int TL_TILES = 128, TL_EV = 10, TL_ROLES = 2 * NCONS;
+static constexpr int TL_TILES = 128, TL_EV = 10, TL_MAX_CONS = 3, TL_ROLES = 2 * TL_MAX_CONS;
 __device__ long long* g_tl;
 __device__ int g_tl_diag;
 static int g_tl_max_slots = 0;   // host: ring slots per consumer at most (0: the plan's)
@@ -249,11 +256,12 @@ __device__ __forceinline__ uint32_t pack2(float a, float b) {
 // NB: output channels per CTA (= p.NB); KS, KST: compile-time taps and K-steps of MODE 1 (0: the runtime loop, p.fixed = 0);
 // PSV: the 16-byte pixel-shuffle epilogue (p.ps_vec), which has no gate / residual
 // BATCH: p.nimg > 1 (a separate instantiation, so that one image keeps its single-image tile loop and addressing)
-template <typename TI, typename TR, typename TO, bool BATCH, int MODE, int NB, int KS, int KST, bool PSV>
-__global__ void __launch_bounds__(128 * (1 + NCONS), 1)
-conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1,
-               const __grid_constant__ CUtensorMap tmg, const __grid_constant__ CUtensorMap tmr,
-               const __grid_constant__ CUtensorMap tmo, const TcP p) {
+// NCONS: consumer warpgroups (2, or 3 in conv_tc3_kernel)
+template <int NCONS, typename TI, typename TR, typename TO, bool BATCH, int MODE, int NB, int KS, int KST, bool PSV>
+__device__ __forceinline__ void conv_tc_body(const CUtensorMap& tm0, const CUtensorMap& tm1, const CUtensorMap& tmg,
+                                             const CUtensorMap& tmr, const CUtensorMap& tmo, const TcP& p) {
+  static_assert(NCONS == 2 || (NCONS == 3 && MODE == 1 && NB == 48 && KS > 0 && !PSV && sizeof(TR) == 2 && sizeof(TO) == 2),
+                "three consumers: the compile-time 48-channel kernel with 16-bit operands only");
   constexpr bool BF = std::is_same<TI, __nv_bfloat16>::value;
   extern __shared__ uint8_t smem_raw[];
   __shared__ uint64_t bar_full[NCONS][MAX_SLOTS], bar_empty[NCONS][MAX_SLOTS], bar_w, bar_turn[NCONS];
@@ -289,8 +297,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
         tc::mbar_init(&bar_efull[c][i], 1);
         tc::mbar_init(&bar_eempty[c][i], 1);   // released by one consumer thread after a named barrier
       }
-    for (int c = 0; c < NCONS; ++c) tc::mbar_init(&bar_turn[c], 4);   // one arrival per warp of the other consumer
-    for (int c = 0; c < NCONS; ++c) tc::mbar_init(&bar_fill[c], 1);   // the other A producer warp's start-up hand-off
+    for (int c = 0; c < NCONS; ++c) tc::mbar_init(&bar_turn[c], 4);   // one arrival per warp of the previous consumer
+    for (int c = 0; c < NCONS; ++c) tc::mbar_init(&bar_fill[c], 1);   // the previous A producer warp's start-up hand-off
     tc::fence_barrier_init();
     tc::prefetch_tmap(&tm0);
     if (p.nch1 || p.nq1) tc::prefetch_tmap(&tm1);
@@ -321,7 +329,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
 
   if (warp_u < 4) {
     // ============================ TMA producers ============================
-    // warp c < NCONS: consumer c's A boxes (and streamed weights); warp NCONS + c: consumer c's gate / residual boxes
+    // warp c < NCONS: consumer c's A boxes (and streamed weights); the other warps: the gate / residual boxes, warp 2 + c
+    // those of consumer c with two consumers, warp 3 those of all three with three
     const int pc = warp_u % NCONS;
     const uint8_t* wsrc = p.wpack + (size_t)nblk * p.S * p.w_bytes;
     if (warp_u == 0 && p.resident && tc::elect_one()) {
@@ -339,17 +348,21 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
         tc::prefetch_tmap(&tmg);
         tc::prefetch_tmap(&tmr);
       }
-      int buf = 0, it = 0;
-      uint32_t eph = 0;
-      for (int tile = blockIdx.x + pc * gridDim.x; tile < ntiles; tile += NCONS * gridDim.x, ++it) {
+      // local tile l is consumer l % NCONS's (l / NCONS)-th; with three consumers the turns make them consume in local
+      // tile order, so one in-order issuer never waits on a buffer behind a later tile's
+      constexpr int LSTEP = NCONS == 2 ? 2 : 1;
+      for (int l = NCONS == 2 ? pc : 0, tile = blockIdx.x + l * gridDim.x; tile < ntiles; l += LSTEP, tile += LSTEP * gridDim.x) {
+        const int c = l % NCONS, it = l / NCONS;
+        const int buf = it & (p.epi_depth - 1);                           // epi_depth 1 or 2
+        const uint32_t eph = (uint32_t)(it >> (p.epi_depth - 1)) & 1u;
         const int img = BATCH ? tile / tiles_img : 0, ti = BATCH ? tile - img * tiles_img : tile;
         const int ty = ti / p.tiles_x, tx = ti - ty * p.tiles_x;
-        RV_TL(tl0, pc, it, 3);
-        tc::mbar_wait(&bar_eempty[pc][buf], eph ^ 1u);
-        RV_TL(tl0, pc, it, 4);
+        RV_TL(tl0, c, it, 3);
+        tc::mbar_wait(&bar_eempty[c][buf], eph ^ 1u);
+        RV_TL(tl0, c, it, 4);
         if (tc::elect_one()) {
-          uint64_t* bar = &bar_efull[pc][buf];
-          uint8_t* g = epi_buf(pc, buf);
+          uint64_t* bar = &bar_efull[c][buf];
+          uint8_t* g = epi_buf(c, buf);
           tc::mbar_expect_tx(bar, p.epi_tx);
           if (batched) {
             if (gate_p != nullptr) tc::tma_load_4d(&tmg, bar, g, nblk * NB, tx * p.tw, ty * p.th, img);
@@ -360,27 +373,30 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
           }
         }
         __syncwarp();
-        RV_TL(tl0, pc, it, 5);
-        if (++buf == p.epi_depth) { buf = 0; eph ^= 1u; }
+        RV_TL(tl0, c, it, 5);
       }
       return;
     }
     const uint32_t tx_bytes = p.a_tx + (p.resident ? 0u : p.w_bytes);
-    // Start-up hand-off (compile-time kernels): the two A warps issue the tiles of their first ring fill alternately
-    // (consumer 0's tile 0, consumer 1's tile 0, consumer 0's tile 1, ...), so that consumer 1's first box does not queue
-    // behind consumer 0's whole fill.  Tile it of warp 1 follows tile it of warp 0, tile it of warp 0 follows tile it - 1 of
-    // warp 1; after the first `lead` tiles (at most two) each waits on its own consumer's slots only.  The runtime-loop
-    // kernels (7 x 7, 1 x 1, 64-channel chunks) measured slower with it and keep independent fills.
+    // Start-up hand-off (compile-time kernels): the A warps issue the tiles of their first ring fill round-robin
+    // (consumer 0's tile 0, consumer 1's tile 0, ..., consumer 0's tile 1, ...), so that consumer 1's first box does not
+    // queue behind consumer 0's whole fill.  Tile it of warp c > 0 follows tile it of warp c - 1, tile it of warp 0 follows
+    // tile it - 1 of the last warp; after the first `lead` tiles (at most two) each waits on its own consumer's slots only.
+    // The runtime-loop kernels (7 x 7, 1 x 1, 64-channel chunks) measured slower with it and keep independent fills.
     const int lead = KS > 0 ? min(2, (p.slots + p.S - 1) / p.S) : 0;
-    const int rest = ntiles - (int)blockIdx.x - (pc ^ 1) * (int)gridDim.x;
-    const int n_other = rest > 0 ? (rest + NCONS * gridDim.x - 1) / (NCONS * gridDim.x) : 0;   // tiles of the other warp
+    const int pprev = pc == 0 ? NCONS - 1 : pc - 1, pnext = pc == NCONS - 1 ? 0 : pc + 1;
+    auto tiles_of = [&](int w) {                                    // local tiles of A warp w
+      const int rest = ntiles - (int)blockIdx.x - w * (int)gridDim.x;
+      return rest > 0 ? (int)((rest + NCONS * gridDim.x - 1) / (NCONS * gridDim.x)) : 0;
+    };
+    const int n_prev = tiles_of(pprev), n_next = tiles_of(pnext);
     uint32_t fph = 0;
     int slot = 0, it = 0;
     uint32_t ph = 0;
     for (int tile = blockIdx.x + pc * gridDim.x; tile < ntiles; tile += NCONS * gridDim.x, ++it) {
       if (RV_TL_DIAG == 3 || (RV_TL_MMA_ONLY && it >= 1)) break;   // diagnostics: only the resident slot / nothing
-      const int after = it - (pc == 0 ? 1 : 0);                     // the other warp's tile this one follows
-      if (it < lead && after >= 0 && after < n_other) {
+      const int after = it - (pc == 0 ? 1 : 0);                     // the previous warp's tile this one follows
+      if (it < lead && after >= 0 && after < n_prev) {
         tc::mbar_wait(&bar_fill[pc], fph);
         fph ^= 1u;
       }
@@ -418,8 +434,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
         else if (++ch == nchunks) { ch = 0; kx += (MODE == 1) ? 0 : 1; }
         if (++slot == p.slots) { slot = 0; ph ^= 1u; }
       }
-      const int next = it + (pc == 0 ? 0 : 1);                      // the other warp's tile that follows this one
-      if (next < lead && next < n_other && tl0) tc::mbar_arrive(&bar_fill[pc ^ 1]);
+      const int next = it + (pc == NCONS - 1 ? 1 : 0);              // the next warp's tile that follows this one
+      if (next < lead && next < n_next && tl0) tc::mbar_arrive(&bar_fill[pnext]);
     }
   } else {
     // ============================ consumers ================================
@@ -434,12 +450,17 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
     asm volatile("griddepcontrol.wait;" ::: "memory");     // gate / residual reads and all stores come after this
     int slot = 0;
     uint32_t ph = 0;
-    // Compile-time kernels: the consumers take turns on the tensor cores.  A consumer issues a tile's MMAs only after the
-    // other consumer has issued its previous tile's MMAs (consumer 0 starts), so the batches queue back to back and one
-    // consumer's epilogue runs under the other's MMAs; left alone, both consumers tend to issue at once, share the tensor
-    // cores, and then both run their epilogues with the tensor cores idle.
+    // Compile-time kernels: the consumers take turns on the tensor cores, in a ring.  Consumer c issues a tile's MMAs only
+    // after consumer c - 1 (the last one for consumer 0) has issued its MMAs of the tile before (consumer 0 starts), so
+    // the batches queue back to back and the epilogues run under the other consumers' MMAs; left alone, the consumers tend
+    // to issue at once, share the tensor cores, and then run their epilogues with the tensor cores idle.
     constexpr bool TURNS = KS > 0;
     uint32_t tph = 0;
+    // two consumers copy a tile's gate / residual values to registers before the epilogue and release the buffer at once;
+    // three read them from the buffer where they are used and release it after the values pass (128 registers a thread)
+    constexpr bool EPI_REGS = NCONS == 2;
+    const uint8_t* epi_g = nullptr;
+    const uint8_t* epi_r = nullptr;
     float acc[2][NB / 2];
     int ebuf = 0;
     uint32_t eph = 0;
@@ -453,6 +474,17 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
     int it = 0;
     const bool tl0 = t == 0;
     (void)tl0;
+    // three consumers: the gate / residual word of tile pixel m, channels nl, nl + 1 in buffer b (tl_diag 4: not read), and
+    // the buffer's release once every thread of the consumer has passed its reads and a proxy fence
+    auto epi_word = [&](const uint8_t* b, int m, int nl) {
+      const uint32_t off = (uint32_t)(m * NB + nl) * 2u;
+      return RV_TL_DIAG == 4 ? 0x3c003c00u ^ off : *reinterpret_cast<const uint32_t*>(b + off);
+    };
+    auto release_epi = [&]() {
+      if (t == 0) tc::mbar_arrive(&bar_eempty[cons][ebuf]);
+      if (++ebuf == p.epi_depth) { ebuf = 0; eph ^= 1u; }
+    };
+    (void)epi_word; (void)release_epi;
     for (int tile = blockIdx.x + cons * gridDim.x; tile < ntiles; tile += NCONS * gridDim.x, ++it) {
       const int img = BATCH ? tile / tiles_img : 0, ti = BATCH ? tile - img * tiles_img : tile;
       const int ty0 = ti / p.tiles_x, tx0 = ti - ty0 * p.tiles_x;
@@ -469,7 +501,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
       typename RawPair<TR>::type rv[2][2][NJ];
       // skipped whole when there is nothing to load: its unrolled, branchy code is several KB of instructions that every
       // tile of a plain conv would otherwise fetch and step through between its epilogue and its next MMA batch
-      if (EARLY && !epi_tma && (gate != nullptr || res != nullptr)) {
+      if (EARLY && EPI_REGS && !epi_tma && (gate != nullptr || res != nullptr)) {
 #pragma unroll
         for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -497,22 +529,22 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
           if (++ch == nchunks) ch = 0;
         }
         if (RV_TL_DIAG == 3) break;
-        RV_TL(tl0 && s == 0, NCONS + cons, it, 0);
+        RV_TL(tl0 && s == 0, TL_MAX_CONS + cons, it, 0);
         if (!RV_TL_MMA_ONLY || it == 0) tc::mbar_wait(&bar_full[cons][slot], ph);
-        RV_TL(tl0 && s == 0, NCONS + cons, it, 1);
+        RV_TL(tl0 && s == 0, TL_MAX_CONS + cons, it, 1);
         if (TURNS && s == 0 && (cons != 0 || it != 0)) {
           tc::mbar_wait(&bar_turn[cons], tph);
           tph ^= 1u;
         }
-        RV_TL(tl0 && s == 0, NCONS + cons, it, 2);
+        RV_TL(tl0 && s == 0, TL_MAX_CONS + cons, it, 2);
         const uint32_t a_addr = ring_addr + (uint32_t)slot * p.slot_bytes;
         const uint32_t b_addr = p.resident ? w_addr + (uint32_t)s * p.w_bytes : a_addr + p.a_bytes;
         tc::wgmma_fence();
-        RV_TL(tl0 && s == 0, NCONS + cons, it, 3);
+        RV_TL(tl0 && s == 0, TL_MAX_CONS + cons, it, 3);
         if (RV_TL_DIAG == 2) issue_stage<MODE, BF, NB, KS, KST, true>(p, acc, a_addr, b_addr, s, ksteps);
         else issue_stage<MODE, BF, NB, KS, KST>(p, acc, a_addr, b_addr, s, ksteps);
         tc::wgmma_commit();
-        if (TURNS && s == p.S - 1 && lane == 0) tc::mbar_arrive(&bar_turn[cons ^ 1]);   // the other consumer's turn
+        if (TURNS && s == p.S - 1 && lane == 0) tc::mbar_arrive(&bar_turn[cons == NCONS - 1 ? 0 : cons + 1]);   // the next turn
         if (RV_TL_MMA_ONLY) continue;    // MMA-only: the slot stays resident (S = 1)
         if (p.slots == 1) {
           // a single slot is refilled only after these MMAs have read it
@@ -527,15 +559,17 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
         if (++slot == p.slots) { slot = 0; ph ^= 1u; }
       }
       tc::wgmma_wait<0>();
-      RV_TL(tl0, NCONS + cons, it, 4);
+      RV_TL(tl0, TL_MAX_CONS + cons, it, 4);
       if (RV_TL_MMA_ONLY) continue;
       if (prev >= 0 && lane == 0) tc::mbar_arrive(&bar_empty[cons][prev]);
       if constexpr (TMA_OK) {
         if (epi_tma) {
           tc::mbar_wait(&bar_efull[cons][ebuf], eph);
-          RV_TL(tl0, NCONS + cons, it, 5);
-          uint8_t* epi_g = epi_buf(cons, ebuf);
-          const uint8_t* epi_r = epi_res(epi_g);
+          RV_TL(tl0, TL_MAX_CONS + cons, it, 5);
+          epi_g = epi_buf(cons, ebuf);
+          epi_r = epi_res(epi_buf(cons, ebuf));
+        }
+        if (epi_tma && EPI_REGS) {
 #pragma unroll
           for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -552,7 +586,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
                 if (res != nullptr) rv[h][r2][j] = *reinterpret_cast<const uint32_t*>(epi_r + off);
               }
           // all 128 threads have read the buffer: order those reads before the async proxy's writes of a later tile, then
-          // hand the buffer back to producer warp NCONS + cons
+          // hand the buffer back to its producer warp
           asm volatile("bar.sync %0, 128;" ::"r"(1 + cons) : "memory");
           if (t == 0) {
             tc::fence_proxy_async();
@@ -561,7 +595,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
           if (++ebuf == p.epi_depth) { ebuf = 0; eph ^= 1u; }
         }
       }
-      RV_TL(tl0 && !epi_tma, NCONS + cons, it, 5);
+      RV_TL(tl0 && !epi_tma, TL_MAX_CONS + cons, it, 5);
 
       // ---- epilogue: thread t holds rows 64 h + 16 wq + lane / 4 (+ 8) and column pairs 8 j + 2 (lane % 4) ----
       if constexpr (PSV) {
@@ -578,10 +612,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           if (out_tma) {
-            RV_TL(tl0 && h == 0, NCONS + cons, it, 6);
+            RV_TL(tl0 && h == 0, TL_MAX_CONS + cons, it, 6);
             if (t == 0) tc::bulk_wait_read<0>();      // this consumer's previous store has read the buffer
             asm volatile("bar.sync %0, 128;" ::"r"(1 + cons) : "memory");
-            RV_TL(tl0 && h == 0, NCONS + cons, it, 7);
+            RV_TL(tl0 && h == 0, TL_MAX_CONS + cons, it, 7);
           }
 #pragma unroll
           for (int r2 = 0; r2 < 2; ++r2) {
@@ -634,17 +668,17 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
             }
           }
         }
-        RV_TL(tl0, NCONS + cons, it, 8);
+        RV_TL(tl0, TL_MAX_CONS + cons, it, 8);
         continue;
       }
       if constexpr (OUT_TMA_OK && !PSV) {
         if (out_tma) {
-          RV_TL(tl0, NCONS + cons, it, 6);
+          RV_TL(tl0, TL_MAX_CONS + cons, it, 6);
           if (RV_TL_DIAG != 4) {
             if (t == 0) tc::bulk_wait_read<0>();      // this consumer's previous store has read the buffer
             asm volatile("bar.sync %0, 128;" ::"r"(1 + cons) : "memory");
           }
-          RV_TL(tl0, NCONS + cons, it, 7);
+          RV_TL(tl0, TL_MAX_CONS + cons, it, 7);
           uint32_t fold = 0;    // tl_diag 4: the epilogue's values, kept live without a shared-memory store
           (void)fold;
           // HG / HR / HP: the conv may have a gate / a residual / a post-activation or clamp.  The compile-time kernels run
@@ -670,11 +704,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
                   if (HG && gate != nullptr) {
                     // __fmul_rn: never contracted with the residual add into one FMA, whose single rounding would change
                     // the bits of gate + residual convs (with runtime tests the two were separate predicated instructions)
-                    const float2 g = raw2_to_f2<TI>(gv[h][r2][j]);
+                    const float2 g = raw2_to_f2<TI>(EPI_REGS ? gv[h][r2][j] : epi_word(epi_g, m, nl));
                     v[0] = __fmul_rn(v[0], g.x); v[1] = __fmul_rn(v[1], g.y);
                   }
                   if (HR && res != nullptr) {
-                    const float2 r = raw2_to_f2<TR>(rv[h][r2][j]);
+                    typename RawPair<TR>::type rw;
+                    if constexpr (EPI_REGS) rw = rv[h][r2][j];
+                    else rw = epi_word(epi_r, m, nl);
+                    const float2 r = raw2_to_f2<TR>(rw);
                     v[0] += r.x; v[1] += r.y;
                   }
                   if (HP) {
@@ -706,20 +743,26 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
           }
           if (RV_TL_DIAG == 4) {
             if (fold == 0x7fc00001u) out[0] = from_f<TO>(0.f);   // practically never taken: keeps the values live
-            RV_TL(tl0, NCONS + cons, it, 8);
+            if (!EPI_REGS && epi_tma) release_epi();             // (not read)
+            RV_TL(tl0, TL_MAX_CONS + cons, it, 8);
             continue;
           }
-          tc::fence_proxy_async();                  // the buffer's writes, before the async proxy reads them
+          // the buffer's writes (and, with three consumers, this thread's gate / residual reads), before the async proxy
+          // reads the one / overwrites the other
+          tc::fence_proxy_async();
           asm volatile("bar.sync %0, 128;" ::"r"(1 + cons) : "memory");
+          if (!EPI_REGS && epi_tma) release_epi();
           if (t == 0) {
             if (batched) tc::tma_store_4d(&tmo, out_s, nblk * NB, tx0 * p.tw, ty0 * p.th, img);
             else tc::tma_store_3d(&tmo, out_s, nblk * NB, tx0 * p.tw, ty0 * p.th);
             tc::bulk_commit();
           }
-          RV_TL(tl0, NCONS + cons, it, 8);
+          RV_TL(tl0, TL_MAX_CONS + cons, it, 8);
           continue;
         }
       }
+      // three consumers: the plan gives them the TMA-store epilogue only
+      if constexpr (EPI_REGS) {
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
 #pragma unroll
@@ -767,10 +810,28 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ 
           }
         }
       }
-      RV_TL(tl0, NCONS + cons, it, 8);
+      }
+      RV_TL(tl0, TL_MAX_CONS + cons, it, 8);
     }
     if (out_tma && t == 0) tc::bulk_wait<0>();     // the last stores are complete before the CTA exits
   }
+}
+
+template <typename TI, typename TR, typename TO, bool BATCH, int MODE, int NB, int KS, int KST, bool PSV>
+__global__ void __launch_bounds__(128 * (1 + 2), 1)
+conv_tc_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1,
+               const __grid_constant__ CUtensorMap tmg, const __grid_constant__ CUtensorMap tmr,
+               const __grid_constant__ CUtensorMap tmo, const TcP p) {
+  conv_tc_body<2, TI, TR, TO, BATCH, MODE, NB, KS, KST, PSV>(tm0, tm1, tmg, tmr, tmo, p);
+}
+
+// the single-source 48 -> 48 3 x 3 conv with three consumers (p.ncons == 3): one 16-bit type T for every operand
+template <typename T, bool BATCH>
+__global__ void __launch_bounds__(128 * (1 + 3), 1)
+conv_tc3_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1,
+                const __grid_constant__ CUtensorMap tmg, const __grid_constant__ CUtensorMap tmr,
+                const __grid_constant__ CUtensorMap tmo, const TcP p) {
+  conv_tc_body<3, T, T, T, BATCH, 1, 48, FIX_KS, FIX_KST, false>(tm0, tm1, tmg, tmr, tmo, p);
 }
 
 PFN_tmapEncodeTiled get_tmap_encoder() {
@@ -837,11 +898,14 @@ static int g_cta_cap = 0;          // rv_set_conv_cta_cap: upper bound of the pe
 int set_conv_cta_cap(int cap) { const int old = g_cta_cap; g_cta_cap = cap > 0 ? cap : 0; return old; }
 static int g_smem_cap = 0;         // rv_set_conv_smem_cap: upper bound of a launch's shared memory (0 = the device's opt-in limit)
 int set_conv_smem_cap(int bytes) { const int old = g_smem_cap; g_smem_cap = bytes > 0 ? bytes : 0; return old; }
+static int g_conv_consumers = 0;   // rv_set_conv_consumers: 2 = the two-consumer kernel for every conv (0 = the plan's choice)
+int set_conv_consumers(int n) { const int old = g_conv_consumers; g_conv_consumers = n == 2 ? 2 : 0; return old; }
 
-template <typename TI, typename TR, typename TO, int MODE, int NB, int KS = 0, int KST = 0, bool PSV = false>
+template <typename TI, typename TR, typename TO, int MODE, int NB, int KS = 0, int KST = 0, bool PSV = false, int NCONS = 2>
 static int launch_tc_mode(const CUtensorMap* tm, const TcP& p, dim3 grid, size_t smem, cudaStream_t st) {
   const int batch = p.nimg > 1 ? 1 : 0;
   auto kern = batch ? conv_tc_kernel<TI, TR, TO, true, MODE, NB, KS, KST, PSV> : conv_tc_kernel<TI, TR, TO, false, MODE, NB, KS, KST, PSV>;
+  if constexpr (NCONS == 3) kern = batch ? conv_tc3_kernel<TO, true> : conv_tc3_kernel<TO, false>;
   static size_t configured[2] = {0, 0};   // per template instantiation
   if (smem > configured[batch]) {
     RV_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -871,6 +935,8 @@ static int launch_tc_nb(const CUtensorMap* tm, const TcP& p, dim3 grid, size_t s
       if constexpr (fixed_nb(NB)) {
         if constexpr (NB == 96 && sizeof(TO) == 2)
           if (p.ps_vec) return launch_tc_mode<TI, TR, TO, 1, NB, FIX_KS, FIX_KST, true>(tm, p, grid, smem, st);
+        if constexpr (NB == 48 && sizeof(TO) == 2 && std::is_same<TI, TO>::value && std::is_same<TR, TO>::value)
+          if (p.ncons == 3) return launch_tc_mode<TI, TR, TO, 1, NB, FIX_KS, FIX_KST, false, 3>(tm, p, grid, smem, st);
         if (p.fixed) return launch_tc_mode<TI, TR, TO, 1, NB, FIX_KS, FIX_KST>(tm, p, grid, smem, st);
       }
       return launch_tc_mode<TI, TR, TO, 1, NB>(tm, p, grid, smem, st);
@@ -951,24 +1017,6 @@ static int plan_tc(const rv_conv_desc* d, TcP& p, size_t& smem_out, int& nblk_ou
     p.w_bytes = (uint32_t)d->kh * p.NB * 128;
   }
   p.tiles_x = (p.Wo + p.tw - 1) / p.tw; p.tiles_y = (p.Ho + p.th - 1) / p.th;
-  // shared-memory plan: weights resident when they leave room for two slots per consumer (layout 1: one), else streamed with
-  // A; a consumer with a single slot still overlaps with the other consumer's ring
-  const size_t w_all = (size_t)p.S * p.w_bytes;
-  const size_t ring_min = (size_t)NCONS * (p.mode == 1 ? 1 : 2) * p.a_bytes;
-  // TMA epilogue: 16-bit gate / residual whose boxes TMA can address (16-byte aligned base and pixel stride), tiles the
-  // register epilogue keeps whole (NB <= 48), and room for the buffers next to resident weights and the minimal ring
-  const int rdt0 = d->res ? d->res_dtype : d->in_dtype;
-  auto tma_ok = [batched](const void* q, int cs, long long bs) {
-    return q == nullptr || ((uintptr_t)q % 16 == 0 && cs > 0 && cs % 8 == 0 && (!batched || bs % 8 == 0));
-  };
-  p.epi_bytes = (uint32_t)p.th * p.tw * p.NB * 2;
-  p.epi_tx = (uint32_t)((d->gate ? 1 : 0) + (d->res ? 1 : 0)) * p.epi_bytes;
-  p.epi_tma = (d->gate || d->res) && p.NB <= 48 && rdt0 == d->in_dtype && tma_ok(d->gate, d->gate_cs, d->bs_gate) &&
-              tma_ok(d->res, d->res_cs, d->bs_res) && w_all + ring_min + (size_t)NCONS * p.epi_tx <= budget;
-  // a second buffer lets the boxes arrive up to two tiles ahead of the epilogue; it is taken only while two A slots and the
-  // output buffer per consumer still fit (gate + residual at NB = 48 keeps two A slots and one buffer)
-  p.epi_depth = p.epi_tma && w_all + (size_t)NCONS * (2 * p.a_bytes + MAX_EPI * p.epi_tx + p.epi_bytes) <= budget ? MAX_EPI : 1;
-  const size_t epi_all = p.epi_tma ? (size_t)NCONS * p.epi_depth * p.epi_tx : 0;
   // the compile-time tap loop: a square FIX_KS kernel whose every channel chunk takes FIX_KST K-steps (e.g. 48 + 48
   // channels, not 8 + 48); other shapes keep the runtime loop
   p.fixed = p.mode == 1 && d->kh == FIX_KS && d->kw == FIX_KS && fixed_nb(p.NB);
@@ -984,6 +1032,17 @@ static int plan_tc(const rv_conv_desc* d, TcP& p, size_t& smem_out, int& nblk_ou
              !d->res && d->out != nullptr && (uintptr_t)d->out % 16 == 0 && (d->out_cs * 2) % 16 == 0 && (!batched || d->bs_out % 8 == 0);
   RV_REQUIRE(!d->ps_order || p.ps_vec, "rv_conv2d(tc): ps_order=1 needs the 3x3 48-channel nb=96 kernel with a 16-bit output "
              "whose HR pixel rows are 16-byte aligned (out_cs=%d), no gate / residual", d->out_cs);
+  // shared-memory plan for nc consumers (buffers below): weights resident when they leave room for two slots per consumer
+  // (layout 1: one), else streamed with A; a consumer with a single slot still overlaps with the other consumers' rings
+  const size_t w_all = (size_t)p.S * p.w_bytes;
+  // TMA epilogue: 16-bit gate / residual whose boxes TMA can address (16-byte aligned base and pixel stride), tiles the
+  // register epilogue keeps whole (NB <= 48), and room for the buffers next to resident weights and the minimal ring
+  const int rdt0 = d->res ? d->res_dtype : d->in_dtype;
+  auto tma_ok = [batched](const void* q, int cs, long long bs) {
+    return q == nullptr || ((uintptr_t)q % 16 == 0 && cs > 0 && cs % 8 == 0 && (!batched || bs % 8 == 0));
+  };
+  p.epi_bytes = (uint32_t)p.th * p.tw * p.NB * 2;
+  p.epi_tx = (uint32_t)((d->gate ? 1 : 0) + (d->res ? 1 : 0)) * p.epi_bytes;
   // TMA-store epilogue, when its buffer per consumer fits next to the resident weights, the gate / residual buffers and the
   // minimal ring: kernels up to NB = 48 writing a plain (not pixel-shuffled) map of the input's 16-bit type whose base
   // and pixel stride TMA can address ([128 pixels][NB] buffer, th x tw of the layout mode), and the PSV kernel (half a tile of HR rows,
@@ -991,12 +1050,32 @@ static int plan_tc(const rv_conv_desc* d, TcP& p, size_t& smem_out, int& nblk_ou
   const bool out_plain = p.NB <= 48 && !d->pixel_shuffle && d->out_dtype == d->in_dtype && d->out != nullptr &&
                          tma_ok(d->out, d->out_cs, d->bs_out);
   p.out_bytes = p.ps_vec ? p.epi_bytes / 2 : p.epi_bytes;
-  p.out_tma = (out_plain || p.ps_vec) && w_all + ring_min + epi_all + (size_t)NCONS * p.out_bytes <= budget;
-  const size_t out_all = p.out_tma ? (size_t)NCONS * p.out_bytes : 0;
-  if (w_all + ring_min + epi_all + out_all <= budget) {
+  size_t epi_all = 0, out_all = 0;
+  // the epilogue buffers of nc consumers; true when they, the resident weights and the minimal ring fit
+  auto buffers = [&](int nc) {
+    const size_t ring_min = (size_t)nc * (p.mode == 1 ? 1 : 2) * p.a_bytes;
+    p.epi_tma = (d->gate || d->res) && p.NB <= 48 && rdt0 == d->in_dtype && tma_ok(d->gate, d->gate_cs, d->bs_gate) &&
+                tma_ok(d->res, d->res_cs, d->bs_res) && w_all + ring_min + (size_t)nc * p.epi_tx <= budget;
+    // a second buffer lets the boxes arrive up to two tiles ahead of the epilogue; it is taken only while two A slots and
+    // the output buffer per consumer still fit (gate + residual at NB = 48 keeps two A slots and one buffer)
+    p.epi_depth = p.epi_tma && w_all + (size_t)nc * (2 * p.a_bytes + MAX_EPI * p.epi_tx + p.epi_bytes) <= budget ? MAX_EPI : 1;
+    epi_all = p.epi_tma ? (size_t)nc * p.epi_depth * p.epi_tx : 0;
+    p.out_tma = (out_plain || p.ps_vec) && w_all + ring_min + epi_all + (size_t)nc * p.out_bytes <= budget;
+    out_all = p.out_tma ? (size_t)nc * p.out_bytes : 0;
+    return w_all + ring_min + epi_all + out_all <= budget;
+  };
+  // Three consumers (conv_tc3_kernel) for the single-source 48 -> 48 3 x 3 convs with a 16-bit output, plain or with a
+  // residual, when the weights, one A slot, the output buffer and (residual) one residual buffer per consumer fit (199 680
+  // bytes with a residual).  Measured on an H100 at 700 W against two consumers (README "Three consumers"): 14.9 -> 13.7 us
+  // plain and 18.4 -> 17.4 us with a residual at 270 x 480, 44.7 -> 42.3 / 57.0 -> 55.1 us at 540 x 960, conv_hr 163 -> 159
+  // us.  Gate + residual needs 236 544 bytes and keeps two consumers (a gate alone, not in the window, too).
+  const bool three = g_conv_consumers != 2 && p.fixed && p.NB == 48 && p.S == 1 && !d->gate && out_plain && rdt0 == d->in_dtype;
+  p.ncons = three && buffers(3) && p.out_tma && (p.epi_tma || !d->res) ? 3 : 2;
+  const size_t nc = (size_t)p.ncons;
+  if (buffers(p.ncons)) {
     p.resident = 1;
     p.slot_bytes = p.a_bytes;
-    p.slots = (int)std::min<size_t>(MAX_SLOTS, (budget - w_all - epi_all - out_all) / ((size_t)NCONS * p.a_bytes));
+    p.slots = (int)std::min<size_t>(MAX_SLOTS, (budget - w_all - epi_all - out_all) / (nc * p.a_bytes));
 #ifdef RV_CONV_TIMELINE
     if (g_tl_max_slots > 0) p.slots = std::min(p.slots, g_tl_max_slots);
 #endif
@@ -1004,11 +1083,11 @@ static int plan_tc(const rv_conv_desc* d, TcP& p, size_t& smem_out, int& nblk_ou
     RV_REQUIRE(p.mode != 1, "rv_conv2d(tc): layout 1 weights do not fit in shared memory");
     p.resident = 0;
     p.slot_bytes = p.a_bytes + p.w_bytes;
-    p.slots = (int)std::min<size_t>(MAX_SLOTS, budget / ((size_t)NCONS * p.slot_bytes));
+    p.slots = (int)std::min<size_t>(MAX_SLOTS, budget / (nc * p.slot_bytes));
     RV_REQUIRE(p.slots >= 1, "rv_conv2d(tc): stage of %u bytes does not fit once per consumer in shared memory", p.slot_bytes);
   }
-  p.out_off = (uint32_t)((size_t)NCONS * p.slots * p.slot_bytes + epi_all);
-  const size_t smem = 1024 + (p.resident ? w_all : 0) + (size_t)NCONS * p.slots * p.slot_bytes + epi_all + out_all;
+  p.out_off = (uint32_t)(nc * p.slots * p.slot_bytes + epi_all);
+  const size_t smem = 1024 + (p.resident ? w_all : 0) + nc * p.slots * p.slot_bytes + epi_all + out_all;
   p.wpack = (const uint8_t*)d->wpack; p.bias = d->bias;
   auto slope = [](int act) { return act == RV_ACT_RELU ? 0.f : act == RV_ACT_LRELU01 ? 0.1f : act == RV_ACT_LRELU02 ? 0.2f : 1.f; };
   RV_REQUIRE(d->act_pre != RV_ACT_CLAMP3, "rv_conv2d(tc): clamp3 is only supported as act_post");
@@ -1079,25 +1158,27 @@ int conv2d_tc(const rv_conv_desc* d, cudaStream_t st) {
   return fail(RV_E_UNSUPPORTED, "rv_conv2d(tc): unsupported dtype combination in=%d res=%d out=%d", d->in_dtype, rdt, d->out_dtype);
 }
 
-// host-only: the launch plan of rv_conv2d (tensor-core path) for given device limits -> out[8] = {mode, slots per consumer,
-// weights resident, S, consumer warpgroups, accumulator sets, nb, smem bytes}.  mode: 0 boxes per (kx, chunk), 1 single box,
-// 2 32B-swizzled quads.
-static int plan_for(const rv_conv_desc* d, int max_smem, int num_sms, TcP& p, size_t& smem) {
-  const int s0 = g_num_sms, s1 = g_max_smem, s2 = g_smem_cap;
+// host-only: the launch plan of rv_conv2d (tensor-core path) for given device limits.  `consumers` 2 plans the two-consumer
+// kernel whatever rv_set_conv_consumers holds, 0 takes that setting (and so the kernel a launch would run).
+static int plan_for(const rv_conv_desc* d, int max_smem, int num_sms, int consumers, TcP& p, size_t& smem) {
+  const int s0 = g_num_sms, s1 = g_max_smem, s2 = g_smem_cap, s3 = g_conv_consumers;
   g_num_sms = num_sms; g_max_smem = max_smem; g_smem_cap = 0;
+  if (consumers == 2) g_conv_consumers = 2;
   int nblk = 1;
   const int rc = plan_tc(d, p, smem, nblk);
-  g_num_sms = s0; g_max_smem = s1; g_smem_cap = s2;
+  g_num_sms = s0; g_max_smem = s1; g_smem_cap = s2; g_conv_consumers = s3;
   return rc;
 }
 
+// host-only, the two-consumer plan -> out[8] = {mode, slots per consumer, weights resident, S, consumer warpgroups,
+// accumulator sets, nb, smem bytes}.  mode: 0 boxes per (kx, chunk), 1 single box, 2 32B-swizzled quads.
 int conv2d_tc_plan(const rv_conv_desc* d, int max_smem, int num_sms, int* out) {
   TcP p;
   size_t smem = 0;
-  const int rc = plan_for(d, max_smem, num_sms, p, smem);
+  const int rc = plan_for(d, max_smem, num_sms, 2, p, smem);
   if (rc) return rc;
   out[0] = p.mode;
-  out[1] = p.slots; out[2] = p.resident; out[3] = p.S; out[4] = NCONS; out[5] = NCONS; out[6] = p.NB; out[7] = (int)smem;
+  out[1] = p.slots; out[2] = p.resident; out[3] = p.S; out[4] = p.ncons; out[5] = p.ncons; out[6] = p.NB; out[7] = (int)smem;
   return RV_OK;
 }
 
@@ -1105,7 +1186,7 @@ int conv2d_tc_plan(const rv_conv_desc* d, int max_smem, int num_sms, int* out) {
 int conv2d_tc_epi_depth(const rv_conv_desc* d, int max_smem, int num_sms, int* depth) {
   TcP p;
   size_t smem = 0;
-  const int rc = plan_for(d, max_smem, num_sms, p, smem);
+  const int rc = plan_for(d, max_smem, num_sms, 2, p, smem);
   if (rc) return rc;
   *depth = p.epi_tma ? p.epi_depth : 0;
   return RV_OK;
@@ -1116,9 +1197,20 @@ int conv2d_tc_epi_depth(const rv_conv_desc* d, int max_smem, int num_sms, int* d
 int conv2d_tc_out_store(const rv_conv_desc* d, int max_smem, int num_sms, int* kind) {
   TcP p;
   size_t smem = 0;
-  const int rc = plan_for(d, max_smem, num_sms, p, smem);
+  const int rc = plan_for(d, max_smem, num_sms, 2, p, smem);
   if (rc) return rc;
   *kind = p.ps_vec ? (p.out_tma ? 2 : 3) : (p.out_tma ? 1 : 0);
+  return RV_OK;
+}
+
+// host-only: the plan a launch takes under the current rv_set_conv_consumers -> out[4] = {consumer warpgroups, slots per
+// consumer, gate / residual buffers per consumer (0: none by TMA), smem bytes}
+int conv2d_tc_consumers(const rv_conv_desc* d, int max_smem, int num_sms, int* out) {
+  TcP p;
+  size_t smem = 0;
+  const int rc = plan_for(d, max_smem, num_sms, 0, p, smem);
+  if (rc) return rc;
+  out[0] = p.ncons; out[1] = p.slots; out[2] = p.epi_tma ? p.epi_depth : 0; out[3] = (int)smem;
   return RV_OK;
 }
 

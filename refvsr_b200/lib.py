@@ -71,6 +71,8 @@ SIGNATURES = {
     'rv_conv2d_tc_epi_depth': (_I, [C.POINTER(rv_conv_desc), _I, _I, C.POINTER(C.c_int32)]),
     'rv_conv2d_tc_out_store': (_I, [C.POINTER(rv_conv_desc), _I, _I, C.POINTER(C.c_int32)]),
     'rv_set_conv_smem_cap': (_I, [_I]),
+    'rv_set_conv_consumers': (_I, [_I]),
+    'rv_conv2d_tc_consumers': (_I, [C.POINTER(rv_conv_desc), _I, _I, C.POINTER(C.c_int32)]),
     'rv_resblock': (_I, [C.POINTER(rv_resblock_desc), _P]),
     'rv_conv_chain': (_I, [C.POINTER(rv_conv_chain_desc), _P]),
     'rv_space_to_depth2': (_I, [_P, _I, _I, _I, _I, _P, _P]),
@@ -164,6 +166,11 @@ class CudaOps:
     def set_conv_smem_cap(self, nbytes):
         """shared-memory bound the following tensor-core conv launches plan with (0 = the device's limit); returns the previous value"""
         return int(self.lib.rv_set_conv_smem_cap(int(nbytes)))
+
+    def set_conv_consumers(self, n):
+        """2: the following tensor-core conv launches run the two-consumer kernel for every conv; 0: the plan's choice (three
+        consumers for the single-source 48 -> 48 3x3 convs when they fit); returns the previous value"""
+        return int(self.lib.rv_set_conv_consumers(int(n)))
 
     # -- convolution ------------------------------------------------------------------------------
     def conv2d(self, layer, src0, src1, out, gate=None, res=None, act_pre=ACT_NONE, act_post=ACT_NONE,

@@ -11,10 +11,11 @@ pipeline with an epilogue that neither reads nor writes shared memory; TMA-store
 one pipeline stage per tile (one channel chunk), which all shapes here are.
 
     python tools/conv_timeline.py [--csrc DIR] [--tag NAME] [--json FILE] [--out DIR] [--build-only | --prebuilt]
-                                  [--shapes SUBSTR,...] [--max-slots N]
+                                  [--shapes SUBSTR,...] [--max-slots N] [--consumers 2]
 
 --csrc builds the conv_tc.cu of another tree (e.g. the parent commit's, whose build() has run) for a before/after
-comparison; the stamp layout of either version is read from the library.
+comparison; the stamp layout of either version is read from the library.  --consumers 2 runs the two-consumer kernel for
+every conv (rv_set_conv_consumers) where the plan would take three.
 The library goes to --out, by default a new temporary directory; --build-only stops there and --prebuilt runs what an
 earlier --build-only left in --out."""
 import argparse
@@ -79,6 +80,7 @@ def stamp_layout(roles):
             ('consumer full-slot + turn wait', 'c', 0, 1), ('consumer fence to first wgmma', 'c', 1, 2),
             ('consumer wgmma issue -> wait_group 0', 'c', 2, 3), ('consumer epilogue-buffer wait (+ copy)', 'c', 3, 4),
             ('consumer epilogue', 'c', 4, 5), ('consumer tile (full wait start -> epilogue end)', 'c', 0, 5)])
+    # roles // 2 consumer roles, consumer c at roles // 2 + c; a kernel with fewer consumers leaves the last ones empty
     n = roles // 2
     return dict(prod=list(range(n)), cons=list(range(n, roles)), mma=(3, 4),
                 lat=[('A box issue -> consumer has it', 2, 1), ('gate/res box issue -> consumer has it', 5, 5)], phases=[
@@ -156,6 +158,7 @@ def main():
     ap.add_argument('--variants', default='full,mma,mma_aligned,epi')
     ap.add_argument('--shapes', default='', help='comma-separated substrings of the shape names to run (default: all)')
     ap.add_argument('--max-slots', type=int, default=0, help='cap the A ring at this many slots per consumer (0: the plan)')
+    ap.add_argument('--consumers', type=int, default=0, help='2: the two-consumer kernel for every conv (0: the plan)')
     args = ap.parse_args()
     out_dir = args.out or tempfile.mkdtemp(prefix='conv_timeline_')
     os.makedirs(out_dir, exist_ok=True)
@@ -195,6 +198,8 @@ def main():
     results = {}
     if args.max_slots:
         lib.rv_conv_timeline_max_slots(args.max_slots)
+    if args.consumers:
+        lib.rv_set_conv_consumers(args.consumers)
     only = [s for s in args.shapes.split(',') if s]
     for name, cin, cout, h, w, res, ps, gate in shapes():
         if only and not any(s in name for s in only):

@@ -5,7 +5,7 @@ windows, torch.profiler (CUDA activities) around the last one only.
 
 --batch N: N clips per forward() call (one batched window schedule; a different seeded scene per clip); the totals are also
 given per clip.  Prints the table, the window's device time and the share of the 3x3 48-channel tensor-core conv (the
-compile-time NB 48 kernel); with OUT_DIR, also writes them to OUT_DIR/profile_window[_nN].txt."""
+compile-time NB 48 kernels, two or three consumers); with OUT_DIR, also writes them to OUT_DIR/profile_window[_nN].txt."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -36,7 +36,7 @@ for k in range(NW):
 ev = prof.key_averages()
 table = ev.table(sort_by='cuda_time_total', row_limit=40, max_name_column_width=90)
 tot = sum(e.self_device_time_total for e in ev)
-conv3 = [e for e in ev if 'conv_tc_kernel' in e.key and ', 1, 48, 3, 3, false>' in e.key]
+conv3 = [e for e in ev if ('conv_tc_kernel' in e.key and ', 1, 48, 3, 3, false>' in e.key) or 'conv_tc3_kernel' in e.key]
 c3 = sum(e.self_device_time_total for e in conv3)
 c3n = sum(e.count for e in conv3)
 summary = (f'batch {nb}: device time of the window, all kernels: {tot / 1e3:.2f} ms ({tot / 1e3 / nb:.2f} ms per clip); '
