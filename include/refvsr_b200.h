@@ -325,6 +325,26 @@ int rv_reconstruct(const void* x, int xc, int x_dtype, const float* lr_nchw, int
 int rv_reconstruct_batched(const void* x, int xc, int x_dtype, const float* lr_nchw, int h, int w, int scale,
                            int clamp01, float* out_nchw, int n, void* stream);   /* see rv_warp_batched */
 
+/* ------------------------------------------------------------------------------------------------
+ * rv_region_metrics - the per-frame sums behind the FOV evaluation mode: evaluation/metrics.py:18-31 (psnr, psnr_masked,
+ * ssim, ssim_masked) as evaluation/eval_quan_FOV.py:153-213 uses them, where every mask is a union or difference of boxes.
+ *   a, b        contiguous fp32 (1, 3, H, W) images (output, ground truth), H, W >= 7
+ *   boxes_host  HOST array of nbox x (y0, y1, x0, x1), half-open, inside the frame (empty and overlapping boxes allowed),
+ *               1 <= nbox <= 8
+ *   sums        device fp64 [2 * nbox]:  sums[k]        = sum over box k and the 3 channels of (a - b)^2 (float32 difference
+ *                                                         and square, as numpy's float32 arrays compute them)
+ *                                        sums[nbox + k] = sum over box k and the 3 channels of the SSIM map S
+ *   S is skimage's structural_similarity map for data_range 1: uniform 7x7 window computed in fp64, sample covariance
+ *   (49/48), C1 = 1e-4, C2 = 9e-4, over the FULL frame with scipy `reflect` borders (index -1 -> 0, -2 -> 1, -3 -> 2, likewise
+ *   at the far edges), i.e. the map ssim_masked multiplies by its mask.
+ *   work        device fp64 scratch of RV_REGION_METRICS_WORK(H, W, nbox) doubles.
+ * Two launches, no allocation, no atomics: the second reduces the per-CTA partials in a fixed order, so repeated calls are
+ * bit-identical.  RV_E_INVALID for any argument outside the above.
+ * ------------------------------------------------------------------------------------------------ */
+#define RV_REGION_METRICS_WORK(H, W, nbox) ((((H) + 15) / 16) * (((W) + 31) / 32) * 2 * (nbox))
+int rv_region_metrics(const float* a, const float* b, int H, int W, const int32_t* boxes_host, int nbox, double* work,
+                      double* sums, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -98,6 +98,7 @@ SIGNATURES = {
     'rv_conf_max': (_I, [_P, _P, _P, _I, _P]),
     'rv_frames_differ': (_I, [_P, _P, _P, _I, _P, _P]),
     'rv_reconstruct': (_I, [_P, _I, _I, _P, _I, _I, _I, _I, _P, _P]),
+    'rv_region_metrics': (_I, [_P, _P, _I, _I, C.POINTER(C.c_int32), _I, _P, _P, _P]),
 }
 
 _lib = None
@@ -414,3 +415,30 @@ class CudaOps:
         _check(self.lib, self.lib.rv_reconstruct(_ptr(x), x.shape[2], DTYPE_CODE[x.dtype], _ptr(lr), lr.shape[1],
                                                  lr.shape[2], scale, int(clamp01), _ptr(out), self._stream()),
                'rv_reconstruct')
+
+    # -- evaluation metrics -----------------------------------------------------------------------
+    def region_metrics(self, a, b, boxes):
+        """a, b: contiguous fp32 (1, 3, H, W) CUDA images; boxes: up to 8 (y0, y1, x0, x1) half-open boxes inside the frame.
+        Returns float64 numpy arrays (sq, s), each [len(boxes)]: per box, the sum of the float32 squared error and the sum of
+        skimage's full-frame SSIM map over the box and the 3 channels (rv_region_metrics).  Synchronises the current stream
+        with one 8 * 2 * len(boxes) byte device-to-host copy."""
+        for name, t in (('a', a), ('b', b)):
+            if not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous():
+                raise ValueError(f'region_metrics: {name} must be a contiguous float32 CUDA tensor')
+            if t.dim() != 4 or t.shape[0] != 1 or t.shape[1] != 3:
+                raise ValueError(f'region_metrics: {name} must be (1, 3, H, W), got {tuple(t.shape)}')
+        if a.shape != b.shape or a.device != b.device:
+            raise ValueError(f'region_metrics: a {tuple(a.shape)} on {a.device} and b {tuple(b.shape)} on {b.device} differ')
+        flat = [int(v) for box in boxes for v in box]
+        if len(flat) != 4 * len(boxes):
+            raise ValueError('region_metrics: every box is (y0, y1, x0, x1)')
+        n, H, W = len(boxes), a.shape[2], a.shape[3]
+        need = ((H + 15) // 16) * ((W + 31) // 32) * 2 * n          # RV_REGION_METRICS_WORK(H, W, nbox)
+        ws = getattr(self, '_region_ws', None)
+        if ws is None or ws[0].device != a.device or ws[0].numel() < need:
+            ws = (torch.empty(max(need, 1), dtype=torch.float64, device=a.device), torch.empty(16, dtype=torch.float64, device=a.device))
+            self._region_ws = ws
+        _check(self.lib, self.lib.rv_region_metrics(_ptr(a), _ptr(b), H, W, (C.c_int32 * max(len(flat), 1))(*flat), n, _ptr(ws[0]),
+                                                    _ptr(ws[1]), self._stream()), 'rv_region_metrics')
+        host = ws[1][:2 * n].cpu().numpy()
+        return host[:n], host[n:]
