@@ -345,6 +345,33 @@ int rv_reconstruct_batched(const void* x, int xc, int x_dtype, const float* lr_n
 int rv_region_metrics(const float* a, const float* b, int H, int W, const int32_t* boxes_host, int nbox, double* work,
                       double* sums, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * rv_conf_map_images - the per-frame image bytes of the confidence-map evaluation mode (evaluation/eval_quan_conf_map.py:
+ * 64-165): the colour-mapped confidence maps, the input and the output, each as the uint8 BGR HWC image cv2.imwrite encodes.
+ *   conf, prop, prop_b, prop_f   fp32 (h, w) maps: conf_map, conf_map_prop, conf_map_prop_backward, conf_map_prop_forward
+ *   normalize    1: the four maps, each min/max-normalised as torch float32 computes it (y = x - min(x); y / max(y))
+ *                0: `conf` alone, coloured as it is (the reference's branch for a vis without conf_map_prop; the other three
+ *                   pointers are ignored)
+ *   inp, out     contiguous fp32 NCHW (1, 3, ih, iw) and (1, 3, oh, ow) RGB frames
+ *   lut_rgb      device uint8 [256][3]: the colormap's entries as the 8-bit values cv2.imwrite writes for them
+ *   work         device scratch of RV_CONF_MAP_WORK uint32 words
+ *   dst          device uint8 of RV_CONF_MAP_BYTES(h, w, ih, iw, oh, ow, normalize) bytes, packed without gaps: the maps
+ *                (h, w, 3) in the order above, then the input (ih, iw, 3), then the output (oh, ow, 3), all BGR
+ * A map value y (after normalisation, if any) takes matplotlib's Colormap.__call__ index for a float32 array: t = fl32(y * 256),
+ * 255 for t == 256, NaN -> black (the "bad" colour), t < 0 -> 0 (under), t >= 256 -> 255 (over), else trunc(t).  A frame value
+ * x becomes cv::Mat::convertTo(CV_8U) of fl32(x * 255): round half to even, saturated to [0, 255]; NaN and values outside
+ * int32 become 0, as x86 builds of OpenCV convert them.  A constant map normalises to 0 / 0 = NaN and comes out black.
+ * At most two launches: per-CTA min / max partials of each map (normalize only), then the image pass, which folds them first.
+ * No atomics, no allocation.
+ * RV_E_INVALID for any argument outside the above.
+ * ------------------------------------------------------------------------------------------------ */
+#define RV_CONF_MAP_WORK 512
+#define RV_CONF_MAP_BYTES(h, w, ih, iw, oh, ow, normalize) \
+  (3ll * ((normalize) ? 4 : 1) * (h) * (w) + 3ll * (ih) * (iw) + 3ll * (oh) * (ow))
+int rv_conf_map_images(const float* conf, const float* prop, const float* prop_b, const float* prop_f, int h, int w,
+                       int normalize, const float* inp, int ih, int iw, const float* out, int oh, int ow,
+                       const uint8_t* lut_rgb, uint32_t* work, uint8_t* dst, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

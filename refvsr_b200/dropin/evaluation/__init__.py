@@ -1,8 +1,9 @@
 """Drop-in for the reference's `evaluation` package (SURVEY 8f row 1: the evaluation loop around the hot path).
 
 With `<repo>/refvsr_b200/dropin` in front of the reference checkout on sys.path this package takes the place of `evaluation`;
-`eval_qual_quan.py` (the default `qual_quan` mode) and `eval_quan_FOV.py` (`--eval_mode FOV`) are overridden, every other
-sub-module (`init`, `metrics`, `eval_quan_conf_map`) resolves to the reference's file through `__path__`."""
+`eval_qual_quan.py` (the default `qual_quan` mode), `eval_quan_FOV.py` (`--eval_mode FOV`) and `eval_quan_conf_map.py`
+(`--eval_mode conf`) are overridden, every other sub-module (`init`, `metrics`) resolves to the reference's file through
+`__path__`."""
 import os
 import sys
 

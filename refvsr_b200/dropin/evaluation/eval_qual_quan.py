@@ -55,13 +55,16 @@ def ssim_device(a, b, data_range=1.0, win=7):
 
 
 def _write_images(job):
+    """(event, arrays, paths): after the event, write each array to each of its paths; float arrays are RGB in [0, 1] and
+    written as the reference writes them, uint8 arrays are BGR images written as they are"""
     ev, arrays, paths = job
     if ev is not None:
         ev.synchronize()
     for arr, path in zip(arrays, paths):
+        img = arr if arr.dtype == np.uint8 else cv2.cvtColor(arr * 255, cv2.COLOR_RGB2BGR)
         for p in path:
             Path(os.path.dirname(p)).mkdir(parents=True, exist_ok=True)
-            cv2.imwrite(p, cv2.cvtColor(arr * 255, cv2.COLOR_RGB2BGR))
+            cv2.imwrite(p, img)
 
 
 def eval_qual_quan(config):

@@ -99,7 +99,15 @@ SIGNATURES = {
     'rv_frames_differ': (_I, [_P, _P, _P, _I, _P, _P]),
     'rv_reconstruct': (_I, [_P, _I, _I, _P, _I, _I, _I, _I, _P, _P]),
     'rv_region_metrics': (_I, [_P, _P, _I, _I, C.POINTER(C.c_int32), _I, _P, _P, _P]),
+    'rv_conf_map_images': (_I, [_P, _P, _P, _P, _I, _I, _I, _P, _I, _I, _P, _I, _I, _P, _P, _P, _P]),
 }
+
+CONF_MAP_WORK = 512                 # RV_CONF_MAP_WORK
+
+
+def conf_map_bytes(h, w, ih, iw, oh, ow, normalize):
+    """RV_CONF_MAP_BYTES: size of rv_conf_map_images' packed output"""
+    return 3 * (4 if normalize else 1) * h * w + 3 * ih * iw + 3 * oh * ow
 
 _lib = None
 
@@ -442,3 +450,38 @@ class CudaOps:
                                                     _ptr(ws[1]), self._stream()), 'rv_region_metrics')
         host = ws[1][:2 * n].cpu().numpy()
         return host[:n], host[n:]
+
+    def conf_map_images(self, maps, inp, out, lut, normalize):
+        """The image bytes of one frame of the confidence-map evaluation mode (rv_conf_map_images).
+        maps: [conf_map, conf_map_prop, conf_map_prop_backward, conf_map_prop_forward] with normalize, [conf_map] without;
+        each a contiguous float32 (1, 1, h, w) CUDA tensor.  inp, out: contiguous float32 (1, 3, ih, iw) / (1, 3, oh, ow) RGB
+        frames.  lut: uint8 (256, 3) RGB CUDA tensor (refvsr_b200.colormap).  Returns a uint8 CUDA tensor of
+        conf_map_bytes(...) bytes: the maps', then the input's, then the output's BGR HWC image, packed.  The tensor is a view
+        of a buffer this object reuses: the next call on the stream overwrites it."""
+        normalize = bool(normalize)
+        if len(maps) != (4 if normalize else 1):
+            raise ValueError(f'conf_map_images: {4 if normalize else 1} maps expected with normalize={normalize}, got {len(maps)}')
+        for name, t, c in [(f'maps[{k}]', m, 1) for k, m in enumerate(maps)] + [('inp', inp, 3), ('out', out, 3)]:
+            if not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous():
+                raise ValueError(f'conf_map_images: {name} must be a contiguous float32 CUDA tensor')
+            if t.dim() != 4 or t.shape[0] != 1 or t.shape[1] != c:
+                raise ValueError(f'conf_map_images: {name} must be (1, {c}, H, W), got {tuple(t.shape)}')
+            if t.device != inp.device:
+                raise ValueError(f'conf_map_images: {name} is on {t.device}, the input on {inp.device}')
+        h, w = maps[0].shape[2:]
+        if any(m.shape != maps[0].shape for m in maps):
+            raise ValueError(f'conf_map_images: the maps differ in shape: {[tuple(m.shape) for m in maps]}')
+        if not (isinstance(lut, torch.Tensor) and lut.dtype == torch.uint8 and lut.shape == (256, 3) and lut.is_contiguous()
+                and lut.device == inp.device):
+            raise ValueError('conf_map_images: lut must be a contiguous uint8 (256, 3) tensor on the frames\' device')
+        ih, iw, oh, ow = inp.shape[2], inp.shape[3], out.shape[2], out.shape[3]
+        need = conf_map_bytes(h, w, ih, iw, oh, ow, normalize)
+        ws = getattr(self, '_conf_ws', None)
+        if ws is None or ws[0].device != inp.device or ws[1].numel() < need:
+            ws = (torch.empty(CONF_MAP_WORK, dtype=torch.int32, device=inp.device), torch.empty(need, dtype=torch.uint8, device=inp.device))
+            self._conf_ws = ws
+        m = list(maps) + [None] * (4 - len(maps))
+        _check(self.lib, self.lib.rv_conf_map_images(_ptr(m[0]), _ptr(m[1]), _ptr(m[2]), _ptr(m[3]), h, w, int(normalize), _ptr(inp),
+                                                     ih, iw, _ptr(out), oh, ow, _ptr(lut), _ptr(ws[0]), _ptr(ws[1]), self._stream()),
+               'rv_conf_map_images')
+        return ws[1][:need]
