@@ -372,6 +372,22 @@ int rv_conf_map_images(const float* conf, const float* prop, const float* prop_b
                        int normalize, const float* inp, int ih, int iw, const float* out, int oh, int ow,
                        const uint8_t* lut_rgb, uint32_t* work, uint8_t* dst, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * rv_eval_images - the per-frame image bytes of the default evaluation mode (evaluation/eval_qual_quan.py:103-125): the
+ * input, the output and the ground truth, each as the uint8 BGR HWC image cv2.imwrite encodes from cv2.cvtColor(x * 255,
+ * cv2.COLOR_RGB2BGR).
+ *   frames     HOST array of nframes device pointers, each a contiguous fp32 NCHW (1, 3, H, W) RGB frame, 1 <= nframes <= 3
+ *   hw_host    HOST array of nframes x (H, W), each H, W >= 1 with H * W <= 2^28
+ *   dst        device uint8 of RV_EVAL_IMAGES_BYTES = sum of 3 * H * W bytes, packed without gaps: the frames' (H, W, 3) BGR
+ *              images in the order of `frames`
+ * A value x becomes cv::Mat::convertTo(CV_8U) of fl32(x * 255), exactly as rv_conf_map_images converts its frames (the same
+ * device function): round half to even, saturated to [0, 255]; NaN and values outside int32 become 0.
+ * One launch, no allocation.  16-byte loads and stores for a frame whose pointer and place in dst are 16-byte aligned and whose
+ * H * W is a multiple of 4; other frames convert pixel by pixel to the same bytes.
+ * RV_E_INVALID for any argument outside the above.
+ * ------------------------------------------------------------------------------------------------ */
+int rv_eval_images(const float* const* frames, const int* hw_host, int nframes, uint8_t* dst, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

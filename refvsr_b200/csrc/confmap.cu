@@ -5,8 +5,9 @@
 // order-preserving uint32 keys of its min and max and store the pair in `work`.  Launch 2 (images_kernel): every CTA owns 4 * NT consecutive pixels of one
 // image; a map CTA first folds its map's RED_BLK partials (so no CTA waits on another and nothing is initialised between
 // calls), then normalises with IEEE float32 operations, takes matplotlib's colormap index and looks the bytes up in the LUT;
-// a frame CTA scales by 255 and rounds like cv::Mat::convertTo(CV_8U).
+// a frame CTA scales by 255 and rounds like cv::Mat::convertTo(CV_8U) (rv::frame_bgr8, shared with rv_eval_images).
 #include "common.cuh"
+#include "frame_u8.cuh"
 
 namespace {
 
@@ -62,13 +63,6 @@ struct Segs {
   int nseg, nmaps, normalize;
 };
 
-// cv::Mat::convertTo(CV_8U) of a float: cvRound (round half to even) then saturation; x86's conversion turns NaN and values
-// outside int32 into INT_MIN, which saturates to 0
-__device__ __forceinline__ uint32_t cv_u8(float v) {
-  if (!(v > -2147483648.f && v < 2147483648.f)) return 0u;
-  return (uint32_t)rv::clampi(__float2int_rn(v), 0, 255);
-}
-
 __global__ void __launch_bounds__(NT) images_kernel(const Segs sg, const uint8_t* __restrict__ lut_rgb,
                                                     const uint32_t* __restrict__ work, uint8_t* __restrict__ dst) {
   __shared__ uint8_t lut[256 * 3];
@@ -113,11 +107,9 @@ __global__ void __launch_bounds__(NT) images_kernel(const Segs sg, const uint8_t
 #pragma unroll
     for (int j = 0; j < PPT; ++j) {
       if (p0 + j >= npix) break;
+      const uint32_t bgr = rv::frame_bgr8(plane[p0 + j], plane[(size_t)npix + p0 + j], plane[2 * (size_t)npix + p0 + j]);
 #pragma unroll
-      for (int c = 0; c < 3; ++c) {                 // BGR: channel 2 first
-        const uint32_t v = cv_u8(__fmul_rn(plane[(size_t)(2 - c) * npix + p0 + j], 255.f));
-        b[(3 * j + c) >> 2] |= v << (8 * ((3 * j + c) & 3));
-      }
+      for (int c = 0; c < 3; ++c) b[(3 * j + c) >> 2] |= ((bgr >> (8 * c)) & 0xffu) << (8 * ((3 * j + c) & 3));
     }
   }
 

@@ -4,15 +4,25 @@ image tree, re-organised so that the host loop no longer caps a fast network at 
   reference (per frame)                                              here
   ------------------------------------------------------------------ ----------------------------------------------------
   gc.collect() + torch.cuda.empty_cache()      (:59-60)              dropped (the engine allocates nothing per call)
-  output.cpu().numpy(), gt.cpu().numpy()       (:76-79, sync D2H)    pinned host buffers, non-blocking copies + an event
-  SSIM by skimage on the CPU, 1080p, 3 channels (:92, ~1 s)          same formula (uniform 7x7 window, sample covariance, valid
-                                                                     interior, mean over channels) in float64 on the device
+  output / gt / inp .cpu().numpy() as float32  (:76-79, :95)         one rv_eval_images call turns the frames to be written
+  and cv2.cvtColor(x * 255, RGB2BGR) per write (:103-125)            into the uint8 BGR images cv2.imwrite stores for them; one
+                                                                     non-blocking copy moves those bytes into pinned memory
+  SSIM by skimage on the CPU, 1080p, 3 channels (:92, ~1 s)          one rv_region_metrics call: skimage's full-frame SSIM map
+                                                                     summed over the interior it averages (3 pixels in from
+                                                                     every edge) and the 3 channels
   6 x cv2.imwrite (png + jpg of input / output / gt) (:103-125)      same files, written by a small thread pool after the
-                                                                     frame's D2H event; the loop never waits for the encoder
-  errs['PSNR'].item() right after the forward  (:84)                 read together with the SSIM value, one sync per frame
+                                                                     frame's copy event; the loop never waits for the encoder
+  errs['PSNR'].item() right after the forward  (:84)                 read after the SSIM sums, one sync per frame
 
-`REFVSR_DROPIN_EVAL=0` restores the reference's own loop (A/B measurements).  flag_HD_in (8K) models keep the reference's CPU SSIM
-on the cv2-resized output (:86-89) - that path is rarely evaluated quantitatively and is kept bit-compatible instead."""
+Every written image takes the device path: input / output / gt in png and jpg, the gradio branch's single png, and the
+flag_HD_in (HD -> 8K) models' 4320x7680 outputs, whose 8-bit image is a quarter of the float32 frame.  Without CUDA (`-cpu`) the
+frames are copied back as float32, scored by the reference's `ssim` and written as the reference writes them.
+
+flag_HD_in models keep the reference's quantitative branch (:86-89, the CPU SSIM of the cv2-resized output), but the reference's
+own Trainer.evaluation cannot compute their PSNR: it subtracts the 1080p ground truth from the 8K output, which does not broadcast.
+These models run with --qualitative_only, as the reference's scripts_eval/eval_*8K.sh do.
+
+`REFVSR_DROPIN_EVAL=0` restores the reference's own loop (A/B measurements)."""
 import importlib.util
 import os
 import sys
@@ -23,7 +33,8 @@ from pathlib import Path
 import cv2
 import numpy as np
 import torch
-import torch.nn.functional as F
+
+from refvsr_b200 import lib as rv_lib
 
 from . import REFERENCE_DIR
 from .init import init
@@ -39,19 +50,18 @@ def _reference_impl():
     return mod.eval_qual_quan
 
 
-def ssim_device(a, b, data_range=1.0, win=7):
-    """skimage.metrics.structural_similarity(a, b, data_range=1.0, multichannel=True) for (1, 3, H, W) tensors in [0, 1]:
-    uniform win x win filter, sample covariance (NP / (NP - 1)), mean over the valid interior and the channels; float64."""
-    a, b = a.double(), b.double()
-    K1, K2 = 0.01, 0.03
-    NP = win * win
-    cov_norm = NP / (NP - 1.0)
-    ux, uy = F.avg_pool2d(a, win, 1), F.avg_pool2d(b, win, 1)             # = the valid interior of the uniform filter
-    uxx, uyy, uxy = F.avg_pool2d(a * a, win, 1), F.avg_pool2d(b * b, win, 1), F.avg_pool2d(a * b, win, 1)
-    vx, vy, vxy = cov_norm * (uxx - ux * ux), cov_norm * (uyy - uy * uy), cov_norm * (uxy - ux * uy)
-    C1, C2 = (K1 * data_range) ** 2, (K2 * data_range) ** 2
-    S = ((2 * ux * uy + C1) * (2 * vxy + C2)) / ((ux ** 2 + uy ** 2 + C1) * (vx + vy + C2))
-    return S.mean(dim=(2, 3)).mean()
+def split_images(buf, hws):
+    """(H, W, 3) views of a packed rv_eval_images or rv_conf_map_images buffer (flat uint8 numpy array), one per (H, W)"""
+    views, off = [], 0
+    for h, w in hws:
+        views.append(buf[off:off + 3 * h * w].reshape(h, w, 3))
+        off += 3 * h * w
+    return views
+
+
+def _host_float(t):
+    """(1, 3, H, W) tensor -> (H, W, 3) float32 numpy array, as the reference copies a frame back"""
+    return t[0].permute(1, 2, 0).float().cpu().numpy().copy()
 
 
 def _write_images(job):
@@ -80,18 +90,8 @@ def eval_qual_quan(config):
     pool = ThreadPoolExecutor(max_workers=int(os.environ.get('REFVSR_EVAL_WRITERS', '4')))
     pending = []
     cuda = torch.cuda.is_available() and getattr(config, 'cuda', False)
-    ring = {}                                             # pinned host buffers, two per image kind (frame k-1 may still be encoding)
-
-    def to_host(t, key, k):
-        """(1, 3, H, W) device tensor -> (H, W, 3) float32 numpy view of a pinned buffer (async), or a plain copy on CPU"""
-        hwc = t[0].permute(1, 2, 0)
-        if not cuda:
-            return hwc.float().cpu().numpy().copy()
-        slot = (key, k % 3, tuple(hwc.shape))
-        if slot not in ring:
-            ring[slot] = torch.empty(tuple(hwc.shape), dtype=torch.float32).pin_memory()
-        ring[slot].copy_(hwc, non_blocking=True)
-        return ring[slot].numpy()
+    ops = rv_lib.CudaOps() if cuda else None
+    ring = {}                                             # pinned host buffers, three per size (two frames may still be encoding)
 
     for i, inputs in enumerate(model.data_loader_eval):
         is_first_frame = inputs['is_first'][0].item()
@@ -110,7 +110,7 @@ def eval_qual_quan(config):
                 line = '[MEAN EVAL {}|{}|{}][{}/{}] PSNR: {:.5f} SSIM: {:.5f} ({:.5f}sec)\n\n'.format(
                     config.mode, config.EVAL.data, inputs['video_name'][0], inputs['video_idx'][0], inputs['video_len'][0], PSNR_mean,
                     SSIM_mean, total_itr_time_video)
-                print(line, end='')
+                print(line)
                 if not config.EVAL.qualitative_only:
                     with open(score_path, 'a') as file:
                         file.write(line)
@@ -125,31 +125,34 @@ def eval_qual_quan(config):
             except Exception:                                               # noqa: BLE001  (the reference's own fallback, :70-74)
                 inp, output = outs['LR_UW'], outs['SR_UW']
             gt = outs['HR_UW']
-            PSNR = SSIM = 0
-            ssim_t = None
-            if not config.EVAL.qualitative_only and ('SR_UW_png' in outs.keys() or 'SR_UW' in outs.keys()):
-                if not config.flag_HD_in:
-                    ssim_t = ssim_device(output.float(), gt.float())
         want_images = not config.EVAL.quantitative_only
-        out_np = gt_np = inp_np = None
-        ev = None
-        if want_images or (config.flag_HD_in and not config.EVAL.qualitative_only):
-            out_np = to_host(output.float(), 'out', i)
-            gt_np = to_host(gt.float(), 'gt', i)
-            if want_images and config.EVAL.is_gradio is False:
-                inp_np = to_host(inp.float(), 'inp', i)
+        has_gt_images = 'gt' in inputs.keys()
+        arrays = ev = None
+        if want_images:                                   # the frames written, in the order of their paths below
+            frames = [inp, output] + ([gt] if has_gt_images else []) if config.EVAL.is_gradio is False else [output]
             if cuda:
+                frames = [f.float().contiguous() for f in frames]
+                packed = ops.eval_images(frames)
+                slot = (total_norm % 3, packed.numel())
+                if slot not in ring:
+                    ring[slot] = torch.empty(packed.numel(), dtype=torch.uint8).pin_memory()
+                ring[slot].copy_(packed, non_blocking=True)
                 ev = torch.cuda.Event()
                 ev.record()
+                arrays = split_images(ring[slot].numpy(), [tuple(f.shape[2:]) for f in frames])
+            else:
+                arrays = [_host_float(f) for f in frames]
+        PSNR = SSIM = 0
         if not config.EVAL.qualitative_only and ('SR_UW_png' in outs.keys() or 'SR_UW' in outs.keys()):
-            PSNR = errs['PSNR'].item()                                        # the frame's one host sync
-            if ssim_t is not None:
-                SSIM = float(ssim_t.item())
-            else:                                                             # flag_HD_in: the reference's CPU path (:86-92)
-                if ev is not None:
-                    ev.synchronize()
-                o_ = cv2.resize(out_np, dsize=(0, 0), fx=1 / config.scale, fy=1 / config.scale, interpolation=cv2.INTER_CUBIC)
-                SSIM = ssim_cpu(o_, gt_np)
+            if config.flag_HD_in:                                             # the reference's CPU path (:86-92)
+                o_ = cv2.resize(_host_float(output), dsize=(0, 0), fx=1 / config.scale, fy=1 / config.scale,
+                                interpolation=cv2.INTER_CUBIC)
+                SSIM = ssim_cpu(o_, _host_float(gt))
+            elif cuda:
+                SSIM = ops.mean_ssim(output.float().contiguous(), gt.float().contiguous())   # the frame's one host sync
+            else:
+                SSIM = ssim_cpu(_host_float(output), _host_float(gt))
+            PSNR = errs['PSNR'].item()
         elif cuda:
             torch.cuda.current_stream().synchronize()
         itr_time = time.time() - init_time
@@ -168,18 +171,11 @@ def eval_qual_quan(config):
             frame_name_no_ext = frame_name.split('.')[0]
             vid = inputs['video_name'][0]
             if config.EVAL.is_gradio is False:
-                arrays, paths = [inp_np, out_np], [[], []]
-                if 'gt' in inputs.keys():
-                    arrays.append(gt_np)
-                    paths.append([])
-                for iformat in ['png', 'jpg']:
-                    root = os.path.join(save_path_root_deblur, iformat)
-                    paths[0].append(os.path.join(root, 'input', vid, '{}.{}'.format(frame_name_no_ext, iformat)))
-                    paths[1].append(os.path.join(root, 'output', vid, '{}.{}'.format(frame_name_no_ext, iformat)))
-                    if 'gt' in inputs.keys():
-                        paths[2].append(os.path.join(root, 'gt', vid, '{}.{}'.format(frame_name_no_ext, iformat)))
+                dirs = ['input', 'output'] + (['gt'] if has_gt_images else [])
+                paths = [[os.path.join(save_path_root_deblur, iformat, d, vid, '{}.{}'.format(frame_name_no_ext, iformat))
+                          for iformat in ('png', 'jpg')] for d in dirs]
             else:
-                arrays, paths = [out_np], [[os.path.join(save_path_root_deblur, '{}.png'.format(frame_name_no_ext))]]
+                paths = [[os.path.join(save_path_root_deblur, '{}.png'.format(frame_name_no_ext))]]
             pending.append(pool.submit(_write_images, (ev, arrays, paths)))
             while len(pending) > 2:                       # a pinned slot is reused every third frame: keep the queue short
                 pending.pop(0).result()

@@ -22,7 +22,7 @@ from refvsr_b200 import lib as rv_lib
 from refvsr_b200.colormap import inferno_lut
 
 from . import REFERENCE_DIR
-from .eval_qual_quan import _write_images
+from .eval_qual_quan import _write_images, split_images
 from .init import init
 
 # eval_vis keys and image directories of the maps, in the order of rv_conf_map_images' packed buffer
@@ -39,17 +39,9 @@ def _reference_impl():
     return mod.eval_quan_conf_map
 
 
-def split_images(buf, map_hw, n_maps, inp_hw, out_hw):
-    """views of a packed rv_conf_map_images buffer (flat uint8 numpy array): n_maps (h, w, 3) maps, the input, the output"""
-    views, off = [], 0
-    for h, w in [map_hw] * n_maps + [inp_hw, out_hw]:
-        views.append(buf[off:off + 3 * h * w].reshape(h, w, 3))
-        off += 3 * h * w
-    return views
-
-
 def frame_images(ops, outs, vis):
-    """one frame's packed image bytes (a uint8 tensor on the frames' device) and the directory of each image, in buffer order"""
+    """one frame's packed image bytes (a uint8 tensor on the frames' device), the (h, w) and the directory of each image, in
+    buffer order"""
     normalize = 'conf_map_prop' in vis.keys()
     keys = MAP_KEYS if normalize else MAP_KEYS[:1]
     try:
@@ -59,7 +51,7 @@ def frame_images(ops, outs, vis):
     maps = [vis[k].float().contiguous() for k in keys]
     inp, output = inp.float().contiguous(), output.float().contiguous()
     packed = ops.conf_map_images(maps, inp, output, inferno_lut(inp.device), normalize)
-    shapes = (tuple(maps[0].shape[2:]), len(maps), tuple(inp.shape[2:]), tuple(output.shape[2:]))
+    shapes = [tuple(maps[0].shape[2:])] * len(maps) + [tuple(inp.shape[2:]), tuple(output.shape[2:])]
     return packed, shapes, MAP_DIRS[:len(keys)] + ('input', 'output')
 
 
@@ -127,7 +119,7 @@ def eval_quan_conf_map(config):
         vid = inputs['video_name'][0]
         paths = [[os.path.join(save_path_root_deblur, iformat, d, vid, '{}.{}'.format(frame_name_no_ext, iformat))
                   for iformat in ('png', 'jpg')] for d in dirs]
-        pending.append(pool.submit(_write_images, (ev, split_images(host, *shapes), paths)))
+        pending.append(pool.submit(_write_images, (ev, split_images(host, shapes), paths)))
         while len(pending) > 2:                           # a pinned slot is reused every third frame: keep the queue short
             pending.pop(0).result()
 

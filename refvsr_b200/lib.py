@@ -100,6 +100,7 @@ SIGNATURES = {
     'rv_reconstruct': (_I, [_P, _I, _I, _P, _I, _I, _I, _I, _P, _P]),
     'rv_region_metrics': (_I, [_P, _P, _I, _I, C.POINTER(C.c_int32), _I, _P, _P, _P]),
     'rv_conf_map_images': (_I, [_P, _P, _P, _P, _I, _I, _I, _P, _I, _I, _P, _I, _I, _P, _P, _P, _P]),
+    'rv_eval_images': (_I, [C.POINTER(C.c_void_p), C.POINTER(C.c_int), _I, _P, _P]),
 }
 
 CONF_MAP_WORK = 512                 # RV_CONF_MAP_WORK
@@ -451,6 +452,14 @@ class CudaOps:
         host = ws[1][:2 * n].cpu().numpy()
         return host[:n], host[n:]
 
+    def mean_ssim(self, a, b):
+        """skimage.metrics.structural_similarity(a, b, data_range=1.0, multichannel=True) of two contiguous fp32 (1, 3, H, W) CUDA
+        images, H, W >= 7.  skimage averages its full-frame SSIM map over the interior 3 pixels in from every edge and over the
+        channels, so this is one region_metrics call with the single box (3, H - 3, 3, W - 3).  Synchronises the current stream."""
+        H, W = a.shape[-2], a.shape[-1]
+        _, s = self.region_metrics(a, b, [(3, H - 3, 3, W - 3)])
+        return float(s[0] / (3 * (H - 6) * (W - 6)))
+
     def conf_map_images(self, maps, inp, out, lut, normalize):
         """The image bytes of one frame of the confidence-map evaluation mode (rv_conf_map_images).
         maps: [conf_map, conf_map_prop, conf_map_prop_backward, conf_map_prop_forward] with normalize, [conf_map] without;
@@ -485,3 +494,28 @@ class CudaOps:
                                                      ih, iw, _ptr(out), oh, ow, _ptr(lut), _ptr(ws[0]), _ptr(ws[1]), self._stream()),
                'rv_conf_map_images')
         return ws[1][:need]
+
+    def eval_images(self, frames):
+        """The image bytes of one frame of the default evaluation mode (rv_eval_images).  frames: 1 to 3 contiguous float32
+        (1, 3, H, W) RGB CUDA tensors on one device (the input, the output, the ground truth; sizes may differ).  Returns a uint8
+        CUDA tensor of sum(3 * H * W) bytes: each frame's BGR HWC image as cv2.imwrite stores cv2.cvtColor(x * 255, RGB2BGR),
+        packed in the order given.  The tensor is a view of a buffer this object reuses: the next call on the stream overwrites it."""
+        if not 1 <= len(frames) <= 3:
+            raise ValueError(f'eval_images: 1 to 3 frames, got {len(frames)}')
+        for k, t in enumerate(frames):
+            if not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous():
+                raise ValueError(f'eval_images: frames[{k}] must be a contiguous float32 CUDA tensor')
+            if t.dim() != 4 or t.shape[0] != 1 or t.shape[1] != 3:
+                raise ValueError(f'eval_images: frames[{k}] must be (1, 3, H, W), got {tuple(t.shape)}')
+            if t.device != frames[0].device:
+                raise ValueError(f'eval_images: frames[{k}] is on {t.device}, frames[0] on {frames[0].device}')
+        hw = [int(v) for t in frames for v in t.shape[2:]]
+        need = sum(3 * t.shape[2] * t.shape[3] for t in frames)
+        buf = getattr(self, '_eval_images_buf', None)
+        if buf is None or buf.device != frames[0].device or buf.numel() < need:
+            buf = torch.empty(need, dtype=torch.uint8, device=frames[0].device)
+            self._eval_images_buf = buf
+        ptrs = (C.c_void_p * len(frames))(*[t.data_ptr() for t in frames])
+        _check(self.lib, self.lib.rv_eval_images(ptrs, (C.c_int * len(hw))(*hw), len(frames), _ptr(buf), self._stream()),
+               'rv_eval_images')
+        return buf[:need]
