@@ -324,6 +324,29 @@ int rv_reconstruct(const void* x, int xc, int x_dtype, const float* lr_nchw, int
                    int clamp01, float* out_nchw, void* stream);
 int rv_reconstruct_batched(const void* x, int xc, int x_dtype, const float* lr_nchw, int h, int w, int scale,
                            int clamp01, float* out_nchw, int n, void* stream);   /* see rv_warp_batched */
+/* The same reconstruction with 8-bit output: each value the matching rv_reconstruct{,_batched} call writes becomes the byte
+ * cv::Mat::convertTo(CV_8U) makes of fl32(v * 255) (csrc/frame_u8.cuh: round half to even, saturated; NaN -> 0), stored HWC
+ * (scale*h, scale*w, 3), images packed one after the other for n > 1.  bgr = 0: R, G, B bytes per pixel; 1: B, G, R (cv2's
+ * order).  The kernel is chosen as rv_reconstruct chooses its own (x4 / x2 fast paths for fp32 x with xc = 4, the generic kernel
+ * otherwise), and computes each value with that kernel's expressions.  16-byte stores of 16-pixel row runs where out is
+ * 16-byte aligned and a row is a multiple of 16 bytes; byte stores elsewhere, to the same bytes. */
+int rv_reconstruct_u8(const void* x, int xc, int x_dtype, const float* lr_nchw, int h, int w, int scale, int clamp01, int bgr,
+                      uint8_t* out_hwc, void* stream);
+int rv_reconstruct_u8_batched(const void* x, int xc, int x_dtype, const float* lr_nchw, int h, int w, int scale, int clamp01,
+                              int bgr, uint8_t* out_hwc, int n, void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * rv_frames_from_u8 - decoded 8-bit video frames into the engine's fp32 frames (data_loader/utils.py::read_frame's
+ * np.array(frame) / 255. cast to float32).
+ *   src    HOST array of k device pointers, each a contiguous uint8 (h, w, 3) HWC frame, any alignment; bgr = 1: the bytes of a
+ *          pixel are B, G, R (cv2's order), 0: R, G, B
+ *   dst    HOST array of k device pointers, each a contiguous fp32 (3, h, w) planar RGB frame
+ *   1 <= k <= 16, h, w >= 1, h * w <= 2^28
+ * Byte u becomes fl32(u / 255) with IEEE division (round to nearest).  One launch; 16-byte loads wherever a frame has 16-byte
+ * aligned runs of 16 pixels (every frame but at most 30 pixels of it), 16-byte stores where dst allows.
+ * RV_E_INVALID for any argument outside the above.
+ * ------------------------------------------------------------------------------------------------ */
+int rv_frames_from_u8(const uint8_t* const* src, float* const* dst, int k, int h, int w, int bgr, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * rv_region_metrics - the per-frame sums behind the FOV evaluation mode: evaluation/metrics.py:18-31 (psnr, psnr_masked,

@@ -6,6 +6,7 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "frame_u8.cuh"
 
 namespace rv {
 
@@ -1152,6 +1153,202 @@ __global__ void __launch_bounds__(128) reconstruct2_kernel(const float4* __restr
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// 8-bit HWC output of the reconstruction tail (rv_reconstruct_u8): one variant per fp32 kernel above, each computing the same
+// fp32 value with the same expressions before rv::frame_u8 turns it into a byte.  A thread owns 16 consecutive output pixels of
+// a row (48 bytes) and writes them as three 16-byte stores where the row and the buffer allow it (vec), byte by byte elsewhere.
+// BGR: the pixel's bytes are B, G, R instead of R, G, B.
+// ---------------------------------------------------------------------------------------------
+template <bool BGR>
+__device__ __forceinline__ void put_u8(uint32_t* words, int j, int c, float v) {   // j: pixel of the run, c: R, G, B
+  const int i = 3 * j + (BGR ? 2 - c : c);
+  words[i >> 2] |= frame_u8(v) << (8 * (i & 3));
+}
+
+__device__ __forceinline__ void store_run(uint8_t* o, const uint32_t* words, int nbytes, bool vec) {
+  if (vec && nbytes == 48) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k)
+      reinterpret_cast<uint4*>(o)[k] = make_uint4(words[4 * k], words[4 * k + 1], words[4 * k + 2], words[4 * k + 3]);
+  } else {
+#pragma unroll
+    for (int i = 0; i < 48; ++i)
+      if (i < nbytes) o[i] = (uint8_t)(words[i >> 2] >> (8 * (i & 3)));
+  }
+}
+
+// x4: reconstruct4_kernel's arithmetic for 4 neighbouring LR pixels per thread -> 4 output rows of 16 pixels
+template <bool BGR>
+__global__ void __launch_bounds__(128) reconstruct4_u8_kernel(const float4* __restrict__ x, const float* __restrict__ lr, int h, int w,
+                                                              int clamp01, int vec, uint8_t* __restrict__ out) {
+  x += (size_t)blockIdx.z * 16 * h * w;
+  lr += (size_t)blockIdx.z * 3 * h * w;
+  out += (size_t)blockIdx.z * 48 * h * w;
+  const int wq = (w + 3) / 4;
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= h * wq) return;
+  const int ly = q / wq, lx0 = 4 * (q - ly * wq);
+  const int nk = min(4, w - lx0);
+  const int Wo = 4 * w;
+  float wt[4][4];
+#pragma unroll
+  for (int a = 0; a < 4; ++a) {
+    const float r = 0.25f * ((float)a + 0.5f) - 0.5f;
+    cubic_weights(r - floorf(r), wt[a]);
+  }
+  uint32_t ob[4][12] = {};                                     // [output row a][little-endian byte words of the 16-pixel run]
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    if (k >= nk) break;
+    const int lx = lx0 + k;
+    int ry[5], rx[5];
+#pragma unroll
+    for (int i = 0; i < 5; ++i) { ry[i] = clampi(ly - 2 + i, 0, h - 1); rx[i] = clampi(lx - 2 + i, 0, w - 1); }
+    float res[3][4][4];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const float* s = lr + (size_t)c * h * w;
+      float hrow[4][5];
+#pragma unroll
+      for (int i = 0; i < 5; ++i) {
+        const float* r = s + (size_t)ry[i] * w;
+        const float v0 = __ldg(r + rx[0]), v1 = __ldg(r + rx[1]), v2 = __ldg(r + rx[2]), v3 = __ldg(r + rx[3]), v4 = __ldg(r + rx[4]);
+#pragma unroll
+        for (int b = 0; b < 4; ++b) {
+          hrow[b][i] = (b < 2) ? (wt[b][0] * v0 + wt[b][1] * v1 + wt[b][2] * v2 + wt[b][3] * v3)
+                               : (wt[b][0] * v1 + wt[b][1] * v2 + wt[b][2] * v3 + wt[b][3] * v4);
+        }
+      }
+#pragma unroll
+      for (int a = 0; a < 4; ++a) {
+        const int r0 = (a < 2) ? 0 : 1;
+#pragma unroll
+        for (int b = 0; b < 4; ++b) {
+          float acc = 0.f;
+#pragma unroll
+          for (int j = 0; j < 4; ++j) acc += wt[a][j] * hrow[b][r0 + j];
+          res[c][a][b] = fminf(fmaxf(acc, 0.f), 1.f);
+        }
+      }
+    }
+#pragma unroll
+    for (int a = 0; a < 4; ++a) {
+      const size_t row = (size_t)(4 * ly + a) * Wo + 4 * lx;
+#pragma unroll
+      for (int b = 0; b < 4; ++b) {
+        const float4 xv = __ldg(x + row + b);
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+          const float xr = (c == 0) ? xv.x : (c == 1 ? xv.y : xv.z);
+          float v = xr + res[c][a][b];
+          if (clamp01) v = fminf(fmaxf(v, 0.f), 1.f);
+          put_u8<BGR>(ob[a], 4 * k + b, c, v);
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int a = 0; a < 4; ++a) store_run(out + 3 * ((size_t)(4 * ly + a) * Wo + 4 * lx0), ob[a], 12 * nk, vec);
+}
+
+// x2: reconstruct2_kernel's arithmetic for 8 neighbouring LR pixels per thread -> 2 output rows of 16 pixels
+template <bool BGR>
+__global__ void __launch_bounds__(128) reconstruct2_u8_kernel(const float4* __restrict__ x, const float* __restrict__ lr, int h, int w,
+                                                              int clamp01, int vec, uint8_t* __restrict__ out) {
+  x += (size_t)blockIdx.z * 4 * h * w;
+  lr += (size_t)blockIdx.z * 3 * h * w;
+  out += (size_t)blockIdx.z * 12 * h * w;
+  const int wq = (w + 7) / 8;
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= h * wq) return;
+  const int ly = q / wq, lx0 = 8 * (q - ly * wq);
+  const int nk = min(8, w - lx0);
+  const int Wo = 2 * w;
+  float wt[2][4];
+#pragma unroll
+  for (int a = 0; a < 2; ++a) {
+    const float r = 0.5f * ((float)a + 0.5f) - 0.5f;
+    cubic_weights(r - floorf(r), wt[a]);
+  }
+  uint32_t ob[2][12] = {};
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    if (k >= nk) break;
+    const int lx = lx0 + k;
+    int ry[5], rx[5];
+#pragma unroll
+    for (int i = 0; i < 5; ++i) { ry[i] = clampi(ly - 2 + i, 0, h - 1); rx[i] = clampi(lx - 2 + i, 0, w - 1); }
+    float res[3][2][2];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const float* s = lr + (size_t)c * h * w;
+      float hrow[2][5];
+#pragma unroll
+      for (int i = 0; i < 5; ++i) {
+        const float* r = s + (size_t)ry[i] * w;
+        const float v0 = __ldg(r + rx[0]), v1 = __ldg(r + rx[1]), v2 = __ldg(r + rx[2]), v3 = __ldg(r + rx[3]), v4 = __ldg(r + rx[4]);
+        hrow[0][i] = row4(wt[0], v0, v1, v2, v3);
+        hrow[1][i] = row4(wt[1], v1, v2, v3, v4);
+      }
+#pragma unroll
+      for (int a = 0; a < 2; ++a) {
+#pragma unroll
+        for (int b = 0; b < 2; ++b) {
+          float acc = 0.f;
+#pragma unroll
+          for (int j = 0; j < 4; ++j) acc = __fmaf_rn(wt[a][j], hrow[b][a + j], acc);
+          res[c][a][b] = fminf(fmaxf(acc, 0.f), 1.f);
+        }
+      }
+    }
+#pragma unroll
+    for (int a = 0; a < 2; ++a) {
+      const size_t row = (size_t)(2 * ly + a) * Wo + 2 * lx;
+      const float4 x0 = __ldg(x + row), x1 = __ldg(x + row + 1);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        float v0 = ((c == 0) ? x0.x : (c == 1 ? x0.y : x0.z)) + res[c][a][0];
+        float v1 = ((c == 0) ? x1.x : (c == 1 ? x1.y : x1.z)) + res[c][a][1];
+        if (clamp01) { v0 = fminf(fmaxf(v0, 0.f), 1.f); v1 = fminf(fmaxf(v1, 0.f), 1.f); }
+        put_u8<BGR>(ob[a], 2 * k, c, v0);
+        put_u8<BGR>(ob[a], 2 * k + 1, c, v1);
+      }
+    }
+  }
+#pragma unroll
+  for (int a = 0; a < 2; ++a) store_run(out + 3 * ((size_t)(2 * ly + a) * Wo + 2 * lx0), ob[a], 6 * nk, vec);
+}
+
+// any scale, x dtype and channel count: reconstruct_kernel's arithmetic for 16 consecutive output pixels (row-major) per thread
+template <typename T, bool BGR>
+__global__ void __launch_bounds__(256) reconstruct_u8_kernel(const T* __restrict__ x, int xc, const float* __restrict__ lr, int h, int w,
+                                                             int scale, int clamp01, int vec, uint8_t* __restrict__ out) {
+  const int Ho = scale * h, Wo = scale * w;
+  x += (size_t)blockIdx.z * Ho * Wo * xc;
+  lr += (size_t)blockIdx.z * 3 * h * w;
+  out += (size_t)blockIdx.z * 3 * Ho * Wo;
+  const int p0 = (blockIdx.x * blockDim.x + threadIdx.x) * 16;
+  if (p0 >= Ho * Wo) return;
+  const int n = min(16, Ho * Wo - p0);
+  const float inv = 1.0f / (float)scale;
+  uint32_t ob[12] = {};
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    if (j >= n) break;
+    const int p = p0 + j;
+    const int Y = p / Wo, X = p % Wo;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      float base = bicubic_planar(lr + (size_t)c * h * w, h, w, Y, X, inv);
+      base = fminf(fmaxf(base, 0.f), 1.f);
+      float v = to_f(x[(size_t)p * xc + c]) + base;
+      if (clamp01) v = fminf(fmaxf(v, 0.f), 1.f);
+      put_u8<BGR>(ob, j, c, v);
+    }
+  }
+  store_run(out + 3 * (size_t)p0, ob, 3 * n, vec);
+}
+
 }  // namespace rv
 
 // =================================================================================================
@@ -1482,4 +1679,41 @@ extern "C" int rv_reconstruct_batched(const void* x, int xc, int x_dtype, const 
 extern "C" int rv_reconstruct(const void* x, int xc, int x_dtype, const float* lr, int h, int w,
                               int scale, int clamp01, float* out, void* stream) {
   return rv_reconstruct_batched(x, xc, x_dtype, lr, h, w, scale, clamp01, out, 1, stream);
+}
+
+extern "C" int rv_reconstruct_u8_batched(const void* x, int xc, int x_dtype, const float* lr, int h, int w, int scale, int clamp01,
+                                         int bgr, uint8_t* out, int nimg, void* stream) {
+  RV_REQUIRE(x && lr && out && h > 0 && w > 0 && xc >= 3 && (scale == 2 || scale == 4),
+             "rv_reconstruct_u8: bad arguments");
+  RV_REQUIRE(nimg >= 1 && nimg <= 65535, "rv_reconstruct_u8: n=%d images out of range", nimg);
+  RV_REQUIRE((long long)scale * h * scale * w <= (1ll << 30), "rv_reconstruct_u8: %d x %d output too large", scale * h, scale * w);
+  // the fp32 path's dispatch (rv_reconstruct_batched), so each output byte comes from the value that kernel writes
+  static const bool fast_ok = getenv("REFVSR_NO_FAST_POINTWISE") == nullptr;
+  const bool aligned = (uintptr_t)out % 16 == 0;
+  const int Wo = scale * w;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (fast_ok && scale == 4 && x_dtype == RV_F32 && xc == 4 && (uintptr_t)x % 16 == 0) {
+    const int vec = aligned && (3 * Wo) % 16 == 0;
+    const dim3 grid(cdiv((long long)h * ((w + 3) / 4), 128), 1, nimg);
+    if (bgr) reconstruct4_u8_kernel<true><<<grid, 128, 0, st>>>((const float4*)x, lr, h, w, clamp01, vec, out);
+    else reconstruct4_u8_kernel<false><<<grid, 128, 0, st>>>((const float4*)x, lr, h, w, clamp01, vec, out);
+  } else if (fast_ok && scale == 2 && x_dtype == RV_F32 && xc == 4 && (uintptr_t)x % 16 == 0) {
+    const int vec = aligned && (3 * Wo) % 16 == 0;
+    const dim3 grid(cdiv((long long)h * ((w + 7) / 8), 128), 1, nimg);
+    if (bgr) reconstruct2_u8_kernel<true><<<grid, 128, 0, st>>>((const float4*)x, lr, h, w, clamp01, vec, out);
+    else reconstruct2_u8_kernel<false><<<grid, 128, 0, st>>>((const float4*)x, lr, h, w, clamp01, vec, out);
+  } else {
+    const long long n = (long long)scale * h * Wo;
+    const int vec = aligned && (3 * n) % 16 == 0;
+    const dim3 grid(cdiv(cdiv(n, 16), 256), 1, nimg);
+    RV_DISPATCH_DTYPE(x_dtype, T, (bgr ? reconstruct_u8_kernel<T, true><<<grid, 256, 0, st>>>((const T*)x, xc, lr, h, w, scale, clamp01, vec, out)
+                                       : reconstruct_u8_kernel<T, false><<<grid, 256, 0, st>>>((const T*)x, xc, lr, h, w, scale, clamp01, vec, out)));
+  }
+  RV_LAUNCH_CHECK("reconstruct_u8");
+  return RV_OK;
+}
+
+extern "C" int rv_reconstruct_u8(const void* x, int xc, int x_dtype, const float* lr, int h, int w, int scale, int clamp01, int bgr,
+                                 uint8_t* out, void* stream) {
+  return rv_reconstruct_u8_batched(x, xc, x_dtype, lr, h, w, scale, clamp01, bgr, out, 1, stream);
 }

@@ -101,6 +101,9 @@ SIGNATURES = {
     'rv_region_metrics': (_I, [_P, _P, _I, _I, C.POINTER(C.c_int32), _I, _P, _P, _P]),
     'rv_conf_map_images': (_I, [_P, _P, _P, _P, _I, _I, _I, _P, _I, _I, _P, _I, _I, _P, _P, _P, _P]),
     'rv_eval_images': (_I, [C.POINTER(C.c_void_p), C.POINTER(C.c_int), _I, _P, _P]),
+    'rv_reconstruct_u8': (_I, [_P, _I, _I, _P, _I, _I, _I, _I, _I, _P, _P]),
+    'rv_reconstruct_u8_batched': (_I, [_P, _I, _I, _P, _I, _I, _I, _I, _I, _P, _I, _P]),
+    'rv_frames_from_u8': (_I, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), _I, _I, _I, _I, _P]),
 }
 
 CONF_MAP_WORK = 512                 # RV_CONF_MAP_WORK
@@ -424,6 +427,39 @@ class CudaOps:
         _check(self.lib, self.lib.rv_reconstruct(_ptr(x), x.shape[2], DTYPE_CODE[x.dtype], _ptr(lr), lr.shape[1],
                                                  lr.shape[2], scale, int(clamp01), _ptr(out), self._stream()),
                'rv_reconstruct')
+
+    def reconstruct_u8(self, x, lr, scale, clamp01, out, bgr):
+        """reconstruct() with 8-bit HWC output: out (scale*h, scale*w, 3) uint8, or (n, scale*h, scale*w, 3) for a batch, gets the
+        bytes frame_u8 makes of the values reconstruct() would write (rv_reconstruct_u8); bgr: B, G, R byte order"""
+        _chk_dev(x, lr, out)
+        assert out.dtype == torch.uint8 and out.shape[-1] == 3
+        if lr.dim() == 4:                          # a batch of n images: (n, ...) operands, one launch
+            assert x.shape[0] == out.shape[0] == lr.shape[0]
+            _check(self.lib, self.lib.rv_reconstruct_u8_batched(_ptr(x), x.shape[3], DTYPE_CODE[x.dtype], _ptr(lr), lr.shape[2],
+                                                                lr.shape[3], scale, int(clamp01), int(bool(bgr)), _ptr(out),
+                                                                lr.shape[0], self._stream()), 'rv_reconstruct_u8')
+            return
+        _check(self.lib, self.lib.rv_reconstruct_u8(_ptr(x), x.shape[2], DTYPE_CODE[x.dtype], _ptr(lr), lr.shape[1], lr.shape[2],
+                                                    scale, int(clamp01), int(bool(bgr)), _ptr(out), self._stream()),
+               'rv_reconstruct_u8')
+
+    # -- 8-bit frames -----------------------------------------------------------------------------
+    def frames_from_u8(self, srcs, dsts, bgr):
+        """srcs: contiguous uint8 (h, w, 3) frames (HWC; bgr: B, G, R byte order), dsts: as many contiguous float32 (3, h, w) frames,
+        all of one size on one device; dsts[i] = srcs[i] as RGB planes of fl32(u / 255) (rv_frames_from_u8, 16 frames per launch)"""
+        assert len(srcs) == len(dsts)
+        if not srcs:
+            return
+        h, w = srcs[0].shape[0], srcs[0].shape[1]
+        for s, d in zip(srcs, dsts):
+            _chk_dev(s, d)
+            assert s.dtype == torch.uint8 and tuple(s.shape) == (h, w, 3), f'frames_from_u8: source {tuple(s.shape)} {s.dtype}'
+            assert d.dtype == torch.float32 and tuple(d.shape) == (3, h, w), f'frames_from_u8: destination {tuple(d.shape)} {d.dtype}'
+        for i in range(0, len(srcs), 16):
+            ps = [s.data_ptr() for s in srcs[i:i + 16]]
+            pd = [d.data_ptr() for d in dsts[i:i + 16]]
+            _check(self.lib, self.lib.rv_frames_from_u8((C.c_void_p * len(ps))(*ps), (C.c_void_p * len(pd))(*pd), len(ps), h, w,
+                                                        int(bool(bgr)), self._stream()), 'rv_frames_from_u8')
 
     # -- evaluation metrics -----------------------------------------------------------------------
     def region_metrics(self, a, b, boxes):

@@ -23,6 +23,7 @@ confined to *how* results are obtained, never to what they are:
     (`b200_reuse_check='sync'`, one int32).
 """
 import collections
+import contextlib
 import os
 
 import torch
@@ -146,6 +147,7 @@ class Network(nn.Module):
         self._b = 0
         self._bn = 1                  # windows of the current call: ring slots and carried state are [bn][...] tensors
         self._bmode = False           # enqueueing the batched steps of a call: every scratch buffer has the batch dimension
+        self._u8 = None               # inside an 8-bit call (forward_u8 / push_frame_u8 / push_frames_u8): its bgr flag
         self.executed_kernels = 0     # kernels of librefvsr_b200.so actually executed (eager launches + graph nodes)
         self.register_load_state_dict_post_hook(lambda module, incompatible: module._invalidate())
 
@@ -579,6 +581,10 @@ class Network(nn.Module):
             hr = dec                                             # x2: no upsample2 (RefVSR.py:89-90,114-115)
         hr2 = self._conv('conv_hr', hr, None, self._buf('up.hr2', (s * h, s * w, C), dt), [(C, C)], act_pre=ACT_LRELU01)
         last = self._conv('conv_last', hr2, None, self._buf('up.last', (s * h, s * w, 4), torch.float32), [(C, C)])
+        if self._u8 is not None:                                 # the same values, written as 8-bit HWC bytes
+            out = self._buf('up.out8', (s * h, s * w, 3), torch.uint8)
+            self.ops.reconstruct_u8(last, lr_center, s, clamp01, out, self._u8)
+            return out
         out = self._buf('up.out', (3, s * h, s * w), torch.float32)
         self.ops.reconstruct(last, lr_center, s, clamp01, out)      # + bicubic x scale of the centre frame (RefVSR.py:288)
         return out
@@ -691,18 +697,32 @@ class Network(nn.Module):
         n, t, c, h, w = lrs.size()
         if c != 3 or refs.size(2) != 3 or refs.size(1) != t or refs.size(0) != n:
             raise ValueError(f'unexpected input shapes {tuple(lrs.shape)} / {tuple(refs.shape)}')
-        if refs.size(3) % 2 or refs.size(4) % 2:
+        self._check_sizes(h, w, refs.size(3), refs.size(4))
+        out, vis = self._call(lrs, refs, n, is_first_frame, is_log, is_train)
+        outs['result'] = out
+        if is_log and vis is not None:
+            outs['vis'].update(vis.get('vis', {}))
+            if _cget(self.config, 'save_sample', False) and 'eval_vis' in vis:
+                outs['eval_vis'] = vis['eval_vis']
+        return outs
+
+    def _check_sizes(self, h, w, hr, wr):
+        """the LR (h, w) / Ref (hr, wr) sizes the schedule computes what the reference computes for"""
+        if hr % 2 or wr % 2:
             raise ValueError('reference frames must have even height/width (2x2 avg-pool and 2x2 block '
                              'gather, attention.py:51,142-144; odd sizes take the reference\'s reflection-'
                              'padded unfold path, which is not implemented)')
-        if self.flag_HD_in and (h % 4 or w % 4 or refs.size(3) % 8 or refs.size(4) % 8):
+        if self.flag_HD_in and (h % 4 or w % 4 or hr % 8 or wr % 8):
             raise ValueError('flag_HD_in: LR height/width must be multiples of 4 and Ref height/width multiples of 8 '
                              '(4x4 / 8x8 alignment blocks on the 1/4-resolution matching grid, attention.py:142-154); '
-                             f'got LR {h}x{w}, Ref {refs.size(3)}x{refs.size(4)}')
-        if self.scale == 2 and (h % 2 or w % 2 or refs.size(3) % 4 or refs.size(4) % 4):
+                             f'got LR {h}x{w}, Ref {hr}x{wr}')
+        if self.scale == 2 and (h % 2 or w % 2 or hr % 4 or wr % 4):
             raise ValueError('scale=2: LR height/width must be even and Ref height/width multiples of 4 '
                              '(2x2 / 4x4 alignment blocks on the 1/2-resolution matching grid, attention.py:142-154); '
-                             f'got LR {h}x{w}, Ref {refs.size(3)}x{refs.size(4)}')
+                             f'got LR {h}x{w}, Ref {hr}x{wr}')
+
+    def _call(self, lrs, refs, n, is_first_frame, is_log, is_train):
+        """one call of n windows (forward / forward_u8) once its inputs are checked -> (result, vis)"""
         self._device = lrs.device
         if is_train and torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             # trainers/trainer.py:159-172 would call loss.backward() on the result: fail here, with a clear message
@@ -736,12 +756,7 @@ class Network(nn.Module):
             if is_first_frame:
                 self.frame_itr_num = 0
             self.frame_itr_num += 1
-        outs['result'] = out
-        if is_log and vis is not None:
-            outs['vis'].update(vis.get('vis', {}))
-            if _cget(self.config, 'save_sample', False) and 'eval_vis' in vis:
-                outs['eval_vis'] = vis['eval_vis']
-        return outs
+        return out, vis
 
     def _batchable(self, is_log, is_train):
         """n > 1 windows can share one schedule: an operator set that takes (n, ...) operands, and none of the per-element-only
@@ -750,13 +765,13 @@ class Network(nn.Module):
                 and not self.fuse_resblocks and self._ring_mod is None)
 
     def _push_state(self, b, lr, ref):
-        if lr.dim() != 3 or ref.dim() != 3 or lr.size(0) != 3 or ref.size(0) != 3:
+        if self._u8 is None and (lr.dim() != 3 or ref.dim() != 3 or lr.size(0) != 3 or ref.size(0) != 3):
             raise ValueError('push_frame takes one LR frame (3, h, w) and one Ref frame (3, hr, wr)')
         st = self._state.get(b)
         if st is None or not st.get('has_prev') or not self.reuse:
             raise RuntimeError('push_frame needs a previous forward() call (the first window of the clip) and b200_reuse=True')
         t, h, w, hr, wr = st['shape']
-        if tuple(lr.shape[1:]) != (h, w) or tuple(ref.shape[1:]) != (hr, wr) or lr.device != self._device:
+        if self._hw(lr) != (h, w) or self._hw(ref) != (hr, wr) or lr.device != self._device:
             raise ValueError(f'push_frame: frame shapes / device differ from the running stream {(h, w)} / {(hr, wr)} on {self._device}')
         return st
 
@@ -807,10 +822,66 @@ class Network(nn.Module):
         self.frame_itr_num += 1
         return out
 
+    # ---- 8-bit frames (no counterpart in the reference) ---------------------------------------------
+    # Video decoders hand out uint8 HWC frames and encoders take them back.  These entries accept and return such frames, so a
+    # caller converts nothing on the host: the entering frames go through rv_frames_from_u8 straight into the fp32 ring slots
+    # (byte u -> fl32(u / 255), the value forward() stages from u8.float() / 255), and the tail's rv_reconstruct_u8 writes the
+    # bytes of the fp32 result forward() returns (csrc/frame_u8.cuh).  The schedule, the stream state and the ring are forward()'s,
+    # so 8-bit and fp32 calls may be interleaved on one clip.
+
+    def forward_u8(self, lrs, refs, is_first_frame, bgr=False):
+        """forward() for 8-bit frames: lrs (n, t, h, w, 3), refs (n, t, hr, wr, 3), contiguous uint8 on the engine's device; bgr:
+        B, G, R byte order (cv2's) in and out.  -> (n, scale*h, scale*w, 3) uint8: frame_u8 of forward()['result'] for the frames
+        u8.float() / 255, as HWC bytes."""
+        self._check_u8('forward_u8', 'lrs', lrs, 5)
+        self._check_u8('forward_u8', 'refs', refs, 5)
+        n, t, h, w, _ = lrs.shape
+        if tuple(refs.shape[:2]) != (n, t):
+            raise ValueError(f'forward_u8: lrs {tuple(lrs.shape)} and refs {tuple(refs.shape)} differ in (n, t)')
+        self._check_sizes(h, w, refs.shape[2], refs.shape[3])
+        with self._frames_u8(bgr):
+            return self._call(lrs, refs, n, is_first_frame, False, False)[0]
+
+    def push_frame_u8(self, lr, ref, bgr=False, b=0):
+        """push_frame() for 8-bit frames: lr (h, w, 3), ref (hr, wr, 3) contiguous uint8 -> (scale*h, scale*w, 3) uint8"""
+        self._check_u8('push_frame_u8', 'lr', lr, 3)
+        self._check_u8('push_frame_u8', 'ref', ref, 3)
+        with self._frames_u8(bgr):
+            return self.push_frame(lr, ref, b)
+
+    def push_frames_u8(self, lrs, refs, bgr=False):
+        """push_frames() for 8-bit frames: lrs (n, h, w, 3), refs (n, hr, wr, 3) contiguous uint8 -> (n, scale*h, scale*w, 3) uint8"""
+        self._check_u8('push_frames_u8', 'lrs', lrs, 4)
+        self._check_u8('push_frames_u8', 'refs', refs, 4)
+        with self._frames_u8(bgr):
+            return self.push_frames(lrs, refs)
+
+    def _check_u8(self, fn, name, x, dims):
+        if not isinstance(x, torch.Tensor) or x.dtype != torch.uint8:
+            raise ValueError(f'{fn}: {name} must be a uint8 tensor, got {getattr(x, "dtype", type(x).__name__)}')
+        if x.dim() != dims or x.shape[-1] != 3:
+            raise ValueError(f'{fn}: {name} must be {dims}-d with the 3 channels last (HWC frames), got {tuple(x.shape)}')
+        if not x.is_contiguous():
+            raise ValueError(f'{fn}: {name} must be contiguous')
+        dev = next(self.parameters()).device
+        if x.device != dev:
+            raise ValueError(f'{fn}: {name} is on {x.device}, the engine on {dev}')
+
+    @contextlib.contextmanager
+    def _frames_u8(self, bgr):
+        self._u8 = bool(bgr)
+        try:
+            yield
+        finally:
+            self._u8 = None
+
+    def _hw(self, x):
+        """(h, w) of a frame or a stack of frames: (..., 3, h, w) fp32, or (..., h, w, 3) uint8 inside an 8-bit call"""
+        return tuple(x.shape[-2:]) if self._u8 is None else tuple(x.shape[-3:-1])
+
     def _is_fresh(self, b, lrs, refs, caller_first, is_train):
         """(state, fresh, shape) of batch element b's stream: fresh = its cached per-frame products cannot be reused"""
-        t, _, h, w = lrs.shape
-        hr, wr = refs.shape[2], refs.shape[3]
+        t, (h, w), (hr, wr) = lrs.shape[0], self._hw(lrs), self._hw(refs)
         self._b = b           # ring / state namespace of this batch element
 
         # stream bookkeeping for exact reuse: a caller-declared first frame starts a new stream; forced
@@ -825,8 +896,7 @@ class Network(nn.Module):
     def _batch_fresh(self, lrs, refs, caller_first):
         """_is_fresh for the n elements of a batched call; with b200_reuse_check='sync' the n reuse-guard verdicts are read back
         in ONE device-to-host copy (one host sync per call, not per element).  -> ([fresh per element], shape)"""
-        n, t, _, h, w = lrs.shape
-        hr, wr = refs.shape[3], refs.shape[4]
+        n, t, (h, w), (hr, wr) = lrs.shape[0], lrs.shape[1], self._hw(lrs), self._hw(refs)
         shape = (t, h, w, hr, wr)
         fresh, pending = [], []
         for b in range(n):
@@ -873,11 +943,15 @@ class Network(nn.Module):
 
         # stage the frames that entered the window into their ring slots (fp32 copies; outside any graph)
         st['staged'] = {a for a in st['staged'] if a >= a0}
-        for j in range(t):
-            if a0 + j not in st['staged']:
+        enter = [j for j in range(t) if a0 + j not in st['staged']]
+        if self._u8 is None:
+            for j in enter:
                 self._ring('lr32', a0 + j, t, (3, h, w)).copy_(lrs[j])
                 self._ring('ref32', a0 + j, t, (3, hr, wr)).copy_(refs[j])
-                st['staged'].add(a0 + j)
+        elif enter:                                   # 8-bit frames: converted straight into their slots, one launch per size
+            self.ops.frames_from_u8([lrs[j] for j in enter], [self._ring('lr32', a0 + j, t, (3, h, w)) for j in enter], self._u8)
+            self.ops.frames_from_u8([refs[j] for j in enter], [self._ring('ref32', a0 + j, t, (3, hr, wr)) for j in enter], self._u8)
+        st['staged'].update(a0 + j for j in enter)
 
         work = self._plan_products(st, a0, t, range_start)
         return st, a0, range_start, work
@@ -913,7 +987,7 @@ class Network(nn.Module):
         variant = 'first' if is_first_frame else 'steady'
         key = None
         if self._graph_ok(fresh, is_log, is_train, lrs):
-            key = (b, self._bn, shape, a0 % t, variant, tuple((k, a - a0) for k, a in work))
+            key = (b, self._bn, shape, a0 % t, variant, tuple((k, a - a0) for k, a in work), self._u8)
         out, vis = self._execute(key, lambda: self._run_window(b, st, a0, t, h, w, hr, wr, work, is_first_frame, range_start,
                                                                 is_log, is_train))
         st['has_prev'] = True
@@ -941,7 +1015,7 @@ class Network(nn.Module):
                 self._b = b
                 key = None
                 if self._graph_ok(fresh[b], False, False, lrs[b]):
-                    key = (b, self._bn, shape, a0 % t, variant, tuple((k, a - a0) for k, a in work))
+                    key = (b, self._bn, shape, a0 % t, variant, tuple((k, a - a0) for k, a in work), self._u8)
                 outs.append(self._execute(key, lambda: self._run_window(b, st, a0, t, h, w, hr, wr, work, is_first_frame, rs,
                                                                          False, False))[0])
                 st['has_prev'] = True
@@ -961,7 +1035,7 @@ class Network(nn.Module):
 
         key = None
         if self._graph_ok(fresh[0], False, False, lrs[0]):
-            key = ('batch', n, shape, a0 % t, variant, tuple((k, a - a0) for k, a in work))
+            key = ('batch', n, shape, a0 % t, variant, tuple((k, a - a0) for k, a in work), self._u8)
         self._bmode = True
         try:
             out, _ = self._execute(key, lambda: self._run_window(0, st0, a0, t, h, w, hr, wr, work, is_first_frame, range_start,
@@ -978,8 +1052,14 @@ class Network(nn.Module):
         returns the int32 device flag (non-zero = the window did NOT slide by one)."""
         flag = self._buf(f'reuse.flag{self._b}', (1,), torch.int32)
         a1 = st['a0'] + 1
-        lr32 = lrs if (lrs.dtype == torch.float32 and lrs.is_contiguous()) else lrs.float().contiguous()
-        rf32 = refs if (refs.dtype == torch.float32 and refs.is_contiguous()) else refs.float().contiguous()
+        if self._u8 is not None:          # 8-bit frames: their fp32 values (the conversion is one to one, so equal bytes <=> equal values)
+            lr32 = self._buf(f'reuse.lr32.{self._b}', (t - 1, 3, h, w), torch.float32)
+            rf32 = self._buf(f'reuse.ref32.{self._b}', (t - 1, 3, hr, wr), torch.float32)
+            self.ops.frames_from_u8([lrs[j] for j in range(t - 1)], [lr32[j] for j in range(t - 1)], self._u8)
+            self.ops.frames_from_u8([refs[j] for j in range(t - 1)], [rf32[j] for j in range(t - 1)], self._u8)
+        else:
+            lr32 = lrs if (lrs.dtype == torch.float32 and lrs.is_contiguous()) else lrs.float().contiguous()
+            rf32 = refs if (refs.dtype == torch.float32 and refs.is_contiguous()) else refs.float().contiguous()
         pairs = []
         for j in range(t - 1):
             pairs.append((lr32[j], self._ring('lr32', a1 + j, t, (3, h, w))))

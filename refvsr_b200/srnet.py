@@ -62,3 +62,17 @@ class SRNet(nn.Module):
         """push_frame for a batch of n streams: the entering frames (n, 3, h, w) / (n, 3, hr, wr) -> (n, 3, scale*h, scale*w), one
         batched window schedule; see Network.push_frames"""
         return self.Network.push_frames(lrs, refs)
+
+    def forward_u8(self, lrs, refs, is_first_frame=True, bgr=False):
+        """forward() for decoded 8-bit video: lrs (n, t, h, w, 3), refs (n, t, hr, wr, 3) contiguous uint8 HWC frames on the
+        engine's device (bgr: cv2's B, G, R order) -> (n, scale*h, scale*w, 3) uint8, the bytes cv2.imwrite would store for
+        forward()'s result on u8 / 255; see Network.forward_u8 (no counterpart in the reference)"""
+        return self.Network.forward_u8(lrs, refs, is_first_frame, bgr=bgr)
+
+    def push_frame_u8(self, lr, ref, bgr=False):
+        """push_frame() for 8-bit frames: lr (h, w, 3), ref (hr, wr, 3) uint8 -> (scale*h, scale*w, 3) uint8"""
+        return self.Network.push_frame_u8(lr, ref, bgr=bgr)
+
+    def push_frames_u8(self, lrs, refs, bgr=False):
+        """push_frames() for 8-bit frames: lrs (n, h, w, 3), refs (n, hr, wr, 3) uint8 -> (n, scale*h, scale*w, 3) uint8"""
+        return self.Network.push_frames_u8(lrs, refs, bgr=bgr)
