@@ -1521,6 +1521,7 @@ extern "C" int rv_gather_blocks(const void* value, int Hv, int Wv, int C, int dt
   const uint8_t* v = (const uint8_t*)value;
   uint8_t* o = (uint8_t*)out;
   bool a16 = ((uintptr_t)value % 16 == 0) && ((uintptr_t)out % 16 == 0);
+  bool a4 = ((uintptr_t)value % 4 == 0) && ((uintptr_t)out % 4 == 0);   // 4-byte words need 4-byte aligned rows
   static const bool fast_ok = getenv("REFVSR_NO_FAST_POINTWISE") == nullptr;
   if (fast_ok && rowbytes % 16 == 0 && a16 && (ks == 1 || ks == 2 || ks == 4) && hq <= 65535) {
     const int nv = rowbytes / 16;
@@ -1538,7 +1539,7 @@ extern "C" int rv_gather_blocks(const void* value, int Hv, int Wv, int C, int dt
     else gather_cells_kernel<1, 0><<<grid, 256, 0, st>>>(v4, Wv, nv, idx, wq, o4);
   } else if (rowbytes % 16 == 0 && a16)
     gather_blocks_kernel<16><<<cdiv(px * (rowbytes / 16), 256), 256, 0, st>>>(v, Hv, Wv, rowbytes, idx, hq, wq, ks, o);
-  else if (rowbytes % 4 == 0)
+  else if (rowbytes % 4 == 0 && a4)
     gather_blocks_kernel<4><<<cdiv(px * (rowbytes / 4), 256), 256, 0, st>>>(v, Hv, Wv, rowbytes, idx, hq, wq, ks, o);
   else
     gather_blocks_kernel<2><<<cdiv(px * (rowbytes / 2), 256), 256, 0, st>>>(v, Hv, Wv, rowbytes, idx, hq, wq, ks, o);
