@@ -10,13 +10,6 @@
 
 namespace rv {
 
-#ifndef RV_W3_TILE_DEFAULT
-#define RV_W3_TILE_DEFAULT 0     // 8 x 16 pixels (see launch_warp3 for the measured shapes)
-#endif
-#ifndef RV_AS_TILE_DEFAULT
-#define RV_AS_TILE_DEFAULT 1     // 4 x 16 cells: 41.2 us vs 43.0 us (8 x 16) at 270x480x48 bf16 (H100 80GB HBM3, 400 W limit)
-#endif
-
 // ---------------------------------------------------------------------------------------------
 // small vector helpers: V elements of T moved as one 16/8/4-byte access
 // ---------------------------------------------------------------------------------------------
@@ -304,8 +297,54 @@ __global__ void flow_resize_kernel(const float* __restrict__ flow, int H, int W,
 
 // ---------------------------------------------------------------------------------------------
 // rv_warp : grid_sample(bilinear, zeros, align_corners=False) with the reference grid
-// one thread = one output pixel x one channel vector
 // ---------------------------------------------------------------------------------------------
+// F.interpolate(flow, x2, bilinear, align_corners=True) * 2 at pixel (Y, X) of the Ho x Wo = 2 hf x 2 wf grid; at(y, x) reads
+// the hf x wf flow (global memory, or warp3_kernel's shared flow tile)
+template <typename F>
+__device__ __forceinline__ float2 flow_up2_at(int Y, int X, int Ho, int Wo, int hf, int wf, F at) {
+  int y0, y1, x0, x1;
+  float ly, lx;
+  const float sy = (Ho > 1) ? (float)(hf - 1) / (float)(Ho - 1) : 0.f;
+  const float sx = (Wo > 1) ? (float)(wf - 1) / (float)(Wo - 1) : 0.f;
+  bilin_src_ac(Y, sy, hf, y0, y1, ly);
+  bilin_src_ac(X, sx, wf, x0, x1, lx);
+  const float hy = 1.f - ly, hx = 1.f - lx;
+  const float2 a = at(y0, x0), b = at(y0, x1), c = at(y1, x0), d = at(y1, x1);
+  return make_float2((hy * (hx * a.x + lx * b.x) + ly * (hx * c.x + lx * d.x)) * 2.0f,
+                     (hy * (hx * a.y + lx * b.y) + ly * (hx * c.y + lx * d.y)) * 2.0f);
+}
+
+// the reference grid (models/utils.py:36-43) at pixel (Xi, Yi) of a Wo x Ho map moved by (fx, fy), unnormalised for a Wi x Hi
+// source (aten grid_sampler_unnormalize, align_corners=False): top-left corner (ix, iy) and the weights of nw, ne, sw, se
+__device__ __forceinline__ void warp_pos(float fx, float fy, int Wo, int Ho, int Wi, int Hi, int Xi, int Yi, int& ix, int& iy,
+                                         float4& wq) {
+  float gx = linspace_m1_1(Xi, Wo) + fx / (((float)Wi - 1.0f) / 2.0f);
+  float gy = linspace_m1_1(Yi, Ho) + fy / (((float)Hi - 1.0f) / 2.0f);
+  float px = ((gx + 1.f) * (float)Wi - 1.f) / 2.f;
+  float py = ((gy + 1.f) * (float)Hi - 1.f) / 2.f;
+  float xw = floorf(px), yn = floorf(py);
+  ix = (int)xw;
+  iy = (int)yn;
+  float xe = xw + 1.f, ys = yn + 1.f;
+  wq = make_float4((xe - px) * (ys - py), (px - xw) * (ys - py), (xe - px) * (py - yn), (px - xw) * (py - yn));
+}
+
+// warp_pos for the branch-free gathers: weights of corners outside the source zeroed, corner pixel offsets clamped into it
+__device__ __forceinline__ void warp_corner(float fx, float fy, int Wo, int Ho, int Wi, int Hi, int Xi, int Yi, float4& wq, int4& off) {
+  int ix, iy;
+  warp_pos(fx, fy, Wo, Ho, Wi, Hi, Xi, Yi, ix, iy, wq);
+  const bool x0ok = ix >= 0 && ix < Wi, x1ok = ix + 1 >= 0 && ix + 1 < Wi;
+  const bool y0ok = iy >= 0 && iy < Hi, y1ok = iy + 1 >= 0 && iy + 1 < Hi;
+  if (!(y0ok && x0ok)) wq.x = 0.f;
+  if (!(y0ok && x1ok)) wq.y = 0.f;
+  if (!(y1ok && x0ok)) wq.z = 0.f;
+  if (!(y1ok && x1ok)) wq.w = 0.f;
+  const int cx0 = clampi(ix, 0, Wi - 1), cx1 = clampi(ix + 1, 0, Wi - 1);
+  const int cy0 = clampi(iy, 0, Hi - 1), cy1 = clampi(iy + 1, 0, Hi - 1);
+  off = make_int4(cy0 * Wi + cx0, cy0 * Wi + cx1, cy1 * Wi + cx0, cy1 * Wi + cx1);
+}
+
+// generic path: one thread = one output pixel x one channel vector
 template <typename T, int V>
 __global__ void warp_kernel(const T* __restrict__ src, int Hi, int Wi, int C,
                             const float* __restrict__ flow, int hf, int wf, int flow_up2,
@@ -320,36 +359,13 @@ __global__ void warp_kernel(const T* __restrict__ src, int Hi, int Wi, int C,
   int vc = (int)(i % cv);
   int p = (int)(i / cv);
   int Y = p / Wo, X = p % Wo;
-  float fx, fy;
-  if (flow_up2) {
-    int y0, y1, x0, x1;
-    float ly, lx;
-    float sy = (Ho > 1) ? (float)(hf - 1) / (float)(Ho - 1) : 0.f;
-    float sx = (Wo > 1) ? (float)(wf - 1) / (float)(Wo - 1) : 0.f;
-    bilin_src_ac(Y, sy, hf, y0, y1, ly);
-    bilin_src_ac(X, sx, wf, x0, x1, lx);
-    float hy = 1.f - ly, hx = 1.f - lx;
-    const float2* f2 = reinterpret_cast<const float2*>(flow);
-    float2 a = __ldg(f2 + y0 * wf + x0), b = __ldg(f2 + y0 * wf + x1), c = __ldg(f2 + y1 * wf + x0),
-           d = __ldg(f2 + y1 * wf + x1);
-    fx = (hy * (hx * a.x + lx * b.x) + ly * (hx * c.x + lx * d.x)) * 2.0f;
-    fy = (hy * (hx * a.y + lx * b.y) + ly * (hx * c.y + lx * d.y)) * 2.0f;
-  } else {
-    float2 f = __ldg(reinterpret_cast<const float2*>(flow) + p);
-    fx = f.x;
-    fy = f.y;
-  }
-  // models/utils.py:36-43
-  float gx = linspace_m1_1(X, Wo) + fx / (((float)Wi - 1.0f) / 2.0f);
-  float gy = linspace_m1_1(Y, Ho) + fy / (((float)Hi - 1.0f) / 2.0f);
-  // aten grid_sampler_unnormalize (align_corners=False)
-  float px = ((gx + 1.f) * (float)Wi - 1.f) / 2.f;
-  float py = ((gy + 1.f) * (float)Hi - 1.f) / 2.f;
-  float xw = floorf(px), yn = floorf(py);
-  int ix = (int)xw, iy = (int)yn;
-  float xe = xw + 1.f, ys = yn + 1.f;
-  float nw = (xe - px) * (ys - py), ne = (px - xw) * (ys - py), sw = (xe - px) * (py - yn),
-        se = (px - xw) * (py - yn);
+  const float2* f2 = reinterpret_cast<const float2*>(flow);
+  float2 f;
+  if (flow_up2) f = flow_up2_at(Y, X, Ho, Wo, hf, wf, [&](int y, int x) { return __ldg(f2 + y * wf + x); });
+  else f = __ldg(f2 + p);
+  int ix, iy;
+  float4 wq;
+  warp_pos(f.x, f.y, Wo, Ho, Wi, Hi, X, Y, ix, iy, wq);
   float acc[V];
 #pragma unroll
   for (int k = 0; k < V; ++k) acc[k] = 0.f;
@@ -359,22 +375,22 @@ __global__ void warp_kernel(const T* __restrict__ src, int Hi, int Wi, int C,
   if (y0ok && x0ok) {
     Vec<T, V> t = ldv<T, V>(base + ((size_t)iy * Wi + ix) * C);
 #pragma unroll
-    for (int k = 0; k < V; ++k) acc[k] += to_f(t.v[k]) * nw;
+    for (int k = 0; k < V; ++k) acc[k] += to_f(t.v[k]) * wq.x;
   }
   if (y0ok && x1ok) {
     Vec<T, V> t = ldv<T, V>(base + ((size_t)iy * Wi + ix + 1) * C);
 #pragma unroll
-    for (int k = 0; k < V; ++k) acc[k] += to_f(t.v[k]) * ne;
+    for (int k = 0; k < V; ++k) acc[k] += to_f(t.v[k]) * wq.y;
   }
   if (y1ok && x0ok) {
     Vec<T, V> t = ldv<T, V>(base + ((size_t)(iy + 1) * Wi + ix) * C);
 #pragma unroll
-    for (int k = 0; k < V; ++k) acc[k] += to_f(t.v[k]) * sw;
+    for (int k = 0; k < V; ++k) acc[k] += to_f(t.v[k]) * wq.z;
   }
   if (y1ok && x1ok) {
     Vec<T, V> t = ldv<T, V>(base + ((size_t)(iy + 1) * Wi + ix + 1) * C);
 #pragma unroll
-    for (int k = 0; k < V; ++k) acc[k] += to_f(t.v[k]) * se;
+    for (int k = 0; k < V; ++k) acc[k] += to_f(t.v[k]) * wq.w;
   }
   Vec<T, V> o;
 #pragma unroll
@@ -386,14 +402,14 @@ __global__ void warp_kernel(const T* __restrict__ src, int Hi, int Wi, int C,
 // offsets (clamped) and weights (zeroed when the corner is outside the image) into shared memory;
 // phase 2 is a branch-free 4-tap gather with one thread per (pixel, 16-byte channel vector), so global
 // loads and stores stay fully coalesced along the NHWC channel axis.
-template <typename T, int V, int NV>
+template <typename T, int V>
 __global__ void __launch_bounds__(256) warp_vec_kernel(const T* __restrict__ src, int Hi, int Wi, int C,
                                                        const float* __restrict__ flow, int hf, int wf,
                                                        int flow_up2, T* __restrict__ out, int ppb) {
   __shared__ float4 s_w[256];
   __shared__ int4 s_o[256];
   const int Ho = flow_up2 ? 2 * hf : hf, Wo = flow_up2 ? 2 * wf : wf;
-  const int cv = C / (V * NV);      // threads per pixel; each moves NV consecutive 16-byte vectors
+  const int cv = C / V;             // threads per pixel
   src += (size_t)blockIdx.z * Hi * Wi * C;           // image blockIdx.z of a batch (rv_warp_batched)
   flow += (size_t)blockIdx.z * hf * wf * 2;
   out += (size_t)blockIdx.z * Ho * Wo * C;
@@ -402,61 +418,25 @@ __global__ void __launch_bounds__(256) warp_vec_kernel(const T* __restrict__ src
   if (threadIdx.x < ppb && p0 + threadIdx.x < npix) {
     const int p = p0 + threadIdx.x;
     const int Y = p / Wo, X = p - Y * Wo;
-    float fx, fy;
-    if (flow_up2) {
-      int y0, y1, x0, x1;
-      float ly, lx;
-      float sy = (Ho > 1) ? (float)(hf - 1) / (float)(Ho - 1) : 0.f;
-      float sx = (Wo > 1) ? (float)(wf - 1) / (float)(Wo - 1) : 0.f;
-      bilin_src_ac(Y, sy, hf, y0, y1, ly);
-      bilin_src_ac(X, sx, wf, x0, x1, lx);
-      float hy = 1.f - ly, hx = 1.f - lx;
-      const float2* f2 = reinterpret_cast<const float2*>(flow);
-      float2 a = __ldg(f2 + y0 * wf + x0), b = __ldg(f2 + y0 * wf + x1), c = __ldg(f2 + y1 * wf + x0),
-             d = __ldg(f2 + y1 * wf + x1);
-      fx = (hy * (hx * a.x + lx * b.x) + ly * (hx * c.x + lx * d.x)) * 2.0f;
-      fy = (hy * (hx * a.y + lx * b.y) + ly * (hx * c.y + lx * d.y)) * 2.0f;
-    } else {
-      float2 f = __ldg(reinterpret_cast<const float2*>(flow) + p);
-      fx = f.x;
-      fy = f.y;
-    }
-    float gx = linspace_m1_1(X, Wo) + fx / (((float)Wi - 1.0f) / 2.0f);   // models/utils.py:36-43
-    float gy = linspace_m1_1(Y, Ho) + fy / (((float)Hi - 1.0f) / 2.0f);
-    float px = ((gx + 1.f) * (float)Wi - 1.f) / 2.f;
-    float py = ((gy + 1.f) * (float)Hi - 1.f) / 2.f;
-    float xw = floorf(px), yn = floorf(py);
-    int ix = (int)xw, iy = (int)yn;
-    float xe = xw + 1.f, ys = yn + 1.f;
-    float4 wq = make_float4((xe - px) * (ys - py), (px - xw) * (ys - py), (xe - px) * (py - yn), (px - xw) * (py - yn));
-    const bool x0ok = ix >= 0 && ix < Wi, x1ok = ix + 1 >= 0 && ix + 1 < Wi;
-    const bool y0ok = iy >= 0 && iy < Hi, y1ok = iy + 1 >= 0 && iy + 1 < Hi;
-    if (!(y0ok && x0ok)) wq.x = 0.f;
-    if (!(y0ok && x1ok)) wq.y = 0.f;
-    if (!(y1ok && x0ok)) wq.z = 0.f;
-    if (!(y1ok && x1ok)) wq.w = 0.f;
-    const int cx0 = clampi(ix, 0, Wi - 1), cx1 = clampi(ix + 1, 0, Wi - 1);
-    const int cy0 = clampi(iy, 0, Hi - 1), cy1 = clampi(iy + 1, 0, Hi - 1);
+    const float2* f2 = reinterpret_cast<const float2*>(flow);
+    float2 f;
+    if (flow_up2) f = flow_up2_at(Y, X, Ho, Wo, hf, wf, [&](int y, int x) { return __ldg(f2 + y * wf + x); });
+    else f = __ldg(f2 + p);
+    float4 wq;
+    int4 off;
+    warp_corner(f.x, f.y, Wo, Ho, Wi, Hi, X, Y, wq, off);
     s_w[threadIdx.x] = wq;
-    s_o[threadIdx.x] = make_int4(cy0 * Wi + cx0, cy0 * Wi + cx1, cy1 * Wi + cx0, cy1 * Wi + cx1);
+    s_o[threadIdx.x] = off;
   }
   __syncthreads();
   const int pl = threadIdx.x / cv, vc = threadIdx.x - pl * cv;
   if (pl >= ppb || p0 + pl >= npix) return;
   const float4 wq = s_w[pl];
   const int4 o = s_o[pl];
-  const T* base = src + (size_t)vc * (V * NV);
-  Vec<T, V> t0[NV], t1[NV], t2[NV], t3[NV];
-#pragma unroll
-  for (int n = 0; n < NV; ++n) {          // all 4*NV loads in flight before any use
-    t0[n] = ldv<T, V>(base + (size_t)o.x * C + n * V);
-    t1[n] = ldv<T, V>(base + (size_t)o.y * C + n * V);
-    t2[n] = ldv<T, V>(base + (size_t)o.z * C + n * V);
-    t3[n] = ldv<T, V>(base + (size_t)o.w * C + n * V);
-  }
-#pragma unroll
-  for (int n = 0; n < NV; ++n)
-    stv<T, V>(out + (size_t)(p0 + pl) * C + (size_t)vc * (V * NV) + n * V, blend4<T, V>(t0[n], t1[n], t2[n], t3[n], wq));
+  const T* base = src + (size_t)vc * V;
+  const Vec<T, V> t0 = ldv<T, V>(base + (size_t)o.x * C), t1 = ldv<T, V>(base + (size_t)o.y * C),
+                  t2 = ldv<T, V>(base + (size_t)o.z * C), t3 = ldv<T, V>(base + (size_t)o.w * C);
+  stv<T, V>(out + (size_t)(p0 + pl) * C + (size_t)vc * V, blend4<T, V>(t0, t1, t2, t3, wq));
 }
 
 
@@ -468,31 +448,13 @@ __global__ void __launch_bounds__(256) warp_vec_kernel(const T* __restrict__ src
 // corner offsets (clamped) and weights (zero outside the image) into shared memory, phase 2 is the branch-free 4-tap gather
 // with one thread per (pixel, 16-byte channel vector): coalesced along the NHWC channel axis, and - because the tile is 2-D -
 // the corner rows shared by vertically adjacent output pixels are fetched from L2 once per CTA (L1 hits), not once per row.
-// Same arithmetic as warp_kernel / warp_vec_kernel (bit-identical results).
+// Same arithmetic as warp_kernel / warp_vec_kernel (bit-identical results).  Measured at 270x480x48 bf16 on an H100 80GB HBM3
+// at a 400 W limit (tools/pointwise_bench.py): 52.7 us for 8 x 16 and 4 x 16 tiles, 57.3 us for 2 x 16 - every CTA pays the
+// flow-tile load and two barriers before its first gather, so the smallest tiles lose.
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void warp_corner(float X, float Y, float fx, float fy, int Wo, int Ho, int Wi, int Hi, int Xi, int Yi,
-                                            float4& wq, int4& off) {
-  float gx = linspace_m1_1(Xi, Wo) + fx / (((float)Wi - 1.0f) / 2.0f);   // models/utils.py:36-43
-  float gy = linspace_m1_1(Yi, Ho) + fy / (((float)Hi - 1.0f) / 2.0f);
-  float px = ((gx + 1.f) * (float)Wi - 1.f) / 2.f;
-  float py = ((gy + 1.f) * (float)Hi - 1.f) / 2.f;
-  float xw = floorf(px), yn = floorf(py);
-  int ix = (int)xw, iy = (int)yn;
-  float xe = xw + 1.f, ys = yn + 1.f;
-  wq = make_float4((xe - px) * (ys - py), (px - xw) * (ys - py), (xe - px) * (py - yn), (px - xw) * (py - yn));
-  const bool x0ok = ix >= 0 && ix < Wi, x1ok = ix + 1 >= 0 && ix + 1 < Wi;
-  const bool y0ok = iy >= 0 && iy < Hi, y1ok = iy + 1 >= 0 && iy + 1 < Hi;
-  if (!(y0ok && x0ok)) wq.x = 0.f;
-  if (!(y0ok && x1ok)) wq.y = 0.f;
-  if (!(y1ok && x0ok)) wq.z = 0.f;
-  if (!(y1ok && x1ok)) wq.w = 0.f;
-  const int cx0 = clampi(ix, 0, Wi - 1), cx1 = clampi(ix + 1, 0, Wi - 1);
-  const int cy0 = clampi(iy, 0, Hi - 1), cy1 = clampi(iy + 1, 0, Hi - 1);
-  off = make_int4(cy0 * Wi + cx0, cy0 * Wi + cx1, cy1 * Wi + cx0, cy1 * Wi + cx1);
-  (void)X; (void)Y;
-}
+constexpr int W3_TH = 8, W3_TW = 16;
 
-template <typename T, int CV, int W3_TH, int W3_TW>      // CV = C / V (16-byte vectors per pixel) when known at compile time, 0 = run-time
+template <typename T, int CV>      // CV = C / V (16-byte vectors per pixel) when known at compile time, 0 = run-time
 __global__ void __launch_bounds__(256) warp3_kernel(const T* __restrict__ feat, const T* __restrict__ featUP,
                                                     const float* __restrict__ conf, const float* __restrict__ flow, int h, int w,
                                                     int C, T* __restrict__ o_feat, T* __restrict__ o_featUP,
@@ -527,23 +489,14 @@ __global__ void __launch_bounds__(256) warp3_kernel(const T* __restrict__ feat, 
       const int Y = ty0 + i / W3_TW, X = tx0 + i % W3_TW;
       if (Y < h && X < w) {
         const float2 f = flow_at(Y, X);
-        warp_corner(0.f, 0.f, f.x, f.y, w, h, w, h, X, Y, wq, off);
+        warp_corner(f.x, f.y, w, h, w, h, X, Y, wq, off);
       }
     } else {
       const int j = i - NLR;
       const int Y = 2 * ty0 + j / (2 * W3_TW), X = 2 * tx0 + j % (2 * W3_TW);
       if (Y < H2 && X < W2) {
-        int y0, y1, x0, x1;
-        float ly, lx;
-        const float sy = (H2 > 1) ? (float)(h - 1) / (float)(H2 - 1) : 0.f;      // F.interpolate(x2, bilinear, align_corners=True)
-        const float sx = (W2 > 1) ? (float)(w - 1) / (float)(W2 - 1) : 0.f;
-        bilin_src_ac(Y, sy, h, y0, y1, ly);
-        bilin_src_ac(X, sx, w, x0, x1, lx);
-        const float hy = 1.f - ly, hx = 1.f - lx;
-        const float2 a = flow_at(y0, x0), b = flow_at(y0, x1), c = flow_at(y1, x0), d = flow_at(y1, x1);
-        const float fx = (hy * (hx * a.x + lx * b.x) + ly * (hx * c.x + lx * d.x)) * 2.0f;
-        const float fy = (hy * (hx * a.y + lx * b.y) + ly * (hx * c.y + lx * d.y)) * 2.0f;
-        warp_corner(0.f, 0.f, fx, fy, W2, H2, W2, H2, X, Y, wq, off);
+        const float2 f = flow_up2_at(Y, X, H2, W2, h, w, flow_at);
+        warp_corner(f.x, f.y, W2, H2, W2, H2, X, Y, wq, off);
       }
     }
     s_w[i] = wq;
@@ -704,10 +657,42 @@ __global__ void space_to_depth2_kernel(const uint4* __restrict__ src, int H, int
   out[((size_t)p * 4 + sub) * cv + v] = __ldg(src + ((size_t)(2 * Y + ry) * W + (2 * X + rx)) * cv + v);
 }
 
+// AlignedConv2d's sample of cell (ci, cj) of a ks x ks block grid over the H x W map, at offset (u, v) from the cell's centre
+// (half = ks / 2) before the cell's rotation (cs, sn): the position, clamped into the reflection-padded map, gives the weights of
+// the corners (lt, rb, lb, rt) and their source rows r0, r1 and columns c0, c1 (ReflectionPad2d(1)).  FMA_AS_GENERIC spells out
+// the contraction the compiler picks for the rotation in aligned_sample_kernel, where the offsets are run-time values: with them
+// known at compile time it would fuse the other product of each pair (its products of v are shared across rows).
+template <bool FMA_AS_GENERIC>
+__device__ __forceinline__ void aligned_tap(float u, float v, float cs, float sn, float half, int ci, int cj, int ks, int H, int W,
+                                            float4& g, int& r0, int& r1, int& c0, int& c1) {
+  const int Hp = H + 2, Wp = W + 2;
+  float rr, cc;
+  if constexpr (FMA_AS_GENERIC) {
+    rr = __fmaf_rn(u, cs, -__fmul_rn(v, sn));
+    cc = __fmaf_rn(v, cs, __fmul_rn(u, sn));
+  } else {
+    rr = u * cs - v * sn;
+    cc = u * sn + v * cs;
+  }
+  float pr = rr + half + (float)(1 + ci * ks);
+  float pc = cc + half + (float)(1 + cj * ks);
+  float ltr = floorf(pr), ltc = floorf(pc);
+  float rbr = ltr + 1.f, rbc = ltc + 1.f;
+  const float Hm = (float)(Hp - 1), Wm = (float)(Wp - 1);
+  ltr = fminf(fmaxf(ltr, 0.f), Hm); rbr = fminf(fmaxf(rbr, 0.f), Hm);
+  ltc = fminf(fmaxf(ltc, 0.f), Wm); rbc = fminf(fmaxf(rbc, 0.f), Wm);
+  pr = fminf(fmaxf(pr, 0.f), Hm); pc = fminf(fmaxf(pc, 0.f), Wm);
+  g = make_float4((1.f + (ltr - pr)) * (1.f + (ltc - pc)), (1.f - (rbr - pr)) * (1.f - (rbc - pc)),
+                  (1.f + (ltr - pr)) * (1.f - (rbc - pc)), (1.f - (rbr - pr)) * (1.f + (ltc - pc)));
+  // padded index -> source index
+  r0 = reflect1((int)ltr - 1, H); r1 = reflect1((int)rbr - 1, H);
+  c0 = reflect1((int)ltc - 1, W); c1 = reflect1((int)rbc - 1, W);
+}
+
 template <typename T, int V>
 __global__ void aligned_sample_kernel(const T* __restrict__ x, int h, int w, int ks, int C,
                                       const float* __restrict__ affine, T* __restrict__ out) {
-  const int H = ks * h, W = ks * w, Hp = H + 2, Wp = W + 2;
+  const int H = ks * h, W = ks * w;
   const int cv = C / V;
   long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)H * W * cv) return;
@@ -720,22 +705,9 @@ __global__ void aligned_sample_kernel(const T* __restrict__ x, int h, int w, int
   float half = (float)((ks - 1) / 2) + 0.5f;  // -(ks-1)//2 - 0.5 + a  ==  a - half
   float u = ((float)a - half) * s_x, v = ((float)b - half) * s_y;
   float cs = cosf(th), sn = sinf(th);
-  float rr = u * cs - v * sn, cc = u * sn + v * cs;
-  float pr = rr + half + (float)(1 + ci * ks);
-  float pc = cc + half + (float)(1 + cj * ks);
-  float ltr = floorf(pr), ltc = floorf(pc);
-  float rbr = ltr + 1.f, rbc = ltc + 1.f;
-  const float Hm = (float)(Hp - 1), Wm = (float)(Wp - 1);
-  ltr = fminf(fmaxf(ltr, 0.f), Hm); rbr = fminf(fmaxf(rbr, 0.f), Hm);
-  ltc = fminf(fmaxf(ltc, 0.f), Wm); rbc = fminf(fmaxf(rbc, 0.f), Wm);
-  pr = fminf(fmaxf(pr, 0.f), Hm); pc = fminf(fmaxf(pc, 0.f), Wm);
-  float g_lt = (1.f + (ltr - pr)) * (1.f + (ltc - pc));
-  float g_rb = (1.f - (rbr - pr)) * (1.f - (rbc - pc));
-  float g_lb = (1.f + (ltr - pr)) * (1.f - (rbc - pc));
-  float g_rt = (1.f - (rbr - pr)) * (1.f + (ltc - pc));
-  // padded index -> source index (ReflectionPad2d(1))
-  int r0 = reflect1((int)ltr - 1, H), r1 = reflect1((int)rbr - 1, H);
-  int c0 = reflect1((int)ltc - 1, W), c1 = reflect1((int)rbc - 1, W);
+  float4 g;
+  int r0, r1, c0, c1;
+  aligned_tap<false>(u, v, cs, sn, half, ci, cj, ks, H, W, g, r0, r1, c0, c1);
   const T* base = x + (size_t)vc * V;
   Vec<T, V> t_lt = ldv<T, V>(base + ((size_t)r0 * W + c0) * C);
   Vec<T, V> t_rb = ldv<T, V>(base + ((size_t)r1 * W + c1) * C);
@@ -744,55 +716,46 @@ __global__ void aligned_sample_kernel(const T* __restrict__ x, int h, int w, int
   Vec<T, V> o;
 #pragma unroll
   for (int k = 0; k < V; ++k)
-    o.v[k] = from_f<T>(g_lt * to_f(t_lt.v[k]) + g_rb * to_f(t_rb.v[k]) + g_lb * to_f(t_lb.v[k]) +
-                       g_rt * to_f(t_rt.v[k]));
+    o.v[k] = from_f<T>(g.x * to_f(t_lt.v[k]) + g.y * to_f(t_rb.v[k]) + g.z * to_f(t_lb.v[k]) +
+                       g.w * to_f(t_rt.v[k]));
   stv<T, V>(out + (size_t)p * C + (size_t)vc * V, o);
 }
 
-
-// ks = 2 (every x4 model): 2-D tiles of AS_TH x 16 cells = 2 AS_TH x 32 output pixels.  Phase 1 evaluates the affine sampling
-// positions ONCE per cell - sin / cos once, then the four samples of the cell (the per-thread version above recomputes
-// sin / cos / floor / reflect for each of the C/8 channel vectors of a pixel) - into shared memory, phase 2 is the same
-// branch-free 4-tap gather as warp3_kernel.  Same arithmetic.
-template <typename T, int CV, int AS_TH>
-__global__ void __launch_bounds__(256) aligned_sample2_kernel(const T* __restrict__ x, int h, int w, int C,
-                                                              const float* __restrict__ affine, T* __restrict__ out) {
+// ks = 2 (every x4 model) and ks = 4 (aa2 of the x2 models, aa1 of the flag_HD_in models) on 2-D tiles of cells: 4 x 16 cells =
+// 8 x 32 output pixels at ks 2 (41.2 us vs 43.0 us for 8 x 16 cells at 270x480x48 bf16, H100 80GB HBM3 at a 400 W limit), 8 x 8
+// cells = 32 x 32 pixels at ks 4.  Phase 1 evaluates the ks * ks sampling positions of a cell once (sin / cos once per cell
+// instead of once per channel vector of every pixel) into shared memory, phase 2 is the same branch-free 4-tap gather as
+// warp3_kernel.  At ks 4 the result is bit-identical to aligned_sample_kernel: the rotation and the blend are written out in the
+// order the compiler contracts that kernel's expressions; at ks 2 the compiler contracts them.
+template <int KS, typename T, int CV>
+__device__ __forceinline__ void aligned_sample_tiled(const T* __restrict__ x, int h, int w, int C, const float* __restrict__ affine,
+                                                     T* __restrict__ out) {
   constexpr int V = 16 / (int)sizeof(T);
-  constexpr int ks = 2, AS_TW = 16, NC = AS_TH * AS_TW, NP = 4 * NC, PW = 2 * AS_TW;
+  constexpr int AS_TH = KS == 2 ? 4 : 8, AS_TW = KS == 2 ? 16 : 8, NC = AS_TH * AS_TW, NP = KS * KS * NC, PW = KS * AS_TW;
   __shared__ float4 s_w[NP];
   __shared__ int4 s_o[NP];
-  const int H = ks * h, W = ks * w, Hp = H + 2, Wp = W + 2;
+  const int H = KS * h, W = KS * w;
   const int tiles_x = (w + AS_TW - 1) / AS_TW;
   const int ci0 = (blockIdx.x / tiles_x) * AS_TH, cj0 = (blockIdx.x % tiles_x) * AS_TW;
-  const int Y0 = 2 * ci0, X0 = 2 * cj0;
+  const int Y0 = KS * ci0, X0 = KS * cj0;
   for (int c = threadIdx.x; c < NC; c += blockDim.x) {
     const int li = c / AS_TW, lj = c % AS_TW;
     const int ci = ci0 + li, cj = cj0 + lj;
     if (ci >= h || cj >= w) continue;                       // (entries of cells outside the image are never read)
     const float* af = affine + ((size_t)ci * w + cj) * 3;
     const float s_x = af[0], s_y = af[1], th = (af[2] - 1.0f) * 1.0472f;
-    const float half = (float)((ks - 1) / 2) + 0.5f;
+    const float half = (float)((KS - 1) / 2) + 0.5f;
     const float cs = cosf(th), sn = sinf(th);
-    const float Hm = (float)(Hp - 1), Wm = (float)(Wp - 1);
 #pragma unroll
-    for (int a = 0; a < 2; ++a)
+    for (int a = 0; a < KS; ++a)
 #pragma unroll
-      for (int b = 0; b < 2; ++b) {
+      for (int b = 0; b < KS; ++b) {
         const float u = ((float)a - half) * s_x, v = ((float)b - half) * s_y;
-        const float rr = u * cs - v * sn, cc = u * sn + v * cs;
-        float pr = rr + half + (float)(1 + ci * ks);
-        float pc = cc + half + (float)(1 + cj * ks);
-        float ltr = floorf(pr), ltc = floorf(pc);
-        float rbr = ltr + 1.f, rbc = ltc + 1.f;
-        ltr = fminf(fmaxf(ltr, 0.f), Hm); rbr = fminf(fmaxf(rbr, 0.f), Hm);
-        ltc = fminf(fmaxf(ltc, 0.f), Wm); rbc = fminf(fmaxf(rbc, 0.f), Wm);
-        pr = fminf(fmaxf(pr, 0.f), Hm); pc = fminf(fmaxf(pc, 0.f), Wm);
-        const int r0 = reflect1((int)ltr - 1, H), r1 = reflect1((int)rbr - 1, H);
-        const int c0 = reflect1((int)ltc - 1, W), c1 = reflect1((int)rbc - 1, W);
-        const int e = (2 * li + a) * PW + 2 * lj + b;
-        // order (lt, rb, lb, rt) as in aligned_sample_kernel
-        s_w[e] = make_float4((1.f + (ltr - pr)) * (1.f + (ltc - pc)), (1.f - (rbr - pr)) * (1.f - (rbc - pc)),
-                             (1.f + (ltr - pr)) * (1.f - (rbc - pc)), (1.f - (rbr - pr)) * (1.f + (ltc - pc)));
+        float4 g;
+        int r0, r1, c0, c1;
+        aligned_tap<KS == 4>(u, v, cs, sn, half, ci, cj, KS, H, W, g, r0, r1, c0, c1);
+        const int e = (KS * li + a) * PW + KS * lj + b;
+        s_w[e] = g;
         s_o[e] = make_int4(r0 * W + c0, r1 * W + c1, r0 * W + c1, r1 * W + c0);
       }
   }
@@ -806,70 +769,21 @@ __global__ void __launch_bounds__(256) aligned_sample2_kernel(const T* __restric
     const int4 o = s_o[pl];
     const Vec<T, V> t_lt = ldvi<T, V>(x, o.x * cv + vc), t_rb = ldvi<T, V>(x, o.y * cv + vc),
                     t_lb = ldvi<T, V>(x, o.z * cv + vc), t_rt = ldvi<T, V>(x, o.w * cv + vc);
-    stvi<T, V>(out, (Y * W + X) * cv + vc, blend4<T, V>(t_lt, t_rb, t_lb, t_rt, g));
+    stvi<T, V>(out, (Y * W + X) * cv + vc,
+               KS == 4 ? blend4_as_generic<T, V>(t_lt, t_rb, t_lb, t_rt, g) : blend4<T, V>(t_lt, t_rb, t_lb, t_rt, g));
   }
 }
 
-// ks = 4 (aa2 of the x2 models, aa1 of the flag_HD_in models): the sibling of aligned_sample2_kernel on tiles of 8 x 8 cells =
-// 32 x 32 output pixels.  Phase 1 evaluates the 16 sampling positions of a cell once (sin / cos once per cell instead of once per
-// channel vector of every pixel), phase 2 is the same 4-tap gather.  Bit-identical to aligned_sample_kernel: the rotation and
-// the blend are written out in the order the compiler contracts that kernel's expressions.
+// one kernel per ks, so that a profile names the path that ran
+template <typename T, int CV>
+__global__ void __launch_bounds__(256) aligned_sample2_kernel(const T* __restrict__ x, int h, int w, int C,
+                                                              const float* __restrict__ affine, T* __restrict__ out) {
+  aligned_sample_tiled<2, T, CV>(x, h, w, C, affine, out);
+}
 template <typename T, int CV>
 __global__ void __launch_bounds__(256) aligned_sample4_kernel(const T* __restrict__ x, int h, int w, int C,
                                                               const float* __restrict__ affine, T* __restrict__ out) {
-  constexpr int V = 16 / (int)sizeof(T);
-  constexpr int ks = 4, AS_TH = 8, AS_TW = 8, NC = AS_TH * AS_TW, NP = ks * ks * NC, PW = ks * AS_TW;
-  __shared__ float4 s_w[NP];
-  __shared__ int4 s_o[NP];
-  const int H = ks * h, W = ks * w, Hp = H + 2, Wp = W + 2;
-  const int tiles_x = (w + AS_TW - 1) / AS_TW;
-  const int ci0 = (blockIdx.x / tiles_x) * AS_TH, cj0 = (blockIdx.x % tiles_x) * AS_TW;
-  const int Y0 = ks * ci0, X0 = ks * cj0;
-  for (int c = threadIdx.x; c < NC; c += blockDim.x) {
-    const int li = c / AS_TW, lj = c % AS_TW;
-    const int ci = ci0 + li, cj = cj0 + lj;
-    if (ci >= h || cj >= w) continue;                       // (entries of cells outside the image are never read)
-    const float* af = affine + ((size_t)ci * w + cj) * 3;
-    const float s_x = af[0], s_y = af[1], th = (af[2] - 1.0f) * 1.0472f;
-    const float half = (float)((ks - 1) / 2) + 0.5f;
-    const float cs = cosf(th), sn = sinf(th);
-    const float Hm = (float)(Hp - 1), Wm = (float)(Wp - 1);
-#pragma unroll
-    for (int a = 0; a < ks; ++a)
-#pragma unroll
-      for (int b = 0; b < ks; ++b) {
-        const float u = ((float)a - half) * s_x, v = ((float)b - half) * s_y;
-        // the contraction aligned_sample_kernel gets from the compiler, spelled out: with a, b known here the compiler would
-        // otherwise fuse the other product of each pair (its products of v are shared across rows)
-        const float rr = __fmaf_rn(u, cs, -__fmul_rn(v, sn)), cc = __fmaf_rn(v, cs, __fmul_rn(u, sn));
-        float pr = rr + half + (float)(1 + ci * ks);
-        float pc = cc + half + (float)(1 + cj * ks);
-        float ltr = floorf(pr), ltc = floorf(pc);
-        float rbr = ltr + 1.f, rbc = ltc + 1.f;
-        ltr = fminf(fmaxf(ltr, 0.f), Hm); rbr = fminf(fmaxf(rbr, 0.f), Hm);
-        ltc = fminf(fmaxf(ltc, 0.f), Wm); rbc = fminf(fmaxf(rbc, 0.f), Wm);
-        pr = fminf(fmaxf(pr, 0.f), Hm); pc = fminf(fmaxf(pc, 0.f), Wm);
-        const int r0 = reflect1((int)ltr - 1, H), r1 = reflect1((int)rbr - 1, H);
-        const int c0 = reflect1((int)ltc - 1, W), c1 = reflect1((int)rbc - 1, W);
-        const int e = (ks * li + a) * PW + ks * lj + b;
-        // order (lt, rb, lb, rt) as in aligned_sample_kernel
-        s_w[e] = make_float4((1.f + (ltr - pr)) * (1.f + (ltc - pc)), (1.f - (rbr - pr)) * (1.f - (rbc - pc)),
-                             (1.f + (ltr - pr)) * (1.f - (rbc - pc)), (1.f - (rbr - pr)) * (1.f + (ltc - pc)));
-        s_o[e] = make_int4(r0 * W + c0, r1 * W + c1, r0 * W + c1, r1 * W + c0);
-      }
-  }
-  __syncthreads();
-  const int cv = CV > 0 ? CV : C / V;
-  for (int it = threadIdx.x; it < NP * cv; it += blockDim.x) {
-    const int pl = it / cv, vc = it - pl * cv;
-    const int Y = Y0 + pl / PW, X = X0 + pl % PW;
-    if (Y >= H || X >= W) continue;
-    const float4 g = s_w[pl];
-    const int4 o = s_o[pl];
-    const Vec<T, V> t_lt = ldvi<T, V>(x, o.x * cv + vc), t_rb = ldvi<T, V>(x, o.y * cv + vc),
-                    t_lb = ldvi<T, V>(x, o.z * cv + vc), t_rt = ldvi<T, V>(x, o.w * cv + vc);
-    stvi<T, V>(out, (Y * W + X) * cv + vc, blend4_as_generic<T, V>(t_lt, t_rb, t_lb, t_rt, g));
-  }
+  aligned_sample_tiled<4, T, CV>(x, h, w, C, affine, out);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -970,6 +884,17 @@ __global__ void conf_max_kernel(const float* __restrict__ a, const float* __rest
   if (i < n) out[i] = fmaxf(a[i], b[i]);
 }
 
+// rv_reconstruct's value of output pixel p = (Y, X), channel c: x + clamp01(bicubic xS of the LR image) [+ clamp01]
+template <typename T>
+__device__ __forceinline__ float reconstruct_at(const T* __restrict__ x, int xc, const float* __restrict__ lr, int h, int w, int Y,
+                                                int X, int p, int c, float inv, int clamp01) {
+  float base = bicubic_planar(lr + (size_t)c * h * w, h, w, Y, X, inv);
+  base = fminf(fmaxf(base, 0.f), 1.f);
+  float v = to_f(x[(size_t)p * xc + c]) + base;
+  if (clamp01) v = fminf(fmaxf(v, 0.f), 1.f);
+  return v;
+}
+
 template <typename T>
 __global__ void reconstruct_kernel(const T* __restrict__ x, int xc, const float* __restrict__ lr,
                                    int h, int w, int scale, int clamp01,
@@ -983,13 +908,7 @@ __global__ void reconstruct_kernel(const T* __restrict__ x, int xc, const float*
   int Y = p / Wo, X = p % Wo;
   float inv = 1.0f / (float)scale;
 #pragma unroll
-  for (int c = 0; c < 3; ++c) {
-    float base = bicubic_planar(lr + (size_t)c * h * w, h, w, Y, X, inv);
-    base = fminf(fmaxf(base, 0.f), 1.f);
-    float v = to_f(x[(size_t)p * xc + c]) + base;
-    if (clamp01) v = fminf(fmaxf(v, 0.f), 1.f);
-    out[(size_t)c * Ho * Wo + p] = v;
-  }
+  for (int c = 0; c < 3; ++c) out[(size_t)c * Ho * Wo + p] = reconstruct_at(x, xc, lr, h, w, Y, X, p, c, inv, clamp01);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1338,13 +1257,7 @@ __global__ void __launch_bounds__(256) reconstruct_u8_kernel(const T* __restrict
     const int p = p0 + j;
     const int Y = p / Wo, X = p % Wo;
 #pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      float base = bicubic_planar(lr + (size_t)c * h * w, h, w, Y, X, inv);
-      base = fminf(fmaxf(base, 0.f), 1.f);
-      float v = to_f(x[(size_t)p * xc + c]) + base;
-      if (clamp01) v = fminf(fmaxf(v, 0.f), 1.f);
-      put_u8<BGR>(ob, j, c, v);
-    }
+    for (int c = 0; c < 3; ++c) put_u8<BGR>(ob, j, c, reconstruct_at(x, xc, lr, h, w, Y, X, p, c, inv, clamp01));
   }
   store_run(out + 3 * (size_t)p0, ob, 3 * n, vec);
 }
@@ -1355,6 +1268,13 @@ __global__ void __launch_bounds__(256) reconstruct_u8_kernel(const T* __restrict
 // C ABI
 // =================================================================================================
 using namespace rv;
+
+// REFVSR_NO_FAST_POINTWISE set: the generic gather, aligned-sample and reconstruct kernels only (the reference the fast paths are
+// checked against).  Read once per process.
+static bool fast_pointwise() {
+  static const bool ok = getenv("REFVSR_NO_FAST_POINTWISE") == nullptr;
+  return ok;
+}
 
 extern "C" int rv_frames_differ(const void* const* a, const void* const* b, const uint64_t* nbytes, int n, int32_t* flag,
                                 void* stream) {
@@ -1429,12 +1349,9 @@ static int warp_launch(const void* src, int Hi, int Wi, int C, const float* flow
   constexpr int VMAX = 16 / sizeof(T);
   long long px = (long long)(up2 ? 4 : 1) * hf * wf;
   bool aligned = ((uintptr_t)src % 16 == 0) && ((uintptr_t)out % 16 == 0);
-  if (false && C % (2 * VMAX) == 0 && aligned && C / (2 * VMAX) <= 256) {   // 32 B / thread variant: disabled
-    const int cv = C / (2 * VMAX), ppb = 256 / cv;   // pixels per block, 32 bytes per thread
-    warp_vec_kernel<T, VMAX, 2><<<dim3(cdiv(px, ppb), 1, nimg), 256, 0, st>>>((const T*)src, Hi, Wi, C, flow, hf, wf, up2, (T*)out, ppb);
-  } else if (C % VMAX == 0 && aligned && C / VMAX <= 256) {
-    const int cv = C / VMAX, ppb = 256 / cv;
-    warp_vec_kernel<T, VMAX, 1><<<dim3(cdiv(px, ppb), 1, nimg), 256, 0, st>>>((const T*)src, Hi, Wi, C, flow, hf, wf, up2, (T*)out, ppb);
+  if (C % VMAX == 0 && aligned && C / VMAX <= 256) {
+    const int cv = C / VMAX, ppb = 256 / cv;         // pixels per block
+    warp_vec_kernel<T, VMAX><<<dim3(cdiv(px, ppb), 1, nimg), 256, 0, st>>>((const T*)src, Hi, Wi, C, flow, hf, wf, up2, (T*)out, ppb);
   } else {
     long long n = px * C;
     warp_kernel<T, 1><<<dim3(cdiv(n, 256), 1, nimg), 256, 0, st>>>((const T*)src, Hi, Wi, C, flow, hf, wf, up2, (T*)out);
@@ -1464,28 +1381,17 @@ extern "C" int rv_warp3_batched(const void* feat, const void* featUP, const floa
   RV_REQUIRE(dtype == RV_F16 || dtype == RV_BF16, "rv_warp3: f16 / bf16 features only (use rv_warp for fp32)");
   RV_REQUIRE(C > 0 && C % 8 == 0, "rv_warp3: C=%d must be a multiple of 8", C);
   RV_REQUIRE((long long)4 * h * w * (C / 8) < (1ll << 31), "rv_warp3: map too large for 32-bit vector indices");
-  // tile shape (REFVSR_W3_TILE: 0 = 8 x 16 LR pixels / 256 threads, 1 = 4 x 16 / 256, 2 = 2 x 16 / 160).  Measured at 270x480x48 bf16
-  // on an H100 80GB HBM3 at a 400 W limit (tools/pointwise_bench.py): 52.7 / 52.7 / 57.3 us - every CTA pays the flow-tile load and
-  // two barriers before its first gather, so the smallest tiles lose
-  static const int tile_env = getenv("REFVSR_W3_TILE") ? atoi(getenv("REFVSR_W3_TILE")) : RV_W3_TILE_DEFAULT;
-  auto launch = [&](auto tag, auto cvtag, auto thtag) {
+  const int tiles = ((h + W3_TH - 1) / W3_TH) * ((w + W3_TW - 1) / W3_TW);
+  auto launch = [&](auto tag, auto cvtag) {
     using T = decltype(tag);
-    constexpr int TH = decltype(thtag)::value, TW = 16;
-    const int tiles = ((h + TH - 1) / TH) * ((w + TW - 1) / TW);
-    const int threads = TH == 2 ? 160 : 256;
-    warp3_kernel<T, decltype(cvtag)::value, TH, TW><<<dim3(tiles, 1, n), threads, 0, (cudaStream_t)stream>>>(
+    warp3_kernel<T, decltype(cvtag)::value><<<dim3(tiles, 1, n), 256, 0, (cudaStream_t)stream>>>(
         (const T*)feat, (const T*)featUP, conf, flow, h, w, C, (T*)out_feat, (T*)out_featUP, out_conf);
   };
-  auto by_tile = [&](auto tag, auto cvtag) {
-    if (tile_env == 2) launch(tag, cvtag, std::integral_constant<int, 2>{});
-    else if (tile_env == 1) launch(tag, cvtag, std::integral_constant<int, 4>{});
-    else launch(tag, cvtag, std::integral_constant<int, 8>{});
-  };
   auto by_cv = [&](auto tag) {           // the reference's widths (48 / 24 channels, config_RefVSR_*.py) + powers of two
-    if (C == 48) by_tile(tag, std::integral_constant<int, 6>{});
-    else if (C == 24) by_tile(tag, std::integral_constant<int, 3>{});
-    else if (C == 64) by_tile(tag, std::integral_constant<int, 8>{});
-    else by_tile(tag, std::integral_constant<int, 0>{});
+    if (C == 48) launch(tag, std::integral_constant<int, 6>{});
+    else if (C == 24) launch(tag, std::integral_constant<int, 3>{});
+    else if (C == 64) launch(tag, std::integral_constant<int, 8>{});
+    else launch(tag, std::integral_constant<int, 0>{});
   };
   if (dtype == RV_F16) by_cv(__half{});
   else by_cv(__nv_bfloat16{});
@@ -1522,8 +1428,7 @@ extern "C" int rv_gather_blocks(const void* value, int Hv, int Wv, int C, int dt
   uint8_t* o = (uint8_t*)out;
   bool a16 = ((uintptr_t)value % 16 == 0) && ((uintptr_t)out % 16 == 0);
   bool a4 = ((uintptr_t)value % 4 == 0) && ((uintptr_t)out % 4 == 0);   // 4-byte words need 4-byte aligned rows
-  static const bool fast_ok = getenv("REFVSR_NO_FAST_POINTWISE") == nullptr;
-  if (fast_ok && rowbytes % 16 == 0 && a16 && (ks == 1 || ks == 2 || ks == 4) && hq <= 65535) {
+  if (fast_pointwise() && rowbytes % 16 == 0 && a16 && (ks == 1 || ks == 2 || ks == 4) && hq <= 65535) {
     const int nv = rowbytes / 16;
     const dim3 grid((unsigned)cdiv((long long)wq * nv, 256), (unsigned)hq);
     const uint4* v4 = (const uint4*)value;
@@ -1553,32 +1458,23 @@ static int aligned_sample_launch(const void* x, int h, int w, int ks, int C, con
   constexpr int VMAX = 16 / sizeof(T);
   long long px = (long long)ks * h * ks * w;
   bool a16 = ((uintptr_t)x % 16 == 0) && ((uintptr_t)out % 16 == 0);
-  static const bool fast_ok = getenv("REFVSR_NO_FAST_POINTWISE") == nullptr;
-  if (fast_ok && ks == 2 && C % VMAX == 0 && a16 && px * (C / VMAX) < (1ll << 31))       // (32-bit vector indices)
-  {
-    static const int tile_env = getenv("REFVSR_AS_TILE") ? atoi(getenv("REFVSR_AS_TILE")) : RV_AS_TILE_DEFAULT;
+  if (fast_pointwise() && (ks == 2 || ks == 4) && C % VMAX == 0 && a16 && px * (C / VMAX) < (1ll << 31)) {   // (32-bit vector indices)
     const int cv = C / VMAX;
-    auto launch = [&](auto cvtag, auto thtag) {
-      constexpr int TH = decltype(thtag)::value;
-      const int tiles = ((h + TH - 1) / TH) * ((w + 15) / 16);
-      aligned_sample2_kernel<T, decltype(cvtag)::value, TH><<<tiles, TH == 2 ? 128 : 256, 0, st>>>((const T*)x, h, w, C, affine, (T*)out);
+    auto launch = [&](auto kstag) {
+      constexpr int KS = decltype(kstag)::value, TH = KS == 2 ? 4 : 8, TW = KS == 2 ? 16 : 8;
+      const int tiles = ((h + TH - 1) / TH) * ((w + TW - 1) / TW);
+      auto run = [&](auto cvtag) {
+        constexpr int CV = decltype(cvtag)::value;
+        const auto kernel = KS == 2 ? aligned_sample2_kernel<T, CV> : aligned_sample4_kernel<T, CV>;
+        kernel<<<tiles, 256, 0, st>>>((const T*)x, h, w, C, affine, (T*)out);
+      };
+      if (cv == 6) run(std::integral_constant<int, 6>{});
+      else if (cv == 3) run(std::integral_constant<int, 3>{});
+      else if (cv == 12) run(std::integral_constant<int, 12>{});
+      else run(std::integral_constant<int, 0>{});
     };
-    auto by_tile = [&](auto cvtag) {
-      if (tile_env == 2) launch(cvtag, std::integral_constant<int, 2>{});
-      else if (tile_env == 1) launch(cvtag, std::integral_constant<int, 4>{});
-      else launch(cvtag, std::integral_constant<int, 8>{});
-    };
-    if (cv == 6) by_tile(std::integral_constant<int, 6>{});
-    else if (cv == 3) by_tile(std::integral_constant<int, 3>{});
-    else if (cv == 12) by_tile(std::integral_constant<int, 12>{});
-    else by_tile(std::integral_constant<int, 0>{});
-  }
-  else if (fast_ok && ks == 4 && C % VMAX == 0 && a16 && px * (C / VMAX) < (1ll << 31)) {
-    const int cv = C / VMAX, tiles = ((h + 7) / 8) * ((w + 7) / 8);
-    if (cv == 6) aligned_sample4_kernel<T, 6><<<tiles, 256, 0, st>>>((const T*)x, h, w, C, affine, (T*)out);
-    else if (cv == 3) aligned_sample4_kernel<T, 3><<<tiles, 256, 0, st>>>((const T*)x, h, w, C, affine, (T*)out);
-    else if (cv == 12) aligned_sample4_kernel<T, 12><<<tiles, 256, 0, st>>>((const T*)x, h, w, C, affine, (T*)out);
-    else aligned_sample4_kernel<T, 0><<<tiles, 256, 0, st>>>((const T*)x, h, w, C, affine, (T*)out);
+    if (ks == 2) launch(std::integral_constant<int, 2>{});
+    else launch(std::integral_constant<int, 4>{});
   }
   else if (C % VMAX == 0 && a16)
     aligned_sample_kernel<T, VMAX><<<cdiv(px * (C / VMAX), 256), 256, 0, st>>>((const T*)x, h, w, ks, C, affine, (T*)out);
@@ -1658,16 +1554,24 @@ extern "C" int rv_conf_max(const float* a, const float* b, float* out, int n, vo
   return RV_OK;
 }
 
+// The reconstruction path of rv_reconstruct{,_u8}_batched: the x4 / x2 kernels for an aligned 4-channel fp32 conv_last output,
+// the generic kernels otherwise.  The 8-bit tail follows the same choice, so each byte comes from the value the fp32 kernel writes.
+enum class RecPath { X4, X2, GENERIC };
+static RecPath reconstruct_path(const void* x, int xc, int x_dtype, int scale) {
+  if (fast_pointwise() && x_dtype == RV_F32 && xc == 4 && (uintptr_t)x % 16 == 0) return scale == 4 ? RecPath::X4 : RecPath::X2;
+  return RecPath::GENERIC;
+}
+
 extern "C" int rv_reconstruct_batched(const void* x, int xc, int x_dtype, const float* lr, int h, int w,
                                       int scale, int clamp01, float* out, int nimg, void* stream) {
   RV_REQUIRE(x && lr && out && h > 0 && w > 0 && xc >= 3 && (scale == 2 || scale == 4),
              "rv_reconstruct: bad arguments");
   RV_REQUIRE(nimg >= 1 && nimg <= 65535, "rv_reconstruct: n=%d images out of range", nimg);
   long long n = (long long)scale * h * scale * w;
-  static const bool fast_ok = getenv("REFVSR_NO_FAST_POINTWISE") == nullptr;
-  if (fast_ok && scale == 4 && x_dtype == RV_F32 && xc == 4 && (uintptr_t)x % 16 == 0 && (uintptr_t)out % 16 == 0) {
+  const RecPath path = reconstruct_path(x, xc, x_dtype, scale);
+  if (path == RecPath::X4 && (uintptr_t)out % 16 == 0) {
     reconstruct4_kernel<<<dim3(cdiv((long long)h * w, 128), 1, nimg), 128, 0, (cudaStream_t)stream>>>((const float4*)x, lr, h, w, clamp01, out);
-  } else if (fast_ok && scale == 2 && x_dtype == RV_F32 && xc == 4 && (uintptr_t)x % 16 == 0 && (uintptr_t)out % 8 == 0) {
+  } else if (path == RecPath::X2 && (uintptr_t)out % 8 == 0) {
     reconstruct2_kernel<<<dim3(cdiv((long long)h * w, 128), 1, nimg), 128, 0, (cudaStream_t)stream>>>((const float4*)x, lr, h, w, clamp01, out);
   } else {
     RV_DISPATCH_DTYPE(x_dtype, T, (reconstruct_kernel<T><<<dim3(cdiv(n, 256), 1, nimg), 256, 0, (cudaStream_t)stream>>>(
@@ -1688,17 +1592,16 @@ extern "C" int rv_reconstruct_u8_batched(const void* x, int xc, int x_dtype, con
              "rv_reconstruct_u8: bad arguments");
   RV_REQUIRE(nimg >= 1 && nimg <= 65535, "rv_reconstruct_u8: n=%d images out of range", nimg);
   RV_REQUIRE((long long)scale * h * scale * w <= (1ll << 30), "rv_reconstruct_u8: %d x %d output too large", scale * h, scale * w);
-  // the fp32 path's dispatch (rv_reconstruct_batched), so each output byte comes from the value that kernel writes
-  static const bool fast_ok = getenv("REFVSR_NO_FAST_POINTWISE") == nullptr;
+  const RecPath path = reconstruct_path(x, xc, x_dtype, scale);
   const bool aligned = (uintptr_t)out % 16 == 0;
   const int Wo = scale * w;
   cudaStream_t st = (cudaStream_t)stream;
-  if (fast_ok && scale == 4 && x_dtype == RV_F32 && xc == 4 && (uintptr_t)x % 16 == 0) {
+  if (path == RecPath::X4) {
     const int vec = aligned && (3 * Wo) % 16 == 0;
     const dim3 grid(cdiv((long long)h * ((w + 3) / 4), 128), 1, nimg);
     if (bgr) reconstruct4_u8_kernel<true><<<grid, 128, 0, st>>>((const float4*)x, lr, h, w, clamp01, vec, out);
     else reconstruct4_u8_kernel<false><<<grid, 128, 0, st>>>((const float4*)x, lr, h, w, clamp01, vec, out);
-  } else if (fast_ok && scale == 2 && x_dtype == RV_F32 && xc == 4 && (uintptr_t)x % 16 == 0) {
+  } else if (path == RecPath::X2) {
     const int vec = aligned && (3 * Wo) % 16 == 0;
     const dim3 grid(cdiv((long long)h * ((w + 7) / 8), 128), 1, nimg);
     if (bgr) reconstruct2_u8_kernel<true><<<grid, 128, 0, st>>>((const float4*)x, lr, h, w, clamp01, vec, out);

@@ -323,19 +323,13 @@ class CudaOps:
     # -- warp -------------------------------------------------------------------------------------
     def warp(self, src, flow, out, flow_up2=False):
         _chk_dev(src, flow, out)
-        if flow.dim() == 4:                        # a batch of n images: (n, ...) operands, one launch
-            n = flow.shape[0]
-            Hi, Wi, Cc = (src.shape[1], src.shape[2], 1) if src.dim() == 3 else src.shape[1:]
-            assert src.shape[0] == out.shape[0] == n
-            _check(self.lib, self.lib.rv_warp_batched(_ptr(src), Hi, Wi, Cc, DTYPE_CODE[src.dtype], _ptr(flow), flow.shape[1],
-                                                      flow.shape[2], int(flow_up2), _ptr(out), n, self._stream()), 'rv_warp')
-            return
-        if src.dim() == 2:
-            Hi, Wi, Cc = src.shape[0], src.shape[1], 1
-        else:
-            Hi, Wi, Cc = src.shape
-        _check(self.lib, self.lib.rv_warp(_ptr(src), Hi, Wi, Cc, DTYPE_CODE[src.dtype], _ptr(flow), flow.shape[0],
-                                          flow.shape[1], int(flow_up2), _ptr(out), self._stream()), 'rv_warp')
+        if flow.dim() == 3:                        # one image: a batch of 1
+            src, flow, out = src[None], flow[None], out[None]
+        n = flow.shape[0]                          # a batch of n images: (n, ...) operands, one launch
+        Hi, Wi, Cc = (src.shape[1], src.shape[2], 1) if src.dim() == 3 else src.shape[1:]
+        assert src.shape[0] == out.shape[0] == n
+        _check(self.lib, self.lib.rv_warp_batched(_ptr(src), Hi, Wi, Cc, DTYPE_CODE[src.dtype], _ptr(flow), flow.shape[1],
+                                                  flow.shape[2], int(flow_up2), _ptr(out), n, self._stream()), 'rv_warp')
 
     def warp3(self, feat, featUP, conf, flow, out_feat, out_featUP, out_conf):
         """the three warps of one propagation step in one launch (16-bit features)"""
@@ -346,12 +340,9 @@ class CudaOps:
         assert tuple(featUP.shape) == lead + (2 * h, 2 * w, Cc) and tuple(conf.shape) == lead + (h, w)
         assert tuple(flow.shape) == lead + (h, w, 2) and tuple(feat.shape) == lead + (h, w, Cc)
         assert feat.dtype == featUP.dtype == out_feat.dtype == out_featUP.dtype and conf.dtype == torch.float32
-        args = (_ptr(feat), _ptr(featUP), _ptr(conf), _ptr(flow), h, w, Cc, DTYPE_CODE[feat.dtype],
-                _ptr(out_feat), _ptr(out_featUP), _ptr(out_conf))
-        if n:
-            _check(self.lib, self.lib.rv_warp3_batched(*args, n, self._stream()), 'rv_warp3')
-        else:
-            _check(self.lib, self.lib.rv_warp3(*args, self._stream()), 'rv_warp3')
+        _check(self.lib, self.lib.rv_warp3_batched(_ptr(feat), _ptr(featUP), _ptr(conf), _ptr(flow), h, w, Cc, DTYPE_CODE[feat.dtype],
+                                                   _ptr(out_feat), _ptr(out_featUP), _ptr(out_conf), max(n, 1), self._stream()),
+               'rv_warp3')
 
     # -- matching ---------------------------------------------------------------------------------
     def patch_pack(self, feat, out, mode):
@@ -389,14 +380,12 @@ class CudaOps:
     # -- confidence maps --------------------------------------------------------------------------
     def conf_pair(self, a, b, out, up2=False):
         _chk_dev(a, b, out)
-        if out.dim() == 4:                         # a batch of n images: (n, ...) operands, one launch
-            assert a.shape[0] == b.shape[0] == out.shape[0]
-            _check(self.lib, self.lib.rv_conf_pair_batched(_ptr(a), _ptr(b), a.shape[1], a.shape[2], int(up2), _ptr(out),
-                                                           out.shape[3], DTYPE_CODE[out.dtype], out.shape[0], self._stream()),
-                   'rv_conf_pair')
-            return
-        _check(self.lib, self.lib.rv_conf_pair(_ptr(a), _ptr(b), a.shape[0], a.shape[1], int(up2), _ptr(out),
-                                               out.shape[2], DTYPE_CODE[out.dtype], self._stream()), 'rv_conf_pair')
+        if out.dim() == 3:                         # one image: a batch of 1
+            a, b, out = a[None], b[None], out[None]
+        assert a.shape[0] == b.shape[0] == out.shape[0]   # a batch of n images: (n, ...) operands, one launch
+        _check(self.lib, self.lib.rv_conf_pair_batched(_ptr(a), _ptr(b), a.shape[1], a.shape[2], int(up2), _ptr(out),
+                                                       out.shape[3], DTYPE_CODE[out.dtype], out.shape[0], self._stream()),
+               'rv_conf_pair')
 
     def conf_max(self, a, b, out):
         _chk_dev(a, b, out)
@@ -418,30 +407,24 @@ class CudaOps:
     # -- tail -------------------------------------------------------------------------------------
     def reconstruct(self, x, lr, scale, clamp01, out):
         _chk_dev(x, lr, out)
-        if lr.dim() == 4:                          # a batch of n images: (n, ...) operands, one launch
-            assert x.shape[0] == out.shape[0] == lr.shape[0]
-            _check(self.lib, self.lib.rv_reconstruct_batched(_ptr(x), x.shape[3], DTYPE_CODE[x.dtype], _ptr(lr), lr.shape[2],
-                                                             lr.shape[3], scale, int(clamp01), _ptr(out), lr.shape[0],
-                                                             self._stream()), 'rv_reconstruct')
-            return
-        _check(self.lib, self.lib.rv_reconstruct(_ptr(x), x.shape[2], DTYPE_CODE[x.dtype], _ptr(lr), lr.shape[1],
-                                                 lr.shape[2], scale, int(clamp01), _ptr(out), self._stream()),
-               'rv_reconstruct')
+        if lr.dim() == 3:                          # one image: a batch of 1
+            x, lr, out = x[None], lr[None], out[None]
+        assert x.shape[0] == out.shape[0] == lr.shape[0]  # a batch of n images: (n, ...) operands, one launch
+        _check(self.lib, self.lib.rv_reconstruct_batched(_ptr(x), x.shape[3], DTYPE_CODE[x.dtype], _ptr(lr), lr.shape[2],
+                                                         lr.shape[3], scale, int(clamp01), _ptr(out), lr.shape[0],
+                                                         self._stream()), 'rv_reconstruct')
 
     def reconstruct_u8(self, x, lr, scale, clamp01, out, bgr):
         """reconstruct() with 8-bit HWC output: out (scale*h, scale*w, 3) uint8, or (n, scale*h, scale*w, 3) for a batch, gets the
         bytes frame_u8 makes of the values reconstruct() would write (rv_reconstruct_u8); bgr: B, G, R byte order"""
         _chk_dev(x, lr, out)
         assert out.dtype == torch.uint8 and out.shape[-1] == 3
-        if lr.dim() == 4:                          # a batch of n images: (n, ...) operands, one launch
-            assert x.shape[0] == out.shape[0] == lr.shape[0]
-            _check(self.lib, self.lib.rv_reconstruct_u8_batched(_ptr(x), x.shape[3], DTYPE_CODE[x.dtype], _ptr(lr), lr.shape[2],
-                                                                lr.shape[3], scale, int(clamp01), int(bool(bgr)), _ptr(out),
-                                                                lr.shape[0], self._stream()), 'rv_reconstruct_u8')
-            return
-        _check(self.lib, self.lib.rv_reconstruct_u8(_ptr(x), x.shape[2], DTYPE_CODE[x.dtype], _ptr(lr), lr.shape[1], lr.shape[2],
-                                                    scale, int(clamp01), int(bool(bgr)), _ptr(out), self._stream()),
-               'rv_reconstruct_u8')
+        if lr.dim() == 3:                          # one image: a batch of 1
+            x, lr, out = x[None], lr[None], out[None]
+        assert x.shape[0] == out.shape[0] == lr.shape[0]  # a batch of n images: (n, ...) operands, one launch
+        _check(self.lib, self.lib.rv_reconstruct_u8_batched(_ptr(x), x.shape[3], DTYPE_CODE[x.dtype], _ptr(lr), lr.shape[2],
+                                                            lr.shape[3], scale, int(clamp01), int(bool(bgr)), _ptr(out),
+                                                            lr.shape[0], self._stream()), 'rv_reconstruct_u8')
 
     # -- 8-bit frames -----------------------------------------------------------------------------
     def frames_from_u8(self, srcs, dsts, bgr):

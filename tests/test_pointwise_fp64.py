@@ -46,13 +46,10 @@ in a batch fail (the CPU self-tests below plant each of them into a fake kernel)
 
 Without a GPU: those self-tests, and the list of operator calls below against what the engine launches.  With a GPU: every
 (signature, geometry) of the list in bf16 and fp16 (and fp32 where the fp32 engine launches it), plus cases named for the
-kernel branch they force: batched, ragged tiles, misaligned outputs and the selectable tile shapes."""
+kernel branch they force: batched, ragged tiles and misaligned outputs."""
 import collections
 import inspect
-import os
 import re
-import subprocess
-import sys
 import zlib
 
 import numpy as np
@@ -65,7 +62,6 @@ from test_conv_fp64 import ulp
 U = 2.0 ** -24
 C_AR = 64.0
 GUARD = 4096
-HERE = os.path.dirname(os.path.abspath(__file__))
 
 # ------------------------------------------------------------------------------------------------------------------
 # the list: every non-conv, non-GEMM operator call of the engine
@@ -1163,7 +1159,7 @@ BRANCH_CASES = [
      dict(n=3, expect=r'reconstruct2_u8_kernel')),
     ('ragged-271x483-warp3', _entry('warp3'), (271, 483), torch.bfloat16, dict(expect=r'warp3_kernel')),
     ('ragged-271x483-warp3-fp16', _entry('warp3'), (271, 483), torch.float16, dict(expect=r'warp3_kernel')),
-    ('ragged-warp3-c24', _entry('warp3'), (37, 53), torch.bfloat16, dict(C=24, expect=r'warp3_kernel<__nv_bfloat16, 3,')),
+    ('ragged-warp3-c24-cv3', _entry('warp3'), (37, 53), torch.bfloat16, dict(C=24, expect=r'warp3_kernel<__nv_bfloat16, 3>')),
     ('ragged-aligned-ks2', _entry('aligned_sample', ks=2), (135, 241), torch.bfloat16, dict(expect=r'aligned_sample2_kernel')),
     ('ragged-aligned-ks4', _entry('aligned_sample', ks=4), (67, 121), torch.float16, dict(expect=r'aligned_sample4_kernel')),
     ('ragged-gather-cells-ks4', _entry('gather_blocks', ks=4, ), (540, 964, 67, 121), torch.bfloat16,
@@ -1199,36 +1195,3 @@ def test_pointwise_branch(cuda_ops, case):
     outs, names = _kernels(lambda: run_guarded(cuda_ops, c, 'cuda', off=opt.get('off', 0)))
     assert any(re.search(opt['expect'], k) for k in names), (cid, sorted(names))
     c.verify(*outs)
-
-
-# the selectable tile shapes: REFVSR_W3_TILE 1 / 2 (4 x 16, 2 x 16 LR pixels) and REFVSR_AS_TILE 0 / 2 (8 x 16, 2 x 16 cells), read
-# once per process, run by tests/pointwise_tile_dump.py in a subprocess; (entry, geometry, dtype) of every dumped case
-TILE_CASES = [(_entry('warp3'), (270, 480), torch.bfloat16), (_entry('warp3'), (271, 483), torch.float16),
-              (_entry('aligned_sample', ks=2), (270, 480), torch.bfloat16), (_entry('aligned_sample', ks=2), (135, 241), torch.float16)]
-
-
-def tile_case(k):
-    e, geom, dt = TILE_CASES[k]
-    return build_case(_cpu_sig(e, dt), geom, dt, 'cuda', _seed('tile', k))
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize('env,want', [('REFVSR_W3_TILE=1', r'warp3_kernel<.*, 4, 16>'), ('REFVSR_W3_TILE=2', r'warp3_kernel<.*, 2, 16>'),
-                                      ('REFVSR_AS_TILE=0', r'aligned_sample2_kernel<.*, 8>'),
-                                      ('REFVSR_AS_TILE=2', r'aligned_sample2_kernel<.*, 2>')])
-def test_tile_shape_variant(cuda_ops, tmp_path, env, want):
-    """the dumped outputs of the variant against the float64 reference; torch.profiler shows that the variant's kernel ran"""
-    k, v = env.split('=')
-    path = str(tmp_path / 'dump.npz')
-    subprocess.run([sys.executable, os.path.join(HERE, 'pointwise_tile_dump.py'), path], check=True, cwd=tmp_path,
-                   env={**os.environ, k: v})
-    d = np.load(path)
-    assert any(re.search(want, n) for n in d['kernels']), (env, list(d['kernels']))
-    which = [i for i, (e, _, _) in enumerate(TILE_CASES) if e.sig.op == ('warp3' if 'W3' in k else 'aligned_sample')]
-    for i in which:
-        c = tile_case(i)
-        outs = []
-        for j, (shape, dtp) in enumerate(c.outs):
-            a = torch.from_numpy(d[f'{i}/{j}']).cuda()
-            outs.append(a.view(dtp) if dtp in (torch.bfloat16, torch.float16) else a)
-        c.verify(*outs)

@@ -1,5 +1,5 @@
 """Graph-timed launches of the HBM-bound kernels at the BASELINE shapes (same method as bench.kernel_rooflines: buffers
-rotated through > L2).  Tile-shape variants are selected by REFVSR_W3_TILE / REFVSR_AS_TILE (read once per process)."""
+rotated through > L2)."""
 import os
 import sys
 import torch
@@ -45,15 +45,14 @@ def main():
     cf, co = torch.rand((H, W), device=dev), torch.empty((H, W), device=dev)
     t = timeit(lambda i: ops.warp3(lf[i % n2], fs[i % n2], cf, flow, lo[i % n2], fo[i % n2], co))
     b = 2.0 * 5 * H * W * C * e + 2.0 * 4 * H * W + 8.0 * H * W
-    tag = f"W3_TILE={os.environ.get('REFVSR_W3_TILE', '-')} AS_TILE={os.environ.get('REFVSR_AS_TILE', '-')}"
-    print(f'{tag} warp3          {t * 1e6:7.2f} us  {b / t / 1e9:7.0f} GB/s  frac {b / t / 1e9 / PEAK:.3f}')
+    print(f'warp3          {t * 1e6:7.2f} us  {b / t / 1e9:7.0f} GB/s  frac {b / t / 1e9 / PEAK:.3f}')
     aff = torch.rand((H, W, 3), device=dev) * 0.4 + 0.8
     t = timeit(lambda i: ops.aligned_sample(fs[i % n2], aff, 2, fo[(i + 1) % n2]))
     b = 12.0 * H * W + 2.0 * 4 * C * H * W * e
-    print(f'{tag} aligned_sample {t * 1e6:7.2f} us  {b / t / 1e9:7.0f} GB/s  frac {b / t / 1e9 / PEAK:.3f}')
+    print(f'aligned_sample {t * 1e6:7.2f} us  {b / t / 1e9:7.0f} GB/s  frac {b / t / 1e9 / PEAK:.3f}')
     t = timeit(lambda i: ops.warp(fs[i % n2], flow, fo[i % n2], flow_up2=True))
     b = 2.0 * 4 * H * W * C * e + 8.0 * H * W
-    print(f'{tag} warp_up        {t * 1e6:7.2f} us  {b / t / 1e9:7.0f} GB/s  frac {b / t / 1e9 / PEAK:.3f}')
+    print(f'warp_up        {t * 1e6:7.2f} us  {b / t / 1e9:7.0f} GB/s  frac {b / t / 1e9 / PEAK:.3f}')
 
 
 if __name__ == '__main__':
