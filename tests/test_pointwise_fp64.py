@@ -131,8 +131,8 @@ DT = {v: k for k, v in DTN.items()}
 POINTWISE_OPS = ('warp', 'warp3', 'spynet_resize_norm', 'avgpool2', 'spynet_level_input', 'flow_resize', 'prep_image', 'maxpool2',
                  'resize_planes', 'patch_pack', 'gather_blocks', 'space_to_depth2', 'bicubic_up2_image', 'aligned_sample', 'conf_pair',
                  'conf_max', 'reconstruct', 'reconstruct_u8')
-# the other operators the engine calls: the convs (test_conv_fp64.py), the matching GEMM (test_match_tc.py), the reuse guard and
-# the 8-bit input conversion (test_gpu_u8_frames.py)
+# the other operators the engine calls: the convs (test_conv_fp64.py), the matching GEMM (test_match_fp64.py), the reuse guard
+# (test_frames_differ.py) and the 8-bit input conversion (test_gpu_u8_frames.py)
 ELSEWHERE = {'conv2d', 'pack_conv', 'match_argmax', 'frames_differ', 'frames_from_u8', 'launch_count'}
 
 
@@ -239,7 +239,7 @@ def _recording_ops(compute):
     return Recording()
 
 
-def _run_engine(ops, h, w, prec, cfg_name='config_RefVSR_MFID', u8=None, **over):
+def _run_engine(ops, h, w, prec, cfg_name='config_RefVSR_MFID', u8=None, ref_scale=1, **over):
     from refvsr_b200 import SRNet, get_config
     from refvsr_b200.modules import seeded_test_weights
     from refvsr_b200.synth import make_clip, sliding_windows
@@ -247,7 +247,7 @@ def _run_engine(ops, h, w, prec, cfg_name='config_RefVSR_MFID', u8=None, **over)
     net = SRNet(cfg).eval()
     seeded_test_weights(net, seed=5)
     net.Network.set_ops(ops)
-    lrs, refs = make_clip(cfg.frame_num, h, w, 1, seed=5)
+    lrs, refs = make_clip(cfg.frame_num, h, w, ref_scale, seed=5)
     with torch.no_grad():
         for n, (k, wl, wr, first) in enumerate(sliding_windows(lrs, refs, cfg.frame_num)):
             if u8 is None:
