@@ -36,6 +36,18 @@ extern "C" {
 #define RV_E_CUDA (-2)    /* CUDA runtime / driver error, see rv_last_error()   */
 #define RV_E_UNSUPPORTED (-3)
 
+/* 8-bit frame formats of rv_frames_from_u8 and rv_reconstruct_u8{,_batched}.  An (H, W) frame is one contiguous block:
+ *   RGB, BGR    (H, W, 3) HWC bytes, R, G, B or B, G, R per pixel: 3 * H * W bytes
+ *   I420        the (H, W) Y plane, then U (H/2, W/2), then V (H/2, W/2): 3 * H * W / 2 bytes (ffmpeg's yuv420p)
+ *   NV12        the (H, W) Y plane, then (H/2, W) rows of interleaved U, V pairs: 3 * H * W / 2 bytes
+ * The 4:2:0 formats are exactly OpenCV's cvtColor conversions (BT.601 limited range, 20-bit fixed point; csrc/frame_u8.cuh):
+ * in, the frame stands for the RGB bytes COLOR_YUV2RGB_I420 / _NV12 gives (nearest chroma); out, it is COLOR_RGB2YUV_I420 of
+ * the RGB bytes (chroma from each 2 x 2 block's top-left pixel), interleaved for NV12.  H and W must be even. */
+#define RV_FRAME_RGB 0
+#define RV_FRAME_BGR 1
+#define RV_FRAME_I420 2
+#define RV_FRAME_NV12 3
+
 /* activation codes used by rv_conv2d epilogues */
 #define RV_ACT_NONE 0
 #define RV_ACT_RELU 1     /* SPyNet ConvModule, ResidualBlockNoBN (sr_backbone_utils.py:85-97)      */
@@ -325,28 +337,32 @@ int rv_reconstruct(const void* x, int xc, int x_dtype, const float* lr_nchw, int
 int rv_reconstruct_batched(const void* x, int xc, int x_dtype, const float* lr_nchw, int h, int w, int scale,
                            int clamp01, float* out_nchw, int n, void* stream);   /* see rv_warp_batched */
 /* The same reconstruction with 8-bit output: each value the matching rv_reconstruct{,_batched} call writes becomes the byte
- * cv::Mat::convertTo(CV_8U) makes of fl32(v * 255) (csrc/frame_u8.cuh: round half to even, saturated; NaN -> 0), stored HWC
- * (scale*h, scale*w, 3), images packed one after the other for n > 1.  bgr = 0: R, G, B bytes per pixel; 1: B, G, R (cv2's
- * order).  The kernel is chosen as rv_reconstruct chooses its own (x4 / x2 fast paths for fp32 x with xc = 4, the generic kernel
- * otherwise), and computes each value with that kernel's expressions.  16-byte stores of 16-pixel row runs where out is
- * 16-byte aligned and a row is a multiple of 16 bytes; byte stores elsewhere, to the same bytes. */
-int rv_reconstruct_u8(const void* x, int xc, int x_dtype, const float* lr_nchw, int h, int w, int scale, int clamp01, int bgr,
-                      uint8_t* out_hwc, void* stream);
+ * cv::Mat::convertTo(CV_8U) makes of fl32(v * 255) (csrc/frame_u8.cuh: round half to even, saturated; NaN -> 0), stored
+ * as an (scale*h, scale*w) frame of format fmt (RV_FRAME_*; RGB: R, G, B bytes per pixel, BGR: cv2's order, I420 / NV12: the
+ * 4:2:0 frame of those RGB bytes), images packed one after the other for n > 1.  The kernel is chosen as rv_reconstruct
+ * chooses its own (x4 / x2 fast paths for fp32 x with xc = 4, the generic kernel otherwise), and computes each value with that
+ * kernel's expressions.  16-byte stores of 16-pixel row runs (8-byte stores of I420's 8-sample chroma runs) where out is 16-byte
+ * aligned and a row is a multiple of 16 pixels (generic kernel: where an image is a multiple of 16 bytes); byte stores
+ * elsewhere, to the same bytes.  RV_E_INVALID for a format code outside RV_FRAME_*. */
+int rv_reconstruct_u8(const void* x, int xc, int x_dtype, const float* lr_nchw, int h, int w, int scale, int clamp01, int fmt,
+                      uint8_t* out, void* stream);
 int rv_reconstruct_u8_batched(const void* x, int xc, int x_dtype, const float* lr_nchw, int h, int w, int scale, int clamp01,
-                              int bgr, uint8_t* out_hwc, int n, void* stream);
+                              int fmt, uint8_t* out, int n, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * rv_frames_from_u8 - decoded 8-bit video frames into the engine's fp32 frames (data_loader/utils.py::read_frame's
  * np.array(frame) / 255. cast to float32).
- *   src    HOST array of k device pointers, each a contiguous uint8 (h, w, 3) HWC frame, any alignment; bgr = 1: the bytes of a
- *          pixel are B, G, R (cv2's order), 0: R, G, B
+ *   src    HOST array of k device pointers, each a contiguous (h, w) uint8 frame of format fmt (RV_FRAME_*), any alignment
  *   dst    HOST array of k device pointers, each a contiguous fp32 (3, h, w) planar RGB frame
- *   1 <= k <= 16, h, w >= 1, h * w <= 2^28
- * Byte u becomes fl32(u / 255) with IEEE division (round to nearest).  One launch; 16-byte loads wherever a frame has 16-byte
- * aligned runs of 16 pixels (every frame but at most 30 pixels of it), 16-byte stores where dst allows.
+ *   1 <= k <= 16, h, w >= 1, h * w <= 2^28; h and w even for I420 / NV12
+ * Byte u of the frame's R, G, B bytes (for 4:2:0, the bytes cv2.cvtColor(COLOR_YUV2RGB_I420 / _NV12) gives) becomes
+ * fl32(u / 255) with IEEE division (round to nearest).  One launch.  RGB / BGR: 16-byte loads wherever a frame has 16-byte
+ * aligned runs of 16 pixels (every frame but at most 30 pixels of it), 16-byte stores where dst allows.  4:2:0: 16-byte loads of
+ * the Y rows and each chroma sample read once per 2 x 2 block where src is 16-byte aligned and w a multiple of 16, byte loads
+ * otherwise; 16-byte stores where dst is aligned too.
  * RV_E_INVALID for any argument outside the above.
  * ------------------------------------------------------------------------------------------------ */
-int rv_frames_from_u8(const uint8_t* const* src, float* const* dst, int k, int h, int w, int bgr, void* stream);
+int rv_frames_from_u8(const uint8_t* const* src, float* const* dst, int k, int h, int w, int fmt, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * rv_region_metrics - the per-frame sums behind the FOV evaluation mode: evaluation/metrics.py:18-31 (psnr, psnr_masked,

@@ -1073,36 +1073,87 @@ __global__ void __launch_bounds__(128) reconstruct2_kernel(const float4* __restr
 }
 
 // ---------------------------------------------------------------------------------------------
-// 8-bit HWC output of the reconstruction tail (rv_reconstruct_u8): one variant per fp32 kernel above, each computing the same
-// fp32 value with the same expressions before rv::frame_u8 turns it into a byte.  A thread owns 16 consecutive output pixels of
-// a row (48 bytes) and writes them as three 16-byte stores where the row and the buffer allow it (vec), byte by byte elsewhere.
-// BGR: the pixel's bytes are B, G, R instead of R, G, B.
+// 8-bit output of the reconstruction tail (rv_reconstruct_u8): one variant per fp32 kernel above, each computing the same
+// fp32 value with the same expressions before rv::frame_u8 turns it into a byte.  A thread owns runs of 16 consecutive output
+// pixels of a row and writes each as 16-byte stores where the row and the buffer allow it (vec), byte by byte elsewhere.
+// FMT (RV_FRAME_*): RGB / BGR write a run's 48 HWC bytes, R, G, B or B, G, R.  I420 / NV12 write its 16 Y bytes, and from each
+// even row the U, V bytes of its 2 x 2 blocks, taken from the blocks' top-left pixels (COLOR_RGB2YUV_I420, rv::rgb8_y/u/v).  The
+// x4 / x2 threads own whole blocks (4 or 2 output rows from an even row and column), so each writes its blocks' chroma itself.
 // ---------------------------------------------------------------------------------------------
-template <bool BGR>
-__device__ __forceinline__ void put_u8(uint32_t* words, int j, int c, float v) {   // j: pixel of the run, c: R, G, B
-  const int i = 3 * j + (BGR ? 2 - c : c);
-  words[i >> 2] |= frame_u8(v) << (8 * (i & 3));
+template <int FMT>
+__host__ __device__ constexpr bool is_yuv420() { return FMT == RV_FRAME_I420 || FMT == RV_FRAME_NV12; }
+
+template <int FMT>
+__host__ __device__ constexpr int run_words() { return is_yuv420<FMT>() ? 4 : 12; }    // the words of one 16-pixel run's bytes
+
+// pixel j of a run from its R, G, B values: HWC bytes, or a Y byte and, for a block's top-left pixel (tl), the block's U and V
+// as chroma sample j / 2 of the run (chroma: I420 U bytes 0-7 and V bytes 8-15, NV12 U, V pairs)
+template <int FMT>
+__device__ __forceinline__ void put_px(uint32_t* words, uint32_t* chroma, int j, bool tl, float r, float g, float b) {
+  const uint32_t R = frame_u8(r), G = frame_u8(g), B = frame_u8(b);
+  if constexpr (is_yuv420<FMT>()) {
+    words[j >> 2] |= rgb8_y(R, G, B) << (8 * (j & 3));
+    if (tl) {
+      const int iu = FMT == RV_FRAME_NV12 ? j : j / 2, iv = FMT == RV_FRAME_NV12 ? j + 1 : 8 + j / 2;
+      chroma[iu >> 2] |= rgb8_u(R, G, B) << (8 * (iu & 3));
+      chroma[iv >> 2] |= rgb8_v(R, G, B) << (8 * (iv & 3));
+    }
+  } else {
+    const uint32_t px = FMT == RV_FRAME_BGR ? (B | (G << 8) | (R << 16)) : (R | (G << 8) | (B << 16));
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const int i = 3 * j + c;
+      words[i >> 2] |= ((px >> (8 * c)) & 0xffu) << (8 * (i & 3));
+    }
+  }
 }
 
+// the first nbytes of a run of NB bytes (NB: 8 or a multiple of 16)
+template <int NB>
 __device__ __forceinline__ void store_run(uint8_t* o, const uint32_t* words, int nbytes, bool vec) {
-  if (vec && nbytes == 48) {
+  if (vec && nbytes == NB) {
+    if constexpr (NB == 8) {
+      *reinterpret_cast<uint2*>(o) = make_uint2(words[0], words[1]);
+    } else {
 #pragma unroll
-    for (int k = 0; k < 3; ++k)
-      reinterpret_cast<uint4*>(o)[k] = make_uint4(words[4 * k], words[4 * k + 1], words[4 * k + 2], words[4 * k + 3]);
+      for (int k = 0; k < NB / 16; ++k)
+        reinterpret_cast<uint4*>(o)[k] = make_uint4(words[4 * k], words[4 * k + 1], words[4 * k + 2], words[4 * k + 3]);
+    }
   } else {
 #pragma unroll
-    for (int i = 0; i < 48; ++i)
+    for (int i = 0; i < NB; ++i)
       if (i < nbytes) o[i] = (uint8_t)(words[i >> 2] >> (8 * (i & 3)));
   }
 }
 
+// one output run of an (Ho, Wo) image: n pixels of row y from column x; a 4:2:0 run from an even row also writes its n / 2
+// chroma samples
+template <int FMT>
+__device__ __forceinline__ void store_px_run(uint8_t* img, int Ho, int Wo, int y, int x, const uint32_t* words,
+                                             const uint32_t* chroma, int n, bool vec) {
+  if constexpr (is_yuv420<FMT>()) {
+    store_run<16>(img + (size_t)y * Wo + x, words, n, vec);
+    if (y % 2 == 0) {
+      uint8_t* c = img + (size_t)Ho * Wo;
+      if (FMT == RV_FRAME_NV12) {
+        store_run<16>(c + (size_t)(y / 2) * Wo + x, chroma, n, vec);
+      } else {
+        store_run<8>(c + (size_t)(y / 2) * (Wo / 2) + x / 2, chroma, n / 2, vec);
+        store_run<8>(c + (size_t)Ho * Wo / 4 + (size_t)(y / 2) * (Wo / 2) + x / 2, chroma + 2, n / 2, vec);
+      }
+    }
+  } else {
+    store_run<48>(img + 3 * ((size_t)y * Wo + x), words, 3 * n, vec);
+  }
+}
+
 // x4: reconstruct4_kernel's arithmetic for 4 neighbouring LR pixels per thread -> 4 output rows of 16 pixels
-template <bool BGR>
+template <int FMT>
 __global__ void __launch_bounds__(128) reconstruct4_u8_kernel(const float4* __restrict__ x, const float* __restrict__ lr, int h, int w,
                                                               int clamp01, int vec, uint8_t* __restrict__ out) {
   x += (size_t)blockIdx.z * 16 * h * w;
   lr += (size_t)blockIdx.z * 3 * h * w;
-  out += (size_t)blockIdx.z * 48 * h * w;
+  out += (size_t)blockIdx.z * (is_yuv420<FMT>() ? 24 : 48) * h * w;
   const int wq = (w + 3) / 4;
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= h * wq) return;
@@ -1115,7 +1166,8 @@ __global__ void __launch_bounds__(128) reconstruct4_u8_kernel(const float4* __re
     const float r = 0.25f * ((float)a + 0.5f) - 0.5f;
     cubic_weights(r - floorf(r), wt[a]);
   }
-  uint32_t ob[4][12] = {};                                     // [output row a][little-endian byte words of the 16-pixel run]
+  uint32_t ob[4][run_words<FMT>()] = {};                       // [output row a][little-endian byte words of the 16-pixel run]
+  uint32_t cb[2][4] = {};                                      // 4:2:0: [even row a / 2][chroma words of its 8 blocks]
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
     if (k >= nk) break;
@@ -1156,27 +1208,28 @@ __global__ void __launch_bounds__(128) reconstruct4_u8_kernel(const float4* __re
 #pragma unroll
       for (int b = 0; b < 4; ++b) {
         const float4 xv = __ldg(x + row + b);
+        float v[3];
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
           const float xr = (c == 0) ? xv.x : (c == 1 ? xv.y : xv.z);
-          float v = xr + res[c][a][b];
-          if (clamp01) v = fminf(fmaxf(v, 0.f), 1.f);
-          put_u8<BGR>(ob[a], 4 * k + b, c, v);
+          v[c] = xr + res[c][a][b];
+          if (clamp01) v[c] = fminf(fmaxf(v[c], 0.f), 1.f);
         }
+        put_px<FMT>(ob[a], cb[a / 2], 4 * k + b, a % 2 == 0 && b % 2 == 0, v[0], v[1], v[2]);
       }
     }
   }
 #pragma unroll
-  for (int a = 0; a < 4; ++a) store_run(out + 3 * ((size_t)(4 * ly + a) * Wo + 4 * lx0), ob[a], 12 * nk, vec);
+  for (int a = 0; a < 4; ++a) store_px_run<FMT>(out, 4 * h, Wo, 4 * ly + a, 4 * lx0, ob[a], cb[a / 2], 4 * nk, vec);
 }
 
 // x2: reconstruct2_kernel's arithmetic for 8 neighbouring LR pixels per thread -> 2 output rows of 16 pixels
-template <bool BGR>
+template <int FMT>
 __global__ void __launch_bounds__(128) reconstruct2_u8_kernel(const float4* __restrict__ x, const float* __restrict__ lr, int h, int w,
                                                               int clamp01, int vec, uint8_t* __restrict__ out) {
   x += (size_t)blockIdx.z * 4 * h * w;
   lr += (size_t)blockIdx.z * 3 * h * w;
-  out += (size_t)blockIdx.z * 12 * h * w;
+  out += (size_t)blockIdx.z * (is_yuv420<FMT>() ? 6 : 12) * h * w;
   const int wq = (w + 7) / 8;
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= h * wq) return;
@@ -1189,7 +1242,8 @@ __global__ void __launch_bounds__(128) reconstruct2_u8_kernel(const float4* __re
     const float r = 0.5f * ((float)a + 0.5f) - 0.5f;
     cubic_weights(r - floorf(r), wt[a]);
   }
-  uint32_t ob[2][12] = {};
+  uint32_t ob[2][run_words<FMT>()] = {};
+  uint32_t cb[4] = {};                                         // 4:2:0: the chroma words of row 0's 8 blocks
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
     if (k >= nk) break;
@@ -1224,42 +1278,59 @@ __global__ void __launch_bounds__(128) reconstruct2_u8_kernel(const float4* __re
     for (int a = 0; a < 2; ++a) {
       const size_t row = (size_t)(2 * ly + a) * Wo + 2 * lx;
       const float4 x0 = __ldg(x + row), x1 = __ldg(x + row + 1);
+      float v0[3], v1[3];
 #pragma unroll
       for (int c = 0; c < 3; ++c) {
-        float v0 = ((c == 0) ? x0.x : (c == 1 ? x0.y : x0.z)) + res[c][a][0];
-        float v1 = ((c == 0) ? x1.x : (c == 1 ? x1.y : x1.z)) + res[c][a][1];
-        if (clamp01) { v0 = fminf(fmaxf(v0, 0.f), 1.f); v1 = fminf(fmaxf(v1, 0.f), 1.f); }
-        put_u8<BGR>(ob[a], 2 * k, c, v0);
-        put_u8<BGR>(ob[a], 2 * k + 1, c, v1);
+        v0[c] = ((c == 0) ? x0.x : (c == 1 ? x0.y : x0.z)) + res[c][a][0];
+        v1[c] = ((c == 0) ? x1.x : (c == 1 ? x1.y : x1.z)) + res[c][a][1];
+        if (clamp01) { v0[c] = fminf(fmaxf(v0[c], 0.f), 1.f); v1[c] = fminf(fmaxf(v1[c], 0.f), 1.f); }
       }
+      put_px<FMT>(ob[a], cb, 2 * k, a == 0, v0[0], v0[1], v0[2]);
+      put_px<FMT>(ob[a], cb, 2 * k + 1, false, v1[0], v1[1], v1[2]);
     }
   }
 #pragma unroll
-  for (int a = 0; a < 2; ++a) store_run(out + 3 * ((size_t)(2 * ly + a) * Wo + 2 * lx0), ob[a], 6 * nk, vec);
+  for (int a = 0; a < 2; ++a) store_px_run<FMT>(out, 2 * h, Wo, 2 * ly + a, 2 * lx0, ob[a], cb, 2 * nk, vec);
 }
 
 // any scale, x dtype and channel count: reconstruct_kernel's arithmetic for 16 consecutive output pixels (row-major) per thread
-template <typename T, bool BGR>
+// (4:2:0: the thread of a block's top-left pixel writes the block's U and V bytes)
+template <typename T, int FMT>
 __global__ void __launch_bounds__(256) reconstruct_u8_kernel(const T* __restrict__ x, int xc, const float* __restrict__ lr, int h, int w,
                                                              int scale, int clamp01, int vec, uint8_t* __restrict__ out) {
   const int Ho = scale * h, Wo = scale * w;
+  constexpr bool YUV = is_yuv420<FMT>();
   x += (size_t)blockIdx.z * Ho * Wo * xc;
   lr += (size_t)blockIdx.z * 3 * h * w;
-  out += (size_t)blockIdx.z * 3 * Ho * Wo;
+  out += (size_t)blockIdx.z * (YUV ? 3 * (size_t)Ho * Wo / 2 : 3 * (size_t)Ho * Wo);
   const int p0 = (blockIdx.x * blockDim.x + threadIdx.x) * 16;
   if (p0 >= Ho * Wo) return;
   const int n = min(16, Ho * Wo - p0);
   const float inv = 1.0f / (float)scale;
-  uint32_t ob[12] = {};
+  uint32_t ob[run_words<FMT>()] = {};
 #pragma unroll
   for (int j = 0; j < 16; ++j) {
     if (j >= n) break;
     const int p = p0 + j;
     const int Y = p / Wo, X = p % Wo;
+    float v[3];
 #pragma unroll
-    for (int c = 0; c < 3; ++c) put_u8<BGR>(ob, j, c, reconstruct_at(x, xc, lr, h, w, Y, X, p, c, inv, clamp01));
+    for (int c = 0; c < 3; ++c) v[c] = reconstruct_at(x, xc, lr, h, w, Y, X, p, c, inv, clamp01);
+    if constexpr (YUV) {
+      const uint32_t R = frame_u8(v[0]), G = frame_u8(v[1]), B = frame_u8(v[2]);
+      ob[j >> 2] |= rgb8_y(R, G, B) << (8 * (j & 3));
+      if (Y % 2 == 0 && X % 2 == 0) {
+        uint8_t* c = out + (size_t)Ho * Wo;
+        const size_t iu = FMT == RV_FRAME_NV12 ? (size_t)(Y / 2) * Wo + X : (size_t)(Y / 2) * (Wo / 2) + X / 2;
+        c[iu] = (uint8_t)rgb8_u(R, G, B);
+        c[FMT == RV_FRAME_NV12 ? iu + 1 : iu + (size_t)Ho * Wo / 4] = (uint8_t)rgb8_v(R, G, B);
+      }
+    } else {
+      put_px<FMT>(ob, nullptr, j, false, v[0], v[1], v[2]);
+    }
   }
-  store_run(out + 3 * (size_t)p0, ob, 3 * n, vec);
+  if constexpr (YUV) store_run<16>(out + (size_t)p0, ob, n, vec);
+  else store_run<48>(out + 3 * (size_t)p0, ob, 3 * n, vec);
 }
 
 }  // namespace rv
@@ -1586,38 +1657,49 @@ extern "C" int rv_reconstruct(const void* x, int xc, int x_dtype, const float* l
   return rv_reconstruct_batched(x, xc, x_dtype, lr, h, w, scale, clamp01, out, 1, stream);
 }
 
+template <int FMT>
+static int launch_reconstruct_u8(RecPath path, const void* x, int xc, int x_dtype, const float* lr, int h, int w, int scale,
+                                  int clamp01, uint8_t* out, int nimg, cudaStream_t st) {
+  const bool aligned = (uintptr_t)out % 16 == 0;
+  if (path == RecPath::X4) {
+    const int vec = aligned && (4 * w) % 16 == 0;
+    const dim3 grid(cdiv((long long)h * ((w + 3) / 4), 128), 1, nimg);
+    reconstruct4_u8_kernel<FMT><<<grid, 128, 0, st>>>((const float4*)x, lr, h, w, clamp01, vec, out);
+  } else if (path == RecPath::X2) {
+    const int vec = aligned && (2 * w) % 16 == 0;
+    const dim3 grid(cdiv((long long)h * ((w + 7) / 8), 128), 1, nimg);
+    reconstruct2_u8_kernel<FMT><<<grid, 128, 0, st>>>((const float4*)x, lr, h, w, clamp01, vec, out);
+  } else {
+    const long long n = (long long)scale * h * scale * w;
+    const int vec = aligned && (is_yuv420<FMT>() ? 3 * n / 2 : 3 * n) % 16 == 0;
+    const dim3 grid(cdiv(cdiv(n, 16), 256), 1, nimg);
+    RV_DISPATCH_DTYPE(x_dtype, T, (reconstruct_u8_kernel<T, FMT><<<grid, 256, 0, st>>>((const T*)x, xc, lr, h, w, scale, clamp01, vec, out)));
+  }
+  return RV_OK;
+}
+
 extern "C" int rv_reconstruct_u8_batched(const void* x, int xc, int x_dtype, const float* lr, int h, int w, int scale, int clamp01,
-                                         int bgr, uint8_t* out, int nimg, void* stream) {
+                                         int fmt, uint8_t* out, int nimg, void* stream) {
   RV_REQUIRE(x && lr && out && h > 0 && w > 0 && xc >= 3 && (scale == 2 || scale == 4),
              "rv_reconstruct_u8: bad arguments");
+  RV_REQUIRE(fmt >= RV_FRAME_RGB && fmt <= RV_FRAME_NV12, "rv_reconstruct_u8: unknown frame format %d", fmt);
   RV_REQUIRE(nimg >= 1 && nimg <= 65535, "rv_reconstruct_u8: n=%d images out of range", nimg);
   RV_REQUIRE((long long)scale * h * scale * w <= (1ll << 30), "rv_reconstruct_u8: %d x %d output too large", scale * h, scale * w);
   const RecPath path = reconstruct_path(x, xc, x_dtype, scale);
-  const bool aligned = (uintptr_t)out % 16 == 0;
-  const int Wo = scale * w;
   cudaStream_t st = (cudaStream_t)stream;
-  if (path == RecPath::X4) {
-    const int vec = aligned && (3 * Wo) % 16 == 0;
-    const dim3 grid(cdiv((long long)h * ((w + 3) / 4), 128), 1, nimg);
-    if (bgr) reconstruct4_u8_kernel<true><<<grid, 128, 0, st>>>((const float4*)x, lr, h, w, clamp01, vec, out);
-    else reconstruct4_u8_kernel<false><<<grid, 128, 0, st>>>((const float4*)x, lr, h, w, clamp01, vec, out);
-  } else if (path == RecPath::X2) {
-    const int vec = aligned && (3 * Wo) % 16 == 0;
-    const dim3 grid(cdiv((long long)h * ((w + 7) / 8), 128), 1, nimg);
-    if (bgr) reconstruct2_u8_kernel<true><<<grid, 128, 0, st>>>((const float4*)x, lr, h, w, clamp01, vec, out);
-    else reconstruct2_u8_kernel<false><<<grid, 128, 0, st>>>((const float4*)x, lr, h, w, clamp01, vec, out);
-  } else {
-    const long long n = (long long)scale * h * Wo;
-    const int vec = aligned && (3 * n) % 16 == 0;
-    const dim3 grid(cdiv(cdiv(n, 16), 256), 1, nimg);
-    RV_DISPATCH_DTYPE(x_dtype, T, (bgr ? reconstruct_u8_kernel<T, true><<<grid, 256, 0, st>>>((const T*)x, xc, lr, h, w, scale, clamp01, vec, out)
-                                       : reconstruct_u8_kernel<T, false><<<grid, 256, 0, st>>>((const T*)x, xc, lr, h, w, scale, clamp01, vec, out)));
+  int rc;
+  switch (fmt) {
+    case RV_FRAME_RGB: rc = launch_reconstruct_u8<RV_FRAME_RGB>(path, x, xc, x_dtype, lr, h, w, scale, clamp01, out, nimg, st); break;
+    case RV_FRAME_BGR: rc = launch_reconstruct_u8<RV_FRAME_BGR>(path, x, xc, x_dtype, lr, h, w, scale, clamp01, out, nimg, st); break;
+    case RV_FRAME_I420: rc = launch_reconstruct_u8<RV_FRAME_I420>(path, x, xc, x_dtype, lr, h, w, scale, clamp01, out, nimg, st); break;
+    default: rc = launch_reconstruct_u8<RV_FRAME_NV12>(path, x, xc, x_dtype, lr, h, w, scale, clamp01, out, nimg, st); break;
   }
+  if (rc != RV_OK) return rc;
   RV_LAUNCH_CHECK("reconstruct_u8");
   return RV_OK;
 }
 
-extern "C" int rv_reconstruct_u8(const void* x, int xc, int x_dtype, const float* lr, int h, int w, int scale, int clamp01, int bgr,
+extern "C" int rv_reconstruct_u8(const void* x, int xc, int x_dtype, const float* lr, int h, int w, int scale, int clamp01, int fmt,
                                  uint8_t* out, void* stream) {
-  return rv_reconstruct_u8_batched(x, xc, x_dtype, lr, h, w, scale, clamp01, bgr, out, 1, stream);
+  return rv_reconstruct_u8_batched(x, xc, x_dtype, lr, h, w, scale, clamp01, fmt, out, 1, stream);
 }

@@ -16,8 +16,18 @@ LIB_PATH = os.path.join(_HERE, 'librefvsr_b200.so')
 RV_F32, RV_F16, RV_BF16 = 0, 1, 2
 ACT_NONE, ACT_RELU, ACT_LRELU01, ACT_LRELU02, ACT_CLAMP3 = 0, 1, 2, 3, 4
 IMPL_SIMT, IMPL_TC = 0, 1
+# 8-bit frame formats (RV_FRAME_*): RGB and BGR are HWC bytes (False / True are accepted for them), I420 and NV12 are YUV 4:2:0
+FRAME_RGB, FRAME_BGR, FRAME_I420, FRAME_NV12 = 0, 1, 2, 3
 
 DTYPE_CODE = {torch.float32: RV_F32, torch.float16: RV_F16, torch.bfloat16: RV_BF16}
+
+
+def frame_shape(h, w, fmt):
+    """the uint8 shape of one (h, w) frame of format fmt: (h, w, 3) HWC bytes, or the (3h/2, w) array cv2 uses for 4:2:0"""
+    if fmt in (FRAME_I420, FRAME_NV12):
+        return (3 * h // 2, w)
+    assert fmt in (FRAME_RGB, FRAME_BGR), f'unknown frame format {fmt!r}'
+    return (h, w, 3)
 
 
 class rv_conv_desc(C.Structure):
@@ -414,35 +424,38 @@ class CudaOps:
                                                          lr.shape[3], scale, int(clamp01), _ptr(out), lr.shape[0],
                                                          self._stream()), 'rv_reconstruct')
 
-    def reconstruct_u8(self, x, lr, scale, clamp01, out, bgr):
-        """reconstruct() with 8-bit HWC output: out (scale*h, scale*w, 3) uint8, or (n, scale*h, scale*w, 3) for a batch, gets the
-        bytes frame_u8 makes of the values reconstruct() would write (rv_reconstruct_u8); bgr: B, G, R byte order"""
+    def reconstruct_u8(self, x, lr, scale, clamp01, out, fmt):
+        """reconstruct() with 8-bit output: out, one (scale*h, scale*w) frame of format fmt or (n, ...) of them for a batch, gets
+        the bytes frame_u8 makes of the values reconstruct() would write (rv_reconstruct_u8).  fmt: False / 0 RGB and True / 1 BGR
+        (out (..., H, W, 3)), FRAME_I420 / FRAME_NV12 (out (..., 3H/2, W), the 4:2:0 frame of those RGB bytes)"""
         _chk_dev(x, lr, out)
-        assert out.dtype == torch.uint8 and out.shape[-1] == 3
+        H, W = scale * lr.shape[-2], scale * lr.shape[-1]
+        assert out.dtype == torch.uint8 and tuple(out.shape[-len(frame_shape(H, W, fmt)):]) == frame_shape(H, W, fmt)
         if lr.dim() == 3:                          # one image: a batch of 1
             x, lr, out = x[None], lr[None], out[None]
         assert x.shape[0] == out.shape[0] == lr.shape[0]  # a batch of n images: (n, ...) operands, one launch
         _check(self.lib, self.lib.rv_reconstruct_u8_batched(_ptr(x), x.shape[3], DTYPE_CODE[x.dtype], _ptr(lr), lr.shape[2],
-                                                            lr.shape[3], scale, int(clamp01), int(bool(bgr)), _ptr(out),
+                                                            lr.shape[3], scale, int(clamp01), int(fmt), _ptr(out),
                                                             lr.shape[0], self._stream()), 'rv_reconstruct_u8')
 
     # -- 8-bit frames -----------------------------------------------------------------------------
-    def frames_from_u8(self, srcs, dsts, bgr):
-        """srcs: contiguous uint8 (h, w, 3) frames (HWC; bgr: B, G, R byte order), dsts: as many contiguous float32 (3, h, w) frames,
-        all of one size on one device; dsts[i] = srcs[i] as RGB planes of fl32(u / 255) (rv_frames_from_u8, 16 frames per launch)"""
+    def frames_from_u8(self, srcs, dsts, fmt):
+        """srcs: contiguous uint8 (h, w) frames of format fmt (see reconstruct_u8), dsts: as many contiguous float32 (3, h, w)
+        frames, all of one size on one device; dsts[i] = the RGB planes of fl32(u / 255) of srcs[i]'s R, G, B bytes
+        (rv_frames_from_u8, 16 frames per launch)"""
         assert len(srcs) == len(dsts)
         if not srcs:
             return
-        h, w = srcs[0].shape[0], srcs[0].shape[1]
+        h, w = dsts[0].shape[1], dsts[0].shape[2]
         for s, d in zip(srcs, dsts):
             _chk_dev(s, d)
-            assert s.dtype == torch.uint8 and tuple(s.shape) == (h, w, 3), f'frames_from_u8: source {tuple(s.shape)} {s.dtype}'
+            assert s.dtype == torch.uint8 and tuple(s.shape) == frame_shape(h, w, fmt), f'frames_from_u8: source {tuple(s.shape)} {s.dtype}'
             assert d.dtype == torch.float32 and tuple(d.shape) == (3, h, w), f'frames_from_u8: destination {tuple(d.shape)} {d.dtype}'
         for i in range(0, len(srcs), 16):
             ps = [s.data_ptr() for s in srcs[i:i + 16]]
             pd = [d.data_ptr() for d in dsts[i:i + 16]]
             _check(self.lib, self.lib.rv_frames_from_u8((C.c_void_p * len(ps))(*ps), (C.c_void_p * len(pd))(*pd), len(ps), h, w,
-                                                        int(bool(bgr)), self._stream()), 'rv_frames_from_u8')
+                                                        int(fmt), self._stream()), 'rv_frames_from_u8')
 
     # -- evaluation metrics -----------------------------------------------------------------------
     def region_metrics(self, a, b, boxes):

@@ -30,7 +30,7 @@ import torch
 import torch.nn as nn
 
 from . import packing
-from .lib import (ACT_CLAMP3, ACT_LRELU01, ACT_LRELU02, ACT_NONE, ACT_RELU)
+from .lib import (ACT_CLAMP3, ACT_LRELU01, ACT_LRELU02, ACT_NONE, ACT_RELU, FRAME_I420, FRAME_NV12, frame_shape)
 from .modules import build_parameter_tree
 
 _PREC = {'fp32': torch.float32, 'fp16': torch.float16, 'bf16': torch.bfloat16}
@@ -147,7 +147,8 @@ class Network(nn.Module):
         self._b = 0
         self._bn = 1                  # windows of the current call: ring slots and carried state are [bn][...] tensors
         self._bmode = False           # enqueueing the batched steps of a call: every scratch buffer has the batch dimension
-        self._u8 = None               # inside an 8-bit call (forward_u8 / push_frame_u8 / push_frames_u8): its bgr flag
+        self._u8 = None               # inside an 8-bit call: its frame format, the bgr flag of forward_u8 / push_frame_u8 /
+        #                               push_frames_u8 (False / True) or FRAME_I420 / FRAME_NV12 of the *_yuv420 entries
         self.executed_kernels = 0     # kernels of librefvsr_b200.so actually executed (eager launches + graph nodes)
         self.register_load_state_dict_post_hook(lambda module, incompatible: module._invalidate())
 
@@ -581,8 +582,8 @@ class Network(nn.Module):
             hr = dec                                             # x2: no upsample2 (RefVSR.py:89-90,114-115)
         hr2 = self._conv('conv_hr', hr, None, self._buf('up.hr2', (s * h, s * w, C), dt), [(C, C)], act_pre=ACT_LRELU01)
         last = self._conv('conv_last', hr2, None, self._buf('up.last', (s * h, s * w, 4), torch.float32), [(C, C)])
-        if self._u8 is not None:                                 # the same values, written as 8-bit HWC bytes
-            out = self._buf('up.out8', (s * h, s * w, 3), torch.uint8)
+        if self._u8 is not None:                                 # the same values, written as 8-bit frames
+            out = self._buf('up.out8', frame_shape(s * h, s * w, self._u8), torch.uint8)
             self.ops.reconstruct_u8(last, lr_center, s, clamp01, out, self._u8)
             return out
         out = self._buf('up.out', (3, s * h, s * w), torch.float32)
@@ -798,7 +799,8 @@ class Network(nn.Module):
         """push_frame for all n windows of the running batch at once: lrs (n, 3, h, w), refs (n, 3, hr, wr), element b being
         the frame entering window b.  The same contract per element as push_frame; returns what forward()['result'] would,
         (n, 3, scale*h, scale*w), computed by one batched window schedule like forward()."""
-        if lrs.dim() != 4 or refs.dim() != 4 or lrs.size(0) != refs.size(0):
+        fdims = 3 if self._u8 is None else len(frame_shape(2, 2, self._u8))     # the dimensions of one frame
+        if lrs.dim() != fdims + 1 or refs.dim() != fdims + 1 or lrs.size(0) != refs.size(0):
             raise ValueError('push_frames takes LR frames (n, 3, h, w) and Ref frames (n, 3, hr, wr)')
         n = lrs.size(0)
         if n != self._bn:
@@ -839,22 +841,69 @@ class Network(nn.Module):
         if tuple(refs.shape[:2]) != (n, t):
             raise ValueError(f'forward_u8: lrs {tuple(lrs.shape)} and refs {tuple(refs.shape)} differ in (n, t)')
         self._check_sizes(h, w, refs.shape[2], refs.shape[3])
-        with self._frames_u8(bgr):
+        with self._frames_u8(bool(bgr)):
             return self._call(lrs, refs, n, is_first_frame, False, False)[0]
 
     def push_frame_u8(self, lr, ref, bgr=False, b=0):
         """push_frame() for 8-bit frames: lr (h, w, 3), ref (hr, wr, 3) contiguous uint8 -> (scale*h, scale*w, 3) uint8"""
         self._check_u8('push_frame_u8', 'lr', lr, 3)
         self._check_u8('push_frame_u8', 'ref', ref, 3)
-        with self._frames_u8(bgr):
+        with self._frames_u8(bool(bgr)):
             return self.push_frame(lr, ref, b)
 
     def push_frames_u8(self, lrs, refs, bgr=False):
         """push_frames() for 8-bit frames: lrs (n, h, w, 3), refs (n, hr, wr, 3) contiguous uint8 -> (n, scale*h, scale*w, 3) uint8"""
         self._check_u8('push_frames_u8', 'lrs', lrs, 4)
         self._check_u8('push_frames_u8', 'refs', refs, 4)
-        with self._frames_u8(bgr):
+        with self._frames_u8(bool(bgr)):
             return self.push_frames(lrs, refs)
+
+    # ---- YUV 4:2:0 frames (no counterpart in the reference) ------------------------------------------
+    # Video decoders and encoders mostly work in 4:2:0: ffmpeg's yuv420p is I420, hardware codecs use NV12.  These entries take and
+    # return such frames as the (3h/2, w) uint8 arrays cv2 uses, converted on the GPU at the same two points as the 8-bit entries:
+    # rv_frames_from_u8 turns an entering frame into the fp32 values of the RGB bytes cv2.cvtColor(COLOR_YUV2RGB_I420 / _NV12)
+    # gives, and rv_reconstruct_u8 writes cv2.cvtColor(COLOR_RGB2YUV_I420) of the RGB bytes forward_u8 returns (interleaved for
+    # NV12).  Everything else is forward_u8's: schedule, stream state, ring; fp32, 8-bit and 4:2:0 calls may be interleaved.
+
+    def forward_yuv420(self, lrs, refs, is_first_frame, nv12=False):
+        """forward() for 4:2:0 frames: lrs (n, t, 3h/2, w), refs (n, t, 3hr/2, wr), contiguous uint8 on the engine's device, I420
+        (Y plane, U plane, V plane) or with nv12 NV12 (Y plane, interleaved U, V rows), LR and Ref alike.  -> (n, 3H/2, W) uint8
+        frames of the same layout, (H, W) = (scale*h, scale*w): the 4:2:0 frames of forward_u8's RGB result for the RGB frames
+        cv2 makes of lrs / refs."""
+        self._check_yuv420('forward_yuv420', 'lrs', lrs, 4)
+        self._check_yuv420('forward_yuv420', 'refs', refs, 4)
+        n, t = lrs.shape[:2]
+        if tuple(refs.shape[:2]) != (n, t):
+            raise ValueError(f'forward_yuv420: lrs {tuple(lrs.shape)} and refs {tuple(refs.shape)} differ in (n, t)')
+        self._check_sizes(2 * lrs.shape[2] // 3, lrs.shape[3], 2 * refs.shape[2] // 3, refs.shape[3])
+        with self._frames_u8(FRAME_NV12 if nv12 else FRAME_I420):
+            return self._call(lrs, refs, n, is_first_frame, False, False)[0]
+
+    def push_frame_yuv420(self, lr, ref, nv12=False, b=0):
+        """push_frame() for 4:2:0 frames: lr (3h/2, w), ref (3hr/2, wr) contiguous uint8 -> (3H/2, W) uint8"""
+        self._check_yuv420('push_frame_yuv420', 'lr', lr, 2)
+        self._check_yuv420('push_frame_yuv420', 'ref', ref, 2)
+        with self._frames_u8(FRAME_NV12 if nv12 else FRAME_I420):
+            return self.push_frame(lr, ref, b)
+
+    def push_frames_yuv420(self, lrs, refs, nv12=False):
+        """push_frames() for 4:2:0 frames: lrs (n, 3h/2, w), refs (n, 3hr/2, wr) contiguous uint8 -> (n, 3H/2, W) uint8"""
+        self._check_yuv420('push_frames_yuv420', 'lrs', lrs, 3)
+        self._check_yuv420('push_frames_yuv420', 'refs', refs, 3)
+        with self._frames_u8(FRAME_NV12 if nv12 else FRAME_I420):
+            return self.push_frames(lrs, refs)
+
+    def _check_yuv420(self, fn, name, x, dims):
+        if not isinstance(x, torch.Tensor) or x.dtype != torch.uint8:
+            raise ValueError(f'{fn}: {name} must be a uint8 tensor, got {getattr(x, "dtype", type(x).__name__)}')
+        if x.dim() != dims or x.shape[-2] % 3 or x.shape[-2] == 0 or x.shape[-1] % 2 or x.shape[-1] == 0:
+            raise ValueError(f'{fn}: {name} must be {dims}-d 4:2:0 frames of (3h/2, w) rows and columns, h and w even, '
+                             f'got {tuple(x.shape)}')
+        if not x.is_contiguous():
+            raise ValueError(f'{fn}: {name} must be contiguous')
+        dev = next(self.parameters()).device
+        if x.device != dev:
+            raise ValueError(f'{fn}: {name} is on {x.device}, the engine on {dev}')
 
     def _check_u8(self, fn, name, x, dims):
         if not isinstance(x, torch.Tensor) or x.dtype != torch.uint8:
@@ -868,16 +917,21 @@ class Network(nn.Module):
             raise ValueError(f'{fn}: {name} is on {x.device}, the engine on {dev}')
 
     @contextlib.contextmanager
-    def _frames_u8(self, bgr):
-        self._u8 = bool(bgr)
+    def _frames_u8(self, fmt):
+        self._u8 = fmt
         try:
             yield
         finally:
             self._u8 = None
 
     def _hw(self, x):
-        """(h, w) of a frame or a stack of frames: (..., 3, h, w) fp32, or (..., h, w, 3) uint8 inside an 8-bit call"""
-        return tuple(x.shape[-2:]) if self._u8 is None else tuple(x.shape[-3:-1])
+        """(h, w) of a frame or a stack of frames: (..., 3, h, w) fp32, or inside an 8-bit call (..., h, w, 3) uint8 HWC or
+        (..., 3h/2, w) uint8 4:2:0"""
+        if self._u8 is None:
+            return tuple(x.shape[-2:])
+        if self._u8 in (FRAME_I420, FRAME_NV12):
+            return (2 * x.shape[-2] // 3, x.shape[-1])
+        return tuple(x.shape[-3:-1])
 
     def _is_fresh(self, b, lrs, refs, caller_first, is_train):
         """(state, fresh, shape) of batch element b's stream: fresh = its cached per-frame products cannot be reused"""
@@ -1052,7 +1106,10 @@ class Network(nn.Module):
         returns the int32 device flag (non-zero = the window did NOT slide by one)."""
         flag = self._buf(f'reuse.flag{self._b}', (1,), torch.int32)
         a1 = st['a0'] + 1
-        if self._u8 is not None:          # 8-bit frames: their fp32 values (the conversion is one to one, so equal bytes <=> equal values)
+        # 8-bit frames: compare their fp32 values.  For RGB / BGR bytes the conversion is one to one, so equal values <=> equal
+        # bytes; the YUV -> RGB map of 4:2:0 frames is not (Y bytes below 16 and saturated channels give
+        # equal RGB bytes for different frames), and equal values are what reuse needs, so comparing bytes would refuse some windows that can be reused.
+        if self._u8 is not None:
             lr32 = self._buf(f'reuse.lr32.{self._b}', (t - 1, 3, h, w), torch.float32)
             rf32 = self._buf(f'reuse.ref32.{self._b}', (t - 1, 3, hr, wr), torch.float32)
             self.ops.frames_from_u8([lrs[j] for j in range(t - 1)], [lr32[j] for j in range(t - 1)], self._u8)

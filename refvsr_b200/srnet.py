@@ -76,3 +76,17 @@ class SRNet(nn.Module):
     def push_frames_u8(self, lrs, refs, bgr=False):
         """push_frames() for 8-bit frames: lrs (n, h, w, 3), refs (n, hr, wr, 3) uint8 -> (n, scale*h, scale*w, 3) uint8"""
         return self.Network.push_frames_u8(lrs, refs, bgr=bgr)
+
+    def forward_yuv420(self, lrs, refs, is_first_frame=True, nv12=False):
+        """forward() for decoded 4:2:0 video: lrs (n, t, 3h/2, w), refs (n, t, 3hr/2, wr) contiguous uint8 I420 frames (nv12:
+        NV12) on the engine's device -> (n, 3H/2, W) uint8 frames of the same layout, the 4:2:0 frames of forward_u8's RGB
+        result for the RGB frames cv2.cvtColor makes of the inputs; see Network.forward_yuv420 (no counterpart in the reference)"""
+        return self.Network.forward_yuv420(lrs, refs, is_first_frame, nv12=nv12)
+
+    def push_frame_yuv420(self, lr, ref, nv12=False):
+        """push_frame() for 4:2:0 frames: lr (3h/2, w), ref (3hr/2, wr) uint8 -> (3H/2, W) uint8"""
+        return self.Network.push_frame_yuv420(lr, ref, nv12=nv12)
+
+    def push_frames_yuv420(self, lrs, refs, nv12=False):
+        """push_frames() for 4:2:0 frames: lrs (n, 3h/2, w), refs (n, 3hr/2, wr) uint8 -> (n, 3H/2, W) uint8"""
+        return self.Network.push_frames_yuv420(lrs, refs, nv12=nv12)
