@@ -17,6 +17,7 @@ Without a GPU: the bound's self-tests, and the list of convolutions below agains
 geometry the two schedules run it at, and each launch-plan branch of the tensor-core kernel at full-size maps."""
 import collections
 import ctypes as C
+import functools
 import zlib
 
 import pytest
@@ -118,9 +119,10 @@ def _nhwc(t):
     return t[0].permute(1, 2, 0)
 
 
-def reference(sig, ops):
+def reference(sig, ops, k_acc=None):
     """float64 (ref, base) in the output's NHWC layout: ref = the conv, then the epilogue in the kernel's order, then the
-    pixel shuffle; base = C_ACC K u A max(1, |gate|) + 2u |ref|, the bound without the output type's ulp"""
+    pixel shuffle; base = C_ACC K u A max(1, |gate|) + 2u |ref|, the bound without the output type's ulp.  k_acc: the
+    number of products that can round in the accumulation, if fewer than K (weights that are exact zeros add nothing)"""
     x = torch.cat([t[..., :r] for t, (r, _) in zip(ops['xs'], sig.srcs)], 2).double()
     w, b = ops['w'].double(), ops['b'].double()
     y = F.conv2d(_nchw(x), w, b, stride=sig.stride, padding=sig.pad)
@@ -136,7 +138,7 @@ def reference(sig, ops):
     if sig.ps:
         y, a = F.pixel_shuffle(y, 2), F.pixel_shuffle(a, 2)
     y, a = _nhwc(y), _nhwc(a)
-    K = sig.k * sig.k * sum(r for r, _ in sig.srcs)
+    K = k_acc or sig.k * sig.k * sum(r for r, _ in sig.srcs)
     return y, C_ACC * K * U * a + 2 * U * y.abs()
 
 
@@ -308,17 +310,37 @@ def _signature(layer, src0, out, gate, res, act_pre, act_post, pixel_shuffle):
                bool(pixel_shuffle), 'f32' if out.dtype == torch.float32 else 'act', out.shape[2])
 
 
-def _recording_ops(compute):
+@functools.lru_cache(maxsize=None)
+def kernel_of(weight_shape, srcs, stride, pad, act_dtype, prefer_tc):
+    """the conv kernel the engine's packing picks for a layer: 'tc' (conv_tc.cu) or 'simt' (conv_simt.cu), from
+    packing.pack_conv_uncached on zero weights on the CPU"""
+    w = torch.zeros(weight_shape)
+    pc = packing.pack_conv_uncached('kernel_of', w, torch.zeros(weight_shape[0]), [tuple(s) for s in srcs], stride, pad,
+                                    act_dtype, 'cpu', prefer_tc)
+    return 'tc' if pc.impl == IMPL_TC else 'simt'
+
+
+def _recording_ops(compute, kernels=False):
     """OracleOps whose conv2d records (signature, input H, W) of every call; compute=False: every other operator (and the conv
-    itself) is a no-op, so that a full-size schedule runs on the CPU in a second"""
+    itself) is a no-op, so that a full-size schedule runs on the CPU in a second.  kernels=True: the record is (signature,
+    kernel, precision class, input H, W), with the kernel of kernel_of and the class '16' (bf16 / fp16 activations) or '32'"""
     from oracle.oracle_ops import OracleOps
 
     class Recording(OracleOps):
         def __init__(self):
             self.seen = collections.Counter()
 
+        def pack_conv(self, name, weight, bias, srcs, stride, pad, act_dtype, device, prefer_tc, bias_add=0.0):
+            layer = super().pack_conv(name, weight, bias, srcs, stride, pad, act_dtype, device, prefer_tc, bias_add)
+            if kernels:
+                layer.kernel = kernel_of(tuple(weight.shape), tuple(tuple(s) for s in srcs), stride, pad, act_dtype,
+                                         bool(prefer_tc))
+                layer.prec = '32' if act_dtype == torch.float32 else '16'
+            return layer
+
         def conv2d(self, layer, src0, src1, out, gate=None, res=None, act_pre=0, act_post=0, pixel_shuffle=False):
-            self.seen[(_signature(layer, src0, out, gate, res, act_pre, act_post, pixel_shuffle), tuple(src0.shape[:2]))] += 1
+            sig = _signature(layer, src0, out, gate, res, act_pre, act_post, pixel_shuffle)
+            self.seen[(sig, layer.kernel, layer.prec, tuple(src0.shape[:2])) if kernels else (sig, tuple(src0.shape[:2]))] += 1
             if compute:
                 super().conv2d(layer, src0, src1, out, gate, res, act_pre, act_post, pixel_shuffle)
 
